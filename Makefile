@@ -4,13 +4,13 @@ GPUS ?= 1
 
 .PHONY: build test test-gpu sanitize model-test bench bench-cpu clean
 
-build:            ## both native libraries, in-tree (nvcc cross-compiles sm_100a without a GPU)
+build:            ## both native libraries, in-tree (nvcc cross-compiles sm_90a without a GPU)
 	$(PY) -c "import __graft_entry__ as g; g.build()"
 
 test: build       ## everything that runs without a GPU (multi-process paths on gloo)
 	$(PY) -m pytest tests/ -x -q -m "not gpu"
 
-test-gpu: build   ## needs a B200
+test-gpu: build   ## needs an H100
 	$(PY) -m pytest tests/ -x -q -m gpu
 
 sanitize:         ## TSAN / ASAN / UBSAN builds of the host runtime + fuzzers

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Headline benchmark: DLRM training samples/sec on N B200 GPUs of one node (BASELINE.json).
+"""Headline benchmark: DLRM training samples/sec on N H100 GPUs of one node (BASELINE.json).
 
   python bench.py --gpus 1 --steps 20 --warmup 5
+  python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs /tmp/out     # + what the last timed step computed, as .npy files
   python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29500 \
          bench.py --gpus 8 --steps 20 --warmup 5
 
@@ -58,12 +59,16 @@ def parse_args():
     ap.add_argument("--no-overlap", action="store_true")
     ap.add_argument("--gemm-v1", action="store_true")
     ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's results (probabilities, loss, updated dense parameters, "
+                         "a seeded sample of the updated embedding rows) "
+                         "as float32 DIR/<name>.npy; the inputs depend only on the arguments, so two builds can be compared")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """SM clock / power / throttle reasons DURING the timed regions (B200_PROFILING.md recipe).  In-process NVML from a sampling thread
-    (a 20-step region lasts ~25 ms: `nvidia-smi -lms` does not even start within it); nvidia-smi is the fallback."""
+    """SM clock / power / throttle reasons DURING the timed regions.  In-process NVML from a sampling thread (a 20-step region lasts tens
+    of ms: `nvidia-smi -lms` does not even start within it); nvidia-smi is the fallback."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
     REASONS = ((0x8, "hw_slowdown"), (0x40, "hw_thermal_slowdown"), (0x20, "sw_thermal_slowdown"), (0x4, "sw_power_cap"), (0x80, "hw_power_brake"))
@@ -182,6 +187,29 @@ def unique_ratio(ids: torch.Tensor) -> float:
     return u / float(ids.numel())
 
 
+def dump_outputs(eng, out_dir: str, last_ids: torch.Tensor, rows_per_table: int = 256) -> None:
+    """What the timed path hands back after its last step: per-sample click probabilities, the loss, the updated dense parameters
+    (MLP weights / biases, BatchNorm statistics) and the embedding rows of a fixed, seeded sample of the last step's ids (what the sparse
+    update wrote), each as <out_dir>/<name>.npy -- float32, the sampled ids float64 (exact below 2^53); a few MB in all."""
+    import numpy as np
+    core = eng.eng if hasattr(eng, "eng") else eng
+    arrays = {"prob": core.prob, "loss": core.loss}
+    if hasattr(core, "state_dict"):
+        arrays.update(core.state_dict())
+    tables = getattr(core, "tables", None)
+    if tables:
+        g = torch.Generator().manual_seed(0)
+        pos = torch.randperm(last_ids.shape[1], generator=g)[:rows_per_table].to(last_ids.device)
+        for t, tb in sorted(tables.items()):
+            keys = last_ids[t, pos].contiguous()
+            arrays[f"emb_rows_t{t:02d}"] = tb.lookup(keys)
+            arrays[f"emb_ids_t{t:02d}"] = keys.double()
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach()
+        np.save(os.path.join(out_dir, name.replace("/", "__") + ".npy"), (t if t.dtype == torch.float64 else t.float()).cpu().numpy())
+
+
 def main():
     args = parse_args()
     if args.impl == "reference":
@@ -276,6 +304,8 @@ def main():
     launches = eng.launches - l0
     keys1 = total_keys()
     final_loss = eng.loss_value()           # mean over the GLOBAL batch of the last timed step (all-reduced)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, args.dump_outputs, dev_timed[(args.steps - 1) % len(dev_timed)][1])
 
     # ---- end-to-end region through the public API: smart_stage (producer thread -> packed pinned H2D on a copy stream, two
     #      batches ahead) -> load_batch -> train_step -> D2H of the loss, every step ------------------------------
@@ -328,7 +358,7 @@ def main():
                        "prefill_steps": args.prefill, "distinct_timed_batches": len(dev_timed),
                        "new_keys_per_step": (keys1 - keys0) / float(args.steps), "unique_ratio": uniq, "alpha": args.alpha,
                        "filter_freq": args.filter_freq,
-                       "l2": f"{len(dev_timed)} distinct resident batches ({len(dev_timed) * in_bytes / 1e6:.0f} MB) + multi-GB embedding tables > 126 MB L2; no flush",
+                       "l2": f"{len(dev_timed)} distinct resident batches ({len(dev_timed) * in_bytes / 1e6:.0f} MB) + multi-GB embedding tables > 50 MB L2; no flush",
                        "cuda_graph": bool(graph and hasattr(eng, "capture")), "final_loss": final_loss,
                        "host_cpus": f"{len(bound)} CPUs local to the GPU (NVML ideal set)" if bound else "unpinned"},
             "clocks": clocks,

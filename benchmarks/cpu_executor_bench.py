@@ -1,6 +1,6 @@
 """Small-batch latency of the CPU Processor's op-program interpreter under the three executor policies (normal / cost_model / inline).
 
-  python benchmarks/cpu_executor_bench.py [--threads 4] [--batches 1,8,32] >> profiles/cpu_executor_bench.jsonl
+  python benchmarks/cpu_executor_bench.py [--threads 4] [--batches 1,8,32] >> cpu_executor_bench.jsonl
 
 The cost-model executor helps where the program has independent branches (MMoE / PLE experts and towers, ESMM / DSSM towers) and the batch is
 too small for an op to use its own team."""

@@ -2,7 +2,7 @@
 """CPU Processor benchmark (the reference deploys its processor on CPU hosts): DLRM p50 / p99 latency and samples/s through the native CPU
 runtime's C ABI, for a few (sessions, client threads, batch) operating points.  Prints one JSON line per point.
 
-  python benchmarks/cpu_serving_bench.py [--out profiles/cpu_serving_bench.jsonl]
+  python benchmarks/cpu_serving_bench.py [--out cpu_serving_bench.jsonl]
 """
 import argparse
 import json

@@ -2,7 +2,7 @@
 """CPU stand-alone training throughput of every zoo model -- the one benchmark the reference PUBLISHES in samples/s
 (BASELINE.md section B: modelzoo/*/README.md, batch 2048, Alibaba ecs.g8i.4xlarge = 16 vCPU Xeon Platinum 8475B).
 
-  python benchmarks/cpu_zoo_bench.py [--models dlrm,deepfm,...] [--dtype fp32|bf16|both] [--out profiles/cpu_zoo_bench.json]
+  python benchmarks/cpu_zoo_bench.py [--models dlrm,deepfm,...] [--dtype fp32|bf16|both] [--out cpu_zoo_bench.json]
 
 Method: synthetic Criteo- / Taobao-shaped batches generated up front, W warm-up steps, then R repetitions of K timed steps (forward,
 backward, optimizer step incl. the sparse EmbeddingVariable apply); the BEST repetition is reported (the box is shared; the reference

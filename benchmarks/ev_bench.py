@@ -2,9 +2,9 @@
 """EmbeddingVariable storage-engine micro-benchmark (the reference's embedding_variable_performance_test.cc / _memory_test.cc):
 lookup (hit / miss), lookup-or-create through the optimizer apply (fresh keys / existing keys, with dedup), snapshot (save), eviction and
 resident memory per key on the host engine at N keys (default 10 M, the scale of the reference's large tests).  One JSON line per
-measurement; ``--out`` appends them to a file.  CPU only (the device table is measured by bench.py / profiles/ncu_summary.md).
+measurement; ``--out`` appends them to a file.  CPU only (the device table is measured by bench.py).
 
-  python benchmarks/ev_bench.py --keys 10000000 --dim 16 --batch 262144 --out profiles/cpu_ev_bench.jsonl
+  python benchmarks/ev_bench.py --keys 10000000 --dim 16 --batch 262144 --out cpu_ev_bench.jsonl
 """
 import argparse
 import json

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""A/B of the dense-path GEMM kernels at the flagship MLP shapes (CUDA events, L2 flushed between iterations, median of N):
-bf16 single-CTA (k_gemm_tn_v2) vs bf16 CTA pair (k_gemm_tn_2cta, cta_group::2) vs block-scaled fp8 (k_gemm_mxfp8_tn; quantisation of the
-activations timed separately).  One JSON line per shape.   python benchmarks/gemm_ab.py [--iters 30]"""
+"""A/B of the dense-path GEMM kernels at the flagship MLP shapes (CUDA events, L2 flushed between iterations, median of N): the streaming
+bf16 wgmma kernel vs its cluster-of-2 variant (B tile multicast, dr_cuda_set_gemm_2cta) vs its B-resident variant (dr_cuda_set_gemm_bres,
+K <= 512) vs block-scaled fp8 (dr_cuda_gemm_mxfp8_tn; quantisation of the activations timed separately).  One JSON line per shape.
+    python benchmarks/gemm_ab.py [--iters 30]"""
 import argparse
 import ctypes as C
 import json
@@ -21,6 +22,7 @@ def main():
     args = ap.parse_args()
     lib = _native.cuda()
     lib.dr_cuda_set_gemm_2cta.argtypes, lib.dr_cuda_set_gemm_2cta.restype = [C.c_int], C.c_int
+    lib.dr_cuda_set_gemm_bres.argtypes, lib.dr_cuda_set_gemm_bres.restype = [C.c_int], C.c_int
     p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
     s = lambda: C.c_void_p(torch.cuda.current_stream().cuda_stream)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
@@ -50,12 +52,17 @@ def main():
         lib.dr_cuda_set_gemm_2cta(1)
         t2 = timed(bf16)
         lib.dr_cuda_set_gemm_2cta(0)
+        tr = None
+        if K <= 512:
+            lib.dr_cuda_set_gemm_bres(1)
+            tr = timed(bf16)
+            lib.dr_cuda_set_gemm_bres(0)
         bq, sfb = mxfp8.quantize_mxfp8(B)
         aq, sfa = mxfp8.quantize_mxfp8(A)
         tq = timed(lambda: mxfp8.quantize_mxfp8(A))
         t8 = timed(lambda: mxfp8.mxfp8_gemm(aq, sfa, bq, sfb, N, bias, True))
         fl = 2.0 * M * N * K
-        print(json.dumps({"M": M, "N": N, "K": K, "bf16_1cta_us": round(t1, 1), "bf16_2cta_us": round(t2, 1), "mxfp8_gemm_us": round(t8, 1),
+        print(json.dumps({"M": M, "N": N, "K": K, "bf16_1cta_us": round(t1, 1), "bf16_2cta_us": round(t2, 1), "bf16_bres_us": round(tr, 1) if tr else None, "mxfp8_gemm_us": round(t8, 1),
                           "mxfp8_quantize_a_us": round(tq, 1), "bf16_1cta_tflops": round(fl / t1 * 1e-6, 1), "bf16_2cta_tflops": round(fl / t2 * 1e-6, 1),
                           "mxfp8_tflops": round(fl / t8 * 1e-6, 1)}), flush=True)
 

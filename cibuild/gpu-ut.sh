@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# GPU unit tests (needs a B200; multi-GPU parts need >= 2).  Mirrors the reference's cibuild/gpu-ut/*.sh shards.
+# GPU unit tests (needs an H100; multi-GPU parts need >= 2).  Mirrors the reference's cibuild/gpu-ut/*.sh shards.
 #   bash cibuild/gpu-ut.sh            # pytest -m gpu
 #   bash cibuild/gpu-ut.sh sanitize   # + compute-sanitizer memcheck / racecheck over the sparse pipeline and the flag protocol
 set -euo pipefail

@@ -1,10 +1,10 @@
-"""deeprec_b200 -- a Blackwell(B200)-native sparse-recommender training & serving engine with the
+"""deeprec_b200 -- a Hopper (H100)-native sparse-recommender training & serving engine with the
 capabilities of DeepRec (EmbeddingVariable, admission/eviction, multi-tier storage, GroupEmbedding,
 model-parallel embeddings + data-parallel dense, SmartStage, incremental checkpoint, SessionGroup serving).
 
 Layers (see DESIGN.md):
   csrc/host   C++17 host engine        (CPU EV, ckpt bundle, staging queue, work queue, serving C ABI)
-  csrc/cuda   sm_100a CUDA kernels     (hash table, fused lookup, sparse optimizers, tcgen05 MLP, P2P collectives)
+  csrc/cuda   sm_90a CUDA kernels     (hash table, fused lookup, sparse optimizers, wgmma MLP, P2P collectives)
   python      framework layer          (this package)
 """
 from .config import (CacheStrategy, CBFFilter, CheckpointOption, CounterFilter, EmbeddingVariableOption,

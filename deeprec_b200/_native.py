@@ -1,7 +1,7 @@
 """ctypes bindings to the two in-tree native libraries.
 
 ``host()``  -> libdeeprec_host.so  (C++17 host engine; always available, built on demand)
-``cuda()``  -> libdeeprec_cuda.so  (sm_100a kernels; REQUIRED on a GPU box: no silent
+``cuda()``  -> libdeeprec_cuda.so  (sm_90a kernels; REQUIRED on a GPU box: no silent
                                     eager/PyTorch fallback -- a missing library raises)
 """
 from __future__ import annotations
@@ -186,12 +186,12 @@ def on_device(t: torch.Tensor) -> bool:
 
 
 def cuda():
-    """The sm_100a kernel library.  Raises if it is missing (never falls back silently)."""
+    """The sm_90a kernel library.  Raises if it is missing (never falls back silently)."""
     global _CUDA
     if _EMU_DEPTH > 0:
         if not getattr(_EMU, "_sigs_bound", False):
             from . import _cuda_sigs
-            _cuda_sigs.bind(_EMU, missing_ok=True)          # entry points of the tcgen05 / NVLS translation units do not exist in the emulation
+            _cuda_sigs.bind(_EMU, missing_ok=True)          # entry points of the wgmma / NVLS translation units do not exist in the emulation
             _EMU._sigs_bound = True
         return _EMU
     if _CUDA is None:

@@ -1,8 +1,8 @@
-"""In-tree native build: g++ for the host engine, nvcc (sm_100a only) for the device engine.
+"""In-tree native build: g++ for the host engine, nvcc (sm_90a only) for the device engine.
 
 Both libraries are plain C-ABI shared objects loaded with ctypes (no torch headers, so a full
 rebuild takes seconds and cross-compiles on a box without a GPU).  The .so files land in
-``deeprec_b200/lib`` so they travel with the gpurun snapshot.
+``deeprec_b200/lib``, so the package imports straight from the source tree.
 """
 from __future__ import annotations
 
@@ -25,7 +25,7 @@ CUDA_SOURCES = [
     "cuda/dense_kernels.cu",
     "cuda/gemm_fp8.cu",
     "cuda/gemm_mxfp8.cu",
-    "cuda/gemm_tcgen05.cu",
+    "cuda/gemm_wgmma.cu",
     "cuda/interaction_kernels.cu",
     "cuda/comm_kernels.cu",
     "cuda/sparse_pipeline.cu",
@@ -33,7 +33,6 @@ CUDA_SOURCES = [
     "cuda/fused_interaction_gemm.cu",
     "cuda/tier_kernels.cu",
     "cuda/nvls.cu",
-    "cuda/runtime.cu",
     "cuda/program_kernels.cu",
     "cuda/sparse_utils.cu",
     "cuda/serving_runtime.cu",
@@ -43,7 +42,7 @@ CUDA_SOURCES = [
 ]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _stamp(srcs: list[str], flags: list[str]) -> str:
@@ -120,13 +119,13 @@ def build_cuda(force: bool = False, verbose_ptxas: bool = False) -> str:
 
 
 # ---- CUDA-on-CPU emulation build (csrc/cuda/emu/cuda_emu.h): the SIMT kernels compiled by g++, one host thread per CUDA thread -----------------
-# Sources without tcgen05 / TMA / mbarrier code.  The library exports the same dr_* C entry points as libdeeprec_cuda.so, taking host pointers.
+# Sources without wgmma / TMA / mbarrier code.  The library exports the same dr_* C entry points as libdeeprec_cuda.so, taking host pointers.
 EMU_SOURCES = [
     "cuda/table_kernels.cu",
     "cuda/embedding_kernels.cu",
     "cuda/optimizer_kernels.cu",
     "cuda/dense_kernels.cu",
-    "cuda/interaction_kernels.cu",      # SIMT variants only (the tcgen05 kernels are compiled out)
+    "cuda/interaction_kernels.cu",      # SIMT variants only (the tensor-core kernels are compiled out)
     "cuda/fused_ops.cu",
     "cuda/program_kernels.cu",
     "cuda/sparse_utils.cu",
@@ -136,7 +135,7 @@ EMU_SOURCES = [
     "cuda/comm_kernels.cu",
     "cuda/ag_embedding.cu",             # all-gather -> lookup -> reduce-scatter embedding (SOK DistributedEmbedding dataflow) over peer memory
     "cuda/tier_kernels.cu",             # multi-tier: miss list / histogram eviction kernels + the manager's background thread
-    "cuda/emu/emu_stubs.cu",            # host-loop stand-ins for the tcgen05 GEMM entry points
+    "cuda/emu/emu_stubs.cu",            # host-loop stand-ins for the wgmma GEMM entry points
 ]
 
 

@@ -16,7 +16,7 @@ import torch
 
 
 class StorageType(enum.IntEnum):
-    """storage_config.h:22-47 (tiers that make sense on a B200 box)."""
+    """storage_config.h:22-47 (tiers that make sense on an H100 box)."""
     DRAM = 0
     HBM = 1
     HBM_DRAM = 2

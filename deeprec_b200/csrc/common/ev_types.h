@@ -1,11 +1,11 @@
-// Shared POD types for the host (C++) and device (CUDA sm_100a) embedding engines.
+// Shared POD types for the host (C++) and device (CUDA sm_90a) embedding engines.
 //
 // Behavioural parity targets in the reference (DeepRec):
 //   EmbeddingConfig            tensorflow/core/framework/embedding/embedding_config.h:12-127
 //   FeatureDescriptor layout   tensorflow/core/framework/embedding/feature_descriptor_impl.h:212-304
 //   sparse apply math          tensorflow/core/kernels/training_ali_ops.cc:73-210,431,1203,1396,2298,2871,3016
 //
-// Layout decision (B200-first, not a translation): one row per admitted key,
+// Layout decision (GPU-first, not a translation): one row per admitted key,
 //   [ emb(dim) | slot0(dim) | ... | slotS-1(dim) | scalars(4) ]   (fp32, 16-byte aligned)
 // so one hash probe serves the variable and all of its optimizer slots; frequency /
 // version / row-index metadata live in SoA arrays indexed by the key's table position

@@ -154,7 +154,7 @@ __global__ void __launch_bounds__(256) k_ag_grad(const DrDeviceTable* __restrict
 
 inline int ag_grid(int64_t work_items) {
   int64_t b = (work_items + 255) / 256;
-  const int64_t cap = (int64_t)kNumSMs * sparse_blocks_per_sm();
+  const int64_t cap = (int64_t)num_sms() * sparse_blocks_per_sm();
   return (int)(b < 1 ? 1 : b > cap ? cap : b);
 }
 

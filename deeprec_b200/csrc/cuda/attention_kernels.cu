@@ -371,7 +371,7 @@ int dr_cuda_din_attention_fwd_w(const float* q, const float* k, const uint8_t* m
   if (L <= 0 || D <= 0 || H1 <= 0 || H2 <= 0 || bytes > 200 * 1024) return -1;
   DR_CUDA_CHECK(cudaFuncSetAttribute(k_din_attention_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
   const int per_sm = bytes <= 100 * 1024 ? 2 : 1;
-  const int grid = (int)(B < (int64_t)kNumSMs * per_sm ? B : (int64_t)kNumSMs * per_sm);
+  const int grid = (int)(B < (int64_t)num_sms() * per_sm ? B : (int64_t)num_sms() * per_sm);
   k_din_attention_fwd<<<grid, kThreads, bytes, s>>>(q, k, mask, B, p, W1, b1, W2, b2, w3, b3, out, weights_out);
   DR_LAUNCH_CHECK();
   return 0;
@@ -392,7 +392,7 @@ int dr_cuda_din_attention_bwd(const float* q, const float* k, const uint8_t* mas
   const size_t bytes = (size_t)DinBwdSmem(p, DinSmem(p).total).total * sizeof(float);
   if (L <= 0 || D <= 0 || H1 <= 0 || H2 <= 0 || bytes > 220 * 1024) return -1;
   DR_CUDA_CHECK(cudaFuncSetAttribute(k_din_attention_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  const int grid = (int)(B < (int64_t)kNumSMs ? B : (int64_t)kNumSMs);
+  const int grid = (int)(B < (int64_t)num_sms() ? B : (int64_t)num_sms());
   k_din_attention_bwd<<<grid, kThreads, bytes, s>>>(q, k, mask, gout, B, p, W1, b1, W2, b2, w3, b3, dq, dk, dW1, db1, dW2, db2, dw3, db3);
   DR_LAUNCH_CHECK();
   return 0;

@@ -68,7 +68,7 @@ __global__ void __launch_bounds__(256) k_allreduce_apply(DrPeers grad_peers, int
   }
 }
 
-inline int grid_for(int64_t n, int block, int max_blocks = kNumSMs * 8) {
+inline int grid_for(int64_t n, int block, int max_blocks = num_sms() * 8) {
   int64_t b = (n + block - 1) / block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -115,7 +115,7 @@ int dr_comm_barrier(const DrPeers* sig, uint32_t* epochs, int channel, int rank,
 int dr_comm_allreduce_apply(const DrPeers* grad_peers, int W, float* w, float* s0, float* s1, int64_t n, const DrOptHyper* hp_dev,
                             float* reduced_out, cudaStream_t s) {
   if (n % 4) return -2;
-  DR_PDL_LAUNCH((k_allreduce_apply), grid_for(n / 4, 256, kNumSMs * 4), 256, 0, s, *grad_peers, W, w, s0, s1, n / 4, hp_dev, reduced_out, DrSpSync{});
+  DR_PDL_LAUNCH((k_allreduce_apply), grid_for(n / 4, 256, num_sms() * 4), 256, 0, s, *grad_peers, W, w, s0, s1, n / 4, hp_dev, reduced_out, DrSpSync{});
   DR_LAUNCH_CHECK();
   return 0;
 }
@@ -123,7 +123,7 @@ int dr_comm_allreduce_apply(const DrPeers* grad_peers, int W, float* w, float* s
 int dr_comm_allreduce_apply_sync(const DrPeers* grad_peers, int W, float* w, float* s0, float* s1, int64_t n, const DrOptHyper* hp_dev,
                                  float* reduced_out, const DrSpSync* sync, cudaStream_t s) {
   if (n % 4) return -2;
-  DR_PDL_LAUNCH((k_allreduce_apply), grid_for(n / 4, 256, kNumSMs * 4), 256, 0, s, *grad_peers, W, w, s0, s1, n / 4, hp_dev, reduced_out, *sync);
+  DR_PDL_LAUNCH((k_allreduce_apply), grid_for(n / 4, 256, num_sms() * 4), 256, 0, s, *grad_peers, W, w, s0, s1, n / 4, hp_dev, reduced_out, *sync);
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -1,7 +1,11 @@
-// Common device helpers for the sm_100a kernel library: PTX wrappers (mbarrier, TMA, tcgen05,
-// system-scope acquire/release for NVLink peer signalling), small vector types, error macros.
+// Common device helpers for the sm_90a kernel library: PTX wrappers (mbarrier, TMA, system-scope acquire/release for NVLink
+// peer signalling), small vector types, error macros.  The warpgroup MMA wrappers are in wgmma.cuh.
 #pragma once
 #include <cstdlib>
+#include <map>
+#include <mutex>
+#include <thread>
+#include <tuple>
 #ifdef DR_CUDA_EMU
 #include "emu/cuda_emu.h"      // g++ build of the SIMT kernels: every CUDA thread is a host thread (CPU CI, ASAN / TSAN over kernel code)
 #else
@@ -54,10 +58,22 @@ inline cudaError_t dr_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block
 #endif
 
 
+// SM count of the current device (132 on an H100 SXM, 114 on an H100 PCIe, fewer in an SM-partitioned context): persistent kernels
+// size their grids from it.  Queried once per device.
 #ifdef DR_CUDA_EMU
-constexpr int kNumSMs = 2;      // emulated blocks run one after the other: the grid-stride kernels get small grids (any grid size must be correct)
+inline int num_sms() { return 2; }   // emulated blocks run one after the other: the grid-stride kernels get small grids (any grid size must be correct)
 #else
-constexpr int kNumSMs = 148;
+inline int num_sms() {
+  static int n[64] = {};
+  int d = 0;
+  cudaGetDevice(&d);
+  d &= 63;
+  if (n[d] == 0) {
+    int v = 0;
+    n[d] = (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d) == cudaSuccess && v > 0) ? v : 132;
+  }
+  return n[d];
+}
 #endif
 
 // cudaFuncSetAttribute is per DEVICE: a process that drives several GPUs (serving ProcessorGroup: one replica per GPU in one process)
@@ -67,8 +83,8 @@ struct DrPerDeviceOnce {
   bool& operator()() { int d = 0; cudaGetDevice(&d); return done[d & 63]; }
 };
 
-// Resident-block budget (per SM) of the sparse-path kernels.  They run on a side stream next to the tcgen05 GEMMs
-// (1 CTA/SM, ~200 KB smem, 192 threads): capping them leaves thread slots so both streams really overlap.
+// Resident-block budget (per SM) of the sparse-path kernels.  They run on a side stream next to the wgmma GEMMs
+// (1 CTA/SM, up to ~200 KB smem, 384 threads): capping them leaves thread slots so both streams really overlap.
 inline int& sparse_blocks_per_sm() { static int v = 16; return v; }
 constexpr int64_t kEmptyKey = INT64_MIN;
 constexpr int64_t kTombKey = INT64_MIN + 1;
@@ -113,13 +129,13 @@ __device__ __forceinline__ uint32_t ld_relaxed_sys(const uint32_t* p) {
 // streaming 16-byte accesses that do not pollute L1 (peer data is L2-bypassed anyway)
 // ---- programmatic dependent launch (PDL) -------------------------------------------------------------------------------
 // Kernels on the training-step path are launched with cudaLaunchAttributeProgrammaticStreamSerialization (dr_launch_pdl below):
-// the next kernel's CTAs may become resident and run their prologue (barrier init, TMEM alloc, descriptor prefetch, index
+// the next kernel's CTAs may become resident and run their prologue (barrier init, descriptor prefetch, index
 // math) while the previous kernel drains.  griddepcontrol.wait blocks until the predecessor grid has completed and its
 // memory is visible, so NOTHING that touches global memory may precede pdl_sync() in such a kernel.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-// An early trigger lets the dependent grid's CTAs become resident while the primary still runs; measured on the DLRM step this
-// steals SM slots from the primary (-4 %), so the trigger is left implicit (at grid completion) unless DEEPREC_PDL_EARLY is built in.
+// An early trigger lets the dependent grid's CTAs become resident while the primary still runs, which steals SM slots from
+// the primary, so the trigger is left implicit (at grid completion) unless DEEPREC_PDL_EARLY is built in.
 #ifdef DEEPREC_PDL_EARLY
 __device__ __forceinline__ void pdl_sync() { pdl_wait(); pdl_trigger(); }
 #else
@@ -188,52 +204,6 @@ __device__ __forceinline__ void tma_store_2d(const void* desc, const void* smem_
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- tcgen05 (5th-gen tensor cores, TMEM) ---------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns (thread t gets lane base+t)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 #endif  // DR_CUDA_EMU
 
 // volatile scalar loads of words that other threads update with atomics (probe-then-CAS): plain volatile on the device; relaxed atomic
@@ -274,21 +244,48 @@ __device__ __forceinline__ int32_t ld_volatile_i32(const int32_t* p) { return *r
 #define DR_LD_V2_VOLATILE_U32(v, p) asm volatile("ld.volatile.global.v2.u32 {%0,%1}, [%2];" : "=r"((v).x), "=r"((v).y) : "l"(p) : "memory")
 #endif
 
-// UMMA shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
+// ---- deterministic reductions ---------------------------------------------------------------------------------------
+// Sums over the batch are never accumulated with floating-point atomics across blocks (their order, and so the rounding, would change
+// from run to run): every block writes its partial to a workspace and k_det_colsum adds the partials in block order.
+// A workspace belongs to one (device, host thread, call site): the producer kernel and its k_det_colsum are two launches, so callers
+// on other host threads (serving sessions, ranks of one process) never share one and cannot interleave on it.  Not keyed by stream:
+// a CUDA-graph capture runs on its own stream and must reuse the buffer the eager step before it sized (it grows only outside
+// capture).  One host thread must not run the same call site on two streams concurrently.  An old buffer is never freed, since
+// kernels still in flight may read it.
+inline float* dr_workspace(int slot, size_t nfloat, cudaStream_t s) {
+  struct Ws { float* p = nullptr; size_t cap = 0; };
+  static std::mutex mu;
+  static std::map<std::tuple<int, std::thread::id, int>, Ws> pool;
+  std::lock_guard<std::mutex> lk(mu);
+  int d = 0;
+  cudaGetDevice(&d);
+  Ws& w = pool[std::make_tuple(d, std::this_thread::get_id(), slot)];
+  if (w.cap >= nfloat) return w.p;
+#ifndef DR_CUDA_EMU
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(s, &st) != cudaSuccess || st != cudaStreamCaptureStatusNone) return nullptr;
+#endif
+  const size_t n = nfloat + nfloat / 2;
+  float* p = nullptr;
+  if (cudaMalloc(&p, n * sizeof(float)) != cudaSuccess) return nullptr;
+  w.p = p;
+  w.cap = n;
+  return p;
 }
-// Instruction descriptor (InstrDescriptor): c=f32, a=b=bf16, K-major or MN-major operands.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+enum { kWsGemmStats = 0, kWsGemmDw = 1, kWsColstats = 2, kWsHead = 3, kWsBnBwd = 4 };
+
+// dst0[c] += scale * sum_r ws[r * ld + c],  dst1[c] += scale * sum_r ws[r * ld + n + c]   (c < n, rows summed in order; dst1 may be null)
+static __global__ void k_det_colsum(const float* __restrict__ ws, int rows, int64_t ld, int n, float* __restrict__ dst0, float* __restrict__ dst1,
+                                    float scale) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n) return;
+  float s0 = 0.f, s1 = 0.f;
+  for (int r = 0; r < rows; ++r) {
+    s0 += ws[(int64_t)r * ld + c];
+    if (dst1) s1 += ws[(int64_t)r * ld + n + c];
+  }
+  dst0[c] += scale * s0;
+  if (dst1) dst1[c] += scale * s1;
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {

@@ -1,7 +1,7 @@
 // Memory-bound dense-path kernels fused as far as data dependencies allow: column statistics
 // (BatchNorm forward/backward sums, bias gradients), BatchNorm apply forward/backward (+ReLU mask),
 // the logit head (Linear(K->1) + sigmoid + BCE + full backward in one pass), weight packing
-// (fp32 master -> bf16 W and W^T for the tcgen05 GEMMs) and input cast/pad.
+// (fp32 master -> bf16 W and W^T for the wgmma GEMMs) and input cast/pad.
 //
 // Reference equivalents are library/Eigen ops (tf.layers.dense + tf.layers.batch_normalization +
 // keras BinaryCrossentropy, modelzoo/dlrm/train.py:163-243); DeepRec ships no CUDA kernel for them.
@@ -16,7 +16,8 @@ namespace {
 // u, v: bf16 [B, ld].  N multiple of 8.  Each thread owns 8 consecutive columns.
 // -------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_colstats(const __nv_bfloat16* __restrict__ u, const __nv_bfloat16* __restrict__ v,
-                                                  int64_t B, int N, int64_t ldu, int64_t ldv, float* __restrict__ S1, float* __restrict__ S2) {
+                                                  int64_t B, int N, int64_t ldu, int64_t ldv, float* __restrict__ part /* [grid][2N] */,
+                                                  int with_s2) {
   pdl_sync();
   const int tpr = N / 8;                         // threads per row
   const int rows_par = blockDim.x / tpr;         // rows processed in parallel by the block
@@ -42,24 +43,19 @@ __global__ void __launch_bounds__(256) k_colstats(const __nv_bfloat16* __restric
       }
     }
   }
-  // reduce across the rows_par row-groups through shared memory, then one atomic per column per block
-  extern __shared__ float sh[];                  // [2][N]
-  for (int i = threadIdx.x; i < 2 * N; i += blockDim.x) sh[i] = 0.f;
-  __syncthreads();
-  bool leader = tr < rows_par;
-  if (tpr < 32 && (32 % tpr) == 0) {      // narrow matrices: lanes with equal (lane % tpr) own the same columns -> shuffle-reduce first
+  // the rows_par row-groups' partials are added in row-group order (no atomics: the sums are the same on every run); the block's
+  // partial goes to part[blockIdx.x] and k_det_colsum adds the blocks in order
+  extern __shared__ float sh[];                  // [rows_par][2N]
+  if (tr < rows_par) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      for (int off = 16; off >= tpr; off >>= 1) { a1[j] += __shfl_xor_sync(0xffffffffu, a1[j], off); a2[j] += __shfl_xor_sync(0xffffffffu, a2[j], off); }
-    }
-    leader = (threadIdx.x & 31) < tpr;
-  }
-  if (leader) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { atomicAdd(&sh[tc * 8 + j], a1[j]); if (S2) atomicAdd(&sh[N + tc * 8 + j], a2[j]); }
+    for (int j = 0; j < 8; ++j) { sh[tr * 2 * N + tc * 8 + j] = a1[j]; sh[tr * 2 * N + N + tc * 8 + j] = a2[j]; }
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < N; i += blockDim.x) { atomicAdd(&S1[i], sh[i]); if (S2) atomicAdd(&S2[i], sh[N + i]); }
+  for (int i = threadIdx.x; i < (with_s2 ? 2 * N : N); i += blockDim.x) {
+    float sum = 0.f;
+    for (int r = 0; r < rows_par; ++r) sum += sh[r * 2 * N + i];
+    part[(int64_t)blockIdx.x * 2 * N + i] = sum;
+  }
 }
 
 // BatchNorm forward finalize: sums -> scale/shift (+ running stats), re-zero sums.
@@ -161,7 +157,8 @@ __global__ void __launch_bounds__(256) k_head(const __nv_bfloat16* __restrict__ 
                                               const float* __restrict__ bias, const float* __restrict__ labels, float inv_batch,
                                               float* __restrict__ prob, float* __restrict__ loss_sum, __nv_bfloat16* __restrict__ dh,
                                               float* __restrict__ dw, float* __restrict__ db, int relu_mask, int train,
-                                              float* __restrict__ dbias_h /* [K]: sum_b dh[b,:] = bias grad of the layer producing h */) {
+                                              float* __restrict__ dbias_h /* [K]: sum_b dh[b,:] = bias grad of the layer producing h */,
+                                              float* __restrict__ part /* [grid][2K + 2]: dw | dbias_h | loss | db of each block */) {
   pdl_sync();
   constexpr int K = 256 * R;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -212,22 +209,22 @@ __global__ void __launch_bounds__(256) k_head(const __nv_bfloat16* __restrict__ 
       }
     }
   }
-  __shared__ float sdw[K];
-  __shared__ float sdh[K];
-  __shared__ float sred[2];
-  for (int i = threadIdx.x; i < K; i += blockDim.x) { sdw[i] = 0.f; sdh[i] = 0.f; }
-  if (threadIdx.x < 2) sred[threadIdx.x] = 0.f;
+  // per-warp partials -> shared memory -> added in warp order -> part[blockIdx.x]; k_det_colsum adds the blocks in order (no atomics:
+  // the loss and the gradients are the same on every run)
+  extern __shared__ float sw[];                  // [8 warps][2K + 2]
+  constexpr int L = 2 * K + 2;
+#pragma unroll
+  for (int r = 0; r < R; ++r)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { sw[warp * L + r * 256 + lane * 8 + j] = dwacc[r][j]; sw[warp * L + K + r * 256 + lane * 8 + j] = dhacc[r][j]; }
+  if (lane == 0) { sw[warp * L + 2 * K] = lossacc * inv_batch; sw[warp * L + 2 * K + 1] = dbacc; }
   __syncthreads();
-  if (train) {
-#pragma unroll
-    for (int r = 0; r < R; ++r)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { atomicAdd(&sdw[r * 256 + lane * 8 + j], dwacc[r][j]); if (dbias_h) atomicAdd(&sdh[r * 256 + lane * 8 + j], dhacc[r][j]); }
+  for (int i = threadIdx.x; i < L; i += blockDim.x) {
+    float sum = 0.f;
+    for (int w = 0; w < wpb; ++w) sum += sw[w * L + i];
+    part[(int64_t)blockIdx.x * L + i] = sum;
   }
-  if (lane == 0) { atomicAdd(&sred[0], lossacc); atomicAdd(&sred[1], dbacc); }
-  __syncthreads();
-  if (train) for (int i = threadIdx.x; i < K; i += blockDim.x) { atomicAdd(&dw[i], sdw[i]); if (dbias_h) atomicAdd(&dbias_h[i], sdh[i]); }
-  if (threadIdx.x == 0) { atomicAdd(loss_sum, sred[0] * inv_batch); if (train) atomicAdd(db, sred[1]); }
+  (void)dw; (void)db; (void)loss_sum; (void)train; (void)dbias_h;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -269,7 +266,7 @@ __global__ void k_l2_flush(float* __restrict__ buf, int64_t n, float v) {
 
 // -------------------------------------------------------------------------------------------------
 // BatchNorm folding (forward): finalize the batch statistics of layer l and fold y = s*a + t into layer l+1:
-//   W'[n,k] = W[n,k] * s[k]   (bf16, the tcgen05 B operand)      b'[n] = b[n] + sum_k W[n,k] * t[k]   (fp32)
+//   W'[n,k] = W[n,k] * s[k]   (bf16, the wgmma B operand)      b'[n] = b[n] + sum_k W[n,k] * t[k]   (fp32)
 // so the normalised activation is never materialised (no extra pass over [B, N]).  One block per output row n;
 // block 0 also publishes mean/rstd/scale/shift and advances the running statistics.
 // -------------------------------------------------------------------------------------------------
@@ -330,7 +327,7 @@ __global__ void __launch_bounds__(256) k_bn_bwd_apply_v2(const __nv_bfloat16* __
                                                          int N, int64_t ld, const float* __restrict__ scale, const float* __restrict__ mean,
                                                          const float* __restrict__ rstd, const float* __restrict__ c1,
                                                          const float* __restrict__ c2, __nv_bfloat16* __restrict__ da, int relu_mask,
-                                                         float* __restrict__ dbias) {
+                                                         float* __restrict__ dbias_part /* [grid][N] or null */) {
   pdl_sync();
   const int tpr = N / 8;
   const int rows_par = blockDim.x / tpr;
@@ -371,27 +368,22 @@ __global__ void __launch_bounds__(256) k_bn_bwd_apply_v2(const __nv_bfloat16* __
       }
     }
   }
-  if (dbias) {
-    extern __shared__ float sh[];
-    for (int i = threadIdx.x; i < N; i += blockDim.x) sh[i] = 0.f;
-    __syncthreads();
-    bool leader = tr < rows_par;
-    if (tpr < 32 && (32 % tpr) == 0) {
+  if (dbias_part) {                               // row-group partials added in order -> part[blockIdx.x] (k_det_colsum adds the blocks)
+    extern __shared__ float sh[];                 // [rows_par][N]
+    if (tr < rows_par) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-        for (int off = 16; off >= tpr; off >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], off);
-      leader = (threadIdx.x & 31) < tpr;
-    }
-    if (leader) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) atomicAdd(&sh[tc * 8 + j], acc[j]);
+      for (int j = 0; j < 8; ++j) sh[tr * N + tc * 8 + j] = acc[j];
     }
     __syncthreads();
-    for (int i = threadIdx.x; i < N; i += blockDim.x) atomicAdd(&dbias[i], sh[i]);
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+      float sum = 0.f;
+      for (int r = 0; r < rows_par; ++r) sum += sh[r * N + i];
+      dbias_part[(int64_t)blockIdx.x * N + i] = sum;
+    }
   }
 }
 
-inline int grid_for(int64_t n, int block, int max_blocks = kNumSMs * 8) {
+inline int grid_for(int64_t n, int block, int max_blocks = num_sms() * 8) {
   int64_t b = (n + block - 1) / block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -405,8 +397,13 @@ extern "C" {
 int dr_cuda_colstats(const void* u, const void* v, int64_t B, int N, int64_t ldu, int64_t ldv, float* S1, float* S2, cudaStream_t s) {
   if (N % 8 || N / 8 > 256) return -2;
   int tpr = N / 8; int rows_par = 256 / tpr;
-  int grid = grid_for((B + rows_par - 1) / rows_par, 2, kNumSMs * 4);   // >= 2 row-groups per block
-  DR_PDL_LAUNCH((k_colstats), grid, 256, 2 * N * sizeof(float), s, (const __nv_bfloat16*)u, (const __nv_bfloat16*)v, B, N, ldu, ldv, S1, S2);
+  int grid = grid_for((B + rows_par - 1) / rows_par, 2, num_sms() * 4);   // >= 2 row-groups per block
+  float* part = dr_workspace(kWsColstats, (size_t)grid * 2 * N, s);
+  if (!part) return -5;
+  DR_PDL_LAUNCH((k_colstats), grid, 256, rows_par * 2 * N * sizeof(float), s, (const __nv_bfloat16*)u, (const __nv_bfloat16*)v, B, N, ldu, ldv, part,
+                S2 ? 1 : 0);
+  DR_LAUNCH_CHECK();
+  k_det_colsum<<<(N + 127) / 128, 128, 0, s>>>(part, grid, 2 * (int64_t)N, N, S1, S2, 1.f);
   DR_LAUNCH_CHECK();
   return 0;
 }
@@ -461,19 +458,45 @@ int dr_cuda_bn_bwd_apply_v2(const void* dy, const void* a, int64_t B, int N, int
                             const float* rstd, const float* c1, const float* c2, void* da, int relu_mask, float* dbias, cudaStream_t s) {
   if (N % 8 || N / 8 > 256) return -2;
   int tpr = N / 8; int rows_par = 256 / tpr;
-  int grid = grid_for((B + rows_par - 1) / rows_par, 2, kNumSMs * 8);
-  DR_PDL_LAUNCH((k_bn_bwd_apply_v2), grid, 256, N * sizeof(float), s, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)a, B, N, ld, scale, mean, rstd, c1, c2,
-                                                        (__nv_bfloat16*)da, relu_mask, dbias);
+  int grid = grid_for((B + rows_par - 1) / rows_par, 2, num_sms() * 8);
+  float* part = nullptr;
+  if (dbias) {
+    part = dr_workspace(kWsBnBwd, (size_t)grid * N, s);
+    if (!part) return -5;
+  }
+  DR_PDL_LAUNCH((k_bn_bwd_apply_v2), grid, 256, rows_par * N * sizeof(float), s, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)a, B, N, ld, scale, mean, rstd,
+                c1, c2, (__nv_bfloat16*)da, relu_mask, part);
   DR_LAUNCH_CHECK();
+  if (dbias) {
+    k_det_colsum<<<(N + 127) / 128, 128, 0, s>>>(part, grid, (int64_t)N, N, dbias, nullptr, 1.f);
+    DR_LAUNCH_CHECK();
+  }
   return 0;
 }
 
 int dr_cuda_head(const void* h, int64_t ldh, int64_t B, int K, const float* w, const float* bias, const float* labels, float inv_batch,
                  float* prob, float* loss_sum, void* dh, float* dw, float* db, int relu_mask, int train, float* dbias_h, cudaStream_t s) {
-  int grid = grid_for((B + 7) / 8, 1, kNumSMs * 4);
-#define HEAD(R) DR_PDL_LAUNCH((k_head<R>), grid, 256, 0, s, (const __nv_bfloat16*)h, ldh, B, w, bias, labels, inv_batch, prob, loss_sum, (__nv_bfloat16*)dh, dw, db, relu_mask, train, dbias_h)
-  if (K == 256) HEAD(1); else if (K == 512) HEAD(2); else if (K == 1024) HEAD(4); else return -2;
+  int grid = grid_for((B + 7) / 8, 1, num_sms() * 4);
+  if (K != 256 && K != 512 && K != 1024) return -2;
+  float* part = dr_workspace(kWsHead, (size_t)grid * (2 * K + 2), s);
+  if (!part) return -5;
+  const size_t smem = 8 * (2 * K + 2) * sizeof(float);
+#define HEAD(R)                                                                                                                     \
+  do {                                                                                                                              \
+    static DrPerDeviceOnce attr_once; bool& attr = attr_once();                                                                     \
+    if (!attr) { DR_CUDA_CHECK(cudaFuncSetAttribute(k_head<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); attr = true; } \
+    DR_PDL_LAUNCH((k_head<R>), grid, 256, smem, s, (const __nv_bfloat16*)h, ldh, B, w, bias, labels, inv_batch, prob, loss_sum, (__nv_bfloat16*)dh, dw, db, \
+                  relu_mask, train, dbias_h, part);                                                                                 \
+  } while (0)
+  if (K == 256) HEAD(1); else if (K == 512) HEAD(2); else HEAD(4);
 #undef HEAD
+  DR_LAUNCH_CHECK();
+  const int64_t L = 2 * (int64_t)K + 2;
+  if (train) {
+    k_det_colsum<<<(K + 127) / 128, 128, 0, s>>>(part, grid, L, K, dw, nullptr, 1.f);
+    if (dbias_h) k_det_colsum<<<(K + 127) / 128, 128, 0, s>>>(part + K, grid, L, K, dbias_h, nullptr, 1.f);
+  }
+  k_det_colsum<<<1, 1, 0, s>>>(part + 2 * K, grid, L, 1, loss_sum, train ? db : nullptr, 1.f);
   DR_LAUNCH_CHECK();
   return 0;
 }
@@ -492,7 +515,7 @@ int dr_cuda_cast_pad(const float* x, int64_t B, int C, void* y, int Cp, cudaStre
 }
 
 int dr_cuda_l2_flush(float* buf, int64_t n, float v, cudaStream_t s) {
-  k_l2_flush<<<kNumSMs * 4, 256, 0, s>>>(buf, n, v);
+  k_l2_flush<<<num_sms() * 4, 256, 0, s>>>(buf, n, v);
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(256) k_segment_sum(const float* __restrict__ r
 }
 
 inline int grid_for(int64_t n, int block, int max_blocks = 0) {
-  if (max_blocks <= 0) max_blocks = kNumSMs * sparse_blocks_per_sm();
+  if (max_blocks <= 0) max_blocks = num_sms() * sparse_blocks_per_sm();
   int64_t b = (n + block - 1) / block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;

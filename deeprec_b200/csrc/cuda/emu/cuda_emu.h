@@ -6,7 +6,7 @@
 // What is emulated: grid / block indices, static and dynamic shared memory, __syncthreads (threads that already returned count as
 // arrived), __syncwarp, shfl / ballot / any / all / match_any / activemask, the atomics, the system-scope acquire / release helpers of
 // common.cuh, the handful of runtime calls the host wrappers make (device memory == host memory, streams are synchronous), cub's
-// DeviceScan / DeviceSelect / DeviceRadixSort entry points.  What is NOT: tcgen05 / TMEM / TMA / mbarrier (those kernels are validated on
+// DeviceScan / DeviceSelect / DeviceRadixSort entry points.  What is NOT: wgmma / mma.sync / TMA / mbarrier (those kernels are validated on
 // hardware only), timing, memory-model weaknesses (x86 is stronger than the GPU: a pass here does not prove a fence is sufficient).
 //
 // Blocks of one grid run one after the other (a kernel whose blocks wait on each other would deadlock; none of ours do); kernels of

@@ -1,4 +1,4 @@
-// Emulation-build stand-ins for the entry points whose kernels are tcgen05 / TMA code (hardware only): the SAME argument contract
+// Emulation-build stand-ins for the entry points whose kernels are wgmma / TMA code (hardware only): the SAME argument contract
 // (shape / alignment checks copied from the real wrappers) over a plain host loop, so that the layers above them -- the op-program
 // interpreter of serving_runtime.cu, the engines' launch sequences -- run end to end on the CPU emulation.  Never part of libdeeprec_cuda.so.
 #ifndef DR_CUDA_EMU
@@ -12,7 +12,7 @@ inline float bf(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
 extern "C" {
 
-// gemm_tcgen05.cu::dr_cuda_gemm_tn_ex: out[M,N] = A[M,K](lda) * B[N,K](ldb)^T (+bias)(relu)(*mask); bf16 in / out, fp32 accumulate
+// gemm_wgmma.cu::dr_cuda_gemm_tn_ex: out[M,N] = A[M,K](lda) * B[N,K](ldb)^T (+bias)(relu)(*mask); bf16 in / out, fp32 accumulate
 int dr_cuda_gemm_tn_ex(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* bias, int relu, const void* mask_src,
                        int64_t ld_mask, int aux_mode, void* out, int64_t ldc, float* out_f32, float* S1, float* S2, int max_ctas, int force_v1, cudaStream_t) {
   (void)max_ctas; (void)force_v1;
@@ -45,7 +45,7 @@ int dr_cuda_gemm_tn(const void* A, int64_t lda, const void* B, int64_t ldb, int 
   return dr_cuda_gemm_tn_ex(A, lda, B, ldb, M, N, K, bias, relu, mask_src, ld_mask, mask_src ? 1 : 0, out, ldc, out_f32, nullptr, nullptr, max_ctas, 0, s);
 }
 
-// gemm_tcgen05.cu::dr_cuda_gemm_dw: dW[N_out,K_in](ldw, fp32, accumulated into) += dY[batch,N_out](ldy)^T * X[batch,K_in](ldx)
+// gemm_wgmma.cu::dr_cuda_gemm_dw: dW[N_out,K_in](ldw, fp32, accumulated into) += dY[batch,N_out](ldy)^T * X[batch,K_in](ldx)
 int dr_cuda_gemm_dw(const void* dY, int64_t ldy, const void* X, int64_t ldx, int batch, int N_out, int K_in, float* dW, int64_t ldw, int splits, cudaStream_t) {
   (void)splits;
   if (batch <= 0 || N_out <= 0 || K_in <= 0) return 0;

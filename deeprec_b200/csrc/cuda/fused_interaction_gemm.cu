@@ -1,38 +1,37 @@
-// k_dlrm_inter_gemm: embedding combine (+ROWS-flag wait) ⊕ DLRM dot interaction ⊕ top-MLP layer 0, ONE tcgen05 kernel (sm_100a).
+// k_dlrm_inter_gemm: embedding combine (+ROWS-flag wait) ⊕ DLRM dot interaction ⊕ top-MLP layer 0, ONE wgmma kernel (sm_90a).
 //
 // Reference dataflow replaced: SOK all2all(vectors) -> reorderKernel (all2all_output_dispatcher.cu:159-193) -> tf.matmul(X, X^T) +
-// boolean_mask + concat (modelzoo/dlrm/train.py:121-133) -> cuBLAS Dense(512)+ReLU.  Round 1 ran three kernels here (rank barrier,
-// k_dot_fwd_tc writing Z, tcgen05 GEMM reading Z back); now the 128-sample Z tile is BUILT IN SHARED MEMORY in the 128B-swizzled
-// K-major layout tcgen05.mma consumes, and multiplied by W0 without the GEMM ever reading it from HBM:
+// boolean_mask + concat (modelzoo/dlrm/train.py:121-133) -> cuBLAS Dense(512)+ReLU.  Unfused, this is three kernels (rank barrier,
+// k_dot_fwd_tc writing Z, GEMM reading Z back); here the 128-sample Z tile is BUILT IN SHARED MEMORY in the 128B-swizzled K-major
+// layout wgmma consumes, and multiplied by W0 without the GEMM ever reading it from HBM:
 //
-//   warp 0        TMA producer: streams W0 [512 x 368] through a 4-stage ring of [128 n x 64 k] tiles (OOB K columns zero-filled)
-//   warp 1        MMA issuer (one elected thread): per 128-sample tile 4 x 6 x 4 tcgen05.mma  acc[128 x 128] += Z[128 x 64] W0^T  with
-//                 the accumulators double-buffered in TMEM; also issues the TMA stores of the finished Z tile (the backward's dW0 GEMM
-//                 and nothing else reads it)
-//   warps 2-9     builders (warp = sample, 16 samples per warp per tile): gather urow[inv[b][t]] rows straight out of the peer-written
-//                 unique-row buffer (the kernel first waits for every owner's ROWS flag), compute the sample's 32 x 32 x 16 Gram
-//                 matrix with six warp-level mma.sync.m16n8k16 (lower-triangle tiles only) and scatter the strict lower triangle
-//                 into the swizzled Z tile.  (The first version padded four samples to one 128 x 128 x 16 tcgen05.mma and read the
-//                 diagonal blocks back from TMEM: 15/16 of the tensor op wasted and, worse, a builder -> MMA thread -> TMEM ->
-//                 builder round trip per four samples with only two pipelines per SM -- 200 us instead of 99 us unfused.  A Gram
-//                 block is too small for a UMMA tile; the GEMM is not.)
-//   warps 10-13   epilogue: tcgen05.ld -> +bias -> ReLU -> bf16 -> 16 B global stores of a0 [B, 512]
-//
-// TMEM (256 columns): two 128 x 128 fp32 GEMM accumulators.
+//   warpgroup 0      TMA producer (one thread): streams W0 [512 x 368] through a 7-stage ring of [128 n x 64 k] tiles (OOB K columns
+//                    zero-filled)
+//   warpgroups 1-2   per 128-sample tile, two phases:
+//                    build -- warp = sample slot (16 samples per warp per tile): gather urow[inv[b][t]] rows straight out of the
+//                    peer-written unique-row buffer (the kernel first waits for every owner's ROWS flag), compute the sample's
+//                    32 x 32 x 16 Gram matrix with six warp-level mma.sync.m16n8k16 (lower-triangle tiles only) and scatter the strict
+//                    lower triangle into the swizzled Z tile; one thread then TMA-stores the finished tile for the backward's dW0 GEMM;
+//                    GEMM -- warpgroup g multiplies rows [64 g, 64 g + 64) of the Z tile by every 128-wide n block of W0 with
+//                    wgmma.mma_async (fp32 register accumulators), then +bias -> ReLU -> bf16 stores of a0 [B, 512].
+//                    The rows of the next tile's first samples are already in flight in registers while the GEMM phase runs.
 #include <cuda.h>
 
 #include "sp_sync.cuh"
+#include "wgmma.cuh"
 
 using namespace drc;
 
 namespace {
+
+__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 constexpr int kD = 16;                  // embedding dim (= bottom MLP output)
 constexpr int kTileM = 128;             // samples per tile
 constexpr int kBN = 128;                // GEMM n-block
 constexpr int kKB = 64;                 // GEMM k-block (one 128 B swizzle row)
 constexpr int kStagesB = 7;             // 7 x 16 KB W0 tiles in flight: the per-SM L2->smem path needs ~100 KB outstanding to stay busy
-constexpr int kThreads = 14 * 32;
+constexpr int kThreads = 3 * 128;
 constexpr int kMaxKb = 6;               // K <= 384
 
 struct FusedSmem {
@@ -71,7 +70,6 @@ int make_tmap(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, u
   return r == CUDA_SUCCESS ? 0 : -101 - (int)r;
 }
 
-// 14 warps: the register file is split in four 16 K partitions and some partition hosts 4 warps => at most 128 registers / thread
 __global__ void __launch_bounds__(kThreads, 1)
 k_dlrm_inter_gemm(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmZ, const __nv_bfloat16* __restrict__ x, int64_t ldx,
                   const __nv_bfloat16* __restrict__ urow, const int32_t* __restrict__ inv, int ldinv, int T, int64_t B, int Kz /* D + F(F-1)/2 */,
@@ -86,11 +84,6 @@ k_dlrm_inter_gemm(const __grid_constant__ CUtensorMap tmW, const __grid_constant
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);
   uint64_t* full_bar = bars;                       // [kStagesB]  W0 tile landed
   uint64_t* empty_bar = bars + kStagesB;           // [kStagesB]  W0 tile consumed
-  uint64_t* tfull_bar = bars + 2 * kStagesB;       // [2] accumulator complete
-  uint64_t* tempty_bar = tfull_bar + 2;            // [2] accumulator drained by the epilogue
-  uint64_t* zfull_bar = tempty_bar + 2;            // Z tile complete (all 8 builder warps)
-  uint64_t* zempty_bar = zfull_bar + 1;            // every MMA reading the Z tile has retired
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(zempty_bar + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int F = T + 1;
@@ -100,18 +93,12 @@ k_dlrm_inter_gemm(const __grid_constant__ CUtensorMap tmW, const __grid_constant
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmW); tma_prefetch_desc(&tmZ);
-    for (int i = 0; i < kStagesB; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 4); }
-    mbar_init(zfull_bar, 8); mbar_init(zempty_bar, 1);
+    for (int i = 0; i < kStagesB; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_ptr, 256); tmem_relinquish(); }
   // zero the Z tile once: the K padding columns [Kz, num_kb * 64) stay zero for the kernel's life, the feature tiles' padding rows too
   for (int i = threadIdx.x; i < (L::kZBytes + kStagesB * L::kBStage + 2 * L::kFBytes) / 16; i += blockDim.x) reinterpret_cast<int4*>(smem)[i] = make_int4(0, 0, 0, 0);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   pdl_sync();
   if (sync.state) sp_wait_all(sync, SP_CH_ROWS);            // every owner has pushed this step's rows into my urow
   for (int i = threadIdx.x; i < 512; i += blockDim.x) s_bias[i] = (bias != nullptr && i < N) ? bias[i] : 0.f;
@@ -131,46 +118,10 @@ k_dlrm_inter_gemm(const __grid_constant__ CUtensorMap tmW, const __grid_constant
             if (++stage == kStagesB) { stage = 0; phase ^= 1; }
           }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      constexpr uint32_t idesc_gemm = umma_idesc_bf16(kTileM, kBN, 0, 0);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      uint32_t zphase = 0;
-      for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        // ---- Z tile complete -> TMA-store it for the backward, then the GEMM
-        mbar_wait(zfull_bar, zphase);
-        tc_fence_after();
-        if (store_z && !(dbg & 4)) {
-          for (int kb = 0; kb < num_kb; ++kb) tma_store_2d(&tmZ, sZ + kb * (kTileM * 128), kb * kKB, (int)(tile * kTileM));
-          tma_store_commit();
-        }
-        for (int nb = 0; nb < n_blks; ++nb) {
-          mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * kBN;
-          for (int kb = 0; kb < num_kb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint64_t adesc = umma_desc_sw128(smem_u32(sZ + kb * (kTileM * 128)), 16, 1024);
-            const uint64_t bdesc = umma_desc_sw128(smem_u32(sB + stage * L::kBStage), 16, 1024);
-#pragma unroll
-            for (int k = 0; k < kKB / 16; ++k) umma_bf16(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc_gemm, (kb | k) != 0);
-            umma_commit(&empty_bar[stage]);
-            if (kb == num_kb - 1) umma_commit(&tfull_bar[acc]);
-            if (++stage == kStagesB) { stage = 0; phase ^= 1; }
-          }
-          if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-        if (store_z && !(dbg & 4)) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");     // the stores have read the tile
-        umma_commit(zempty_bar);                                                       // ... and so will have every MMA above
-        zphase ^= 1;
-      }
-    }
-  } else if (warp < 10) {
-    // ================= builders: gather + warp-level Gram (mma.sync) + lower-triangle scatter into the swizzled Z tile =================
-    const int bw = warp - 2;                          // 0..7: this warp handles samples bw, bw + 8, ... of every tile
+  } else if (warp >= 4) {
+    // ================= builders + GEMM: gather + warp-level Gram (mma.sync) + lower-triangle scatter into the swizzled Z tile =================
+    const int bw = warp - 4;                          // 0..7: this warp handles samples bw, bw + 8, ... of every tile
+    const int wg = bw >> 2, wl = bw & 3, ct = threadIdx.x - 128;
     uint8_t* myF = sF + bw * 1024;                    // [32 feature rows][32 B] row-major staging tile of the current sample
     const int gI = lane >> 2, tI = lane & 3;          // mma.sync fragment coordinates
     // scatter plan of this lane's 12 accumulator pairs: byte offset inside a Z row of (fi, j) (k-block, 16 B chunk, element), before
@@ -195,7 +146,7 @@ k_dlrm_inter_gemm(const __grid_constant__ CUtensorMap tmW, const __grid_constant
           }
         }
     }
-    uint32_t zeph = 0;
+    int stage = 0; uint32_t phase = 0;
     // Gather pipeline: a warp keeps a CHUNK of 4 samples in flight (rows of chunk k+1 and indices of chunk k+2 are loading while
     // chunk k is processed) -- one sample in flight per warp left the kernel bound by the L2 / NVLink-written-row latency.
     constexpr int SPW = kTileM / 8;                   // samples per warp per tile
@@ -230,8 +181,8 @@ k_dlrm_inter_gemm(const __grid_constant__ CUtensorMap tmW, const __grid_constant
       for (int u = 0; u < CH; ++u) fetch_idx1(t1, k1, u);
     }
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      // the previous tile's GEMM (and Z stores) must have finished reading the Z tile before the first write of this one
-      if (tile != (int64_t)blockIdx.x) { mbar_wait(zempty_bar, zeph); zeph ^= 1; }
+      // the previous tile's GEMM (both warpgroups) and Z stores must have finished reading the Z tile before the first write of this one
+      if (tile != (int64_t)blockIdx.x) consumer_bar_sync();
       for (int k = 0; k < CPT; ++k) {
         int64_t t1 = tile; int k1 = k; advance(t1, k1);        // next chunk (rows to fetch now)
         int64_t t2 = t1; int k2 = k1; advance(t2, k2);         // the chunk after it (indices to fetch now)
@@ -302,54 +253,56 @@ k_dlrm_inter_gemm(const __grid_constant__ CUtensorMap tmW, const __grid_constant
         __syncwarp();                                   // the staging tile is rewritten by the next sample
         }
       }
-      // ---- this warp's 16 rows of the tile are written
+      // ---- the Z tile is complete: hand it to the async proxy (TMA store, wgmma)
       fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(zfull_bar);
-    }
-  } else {
-    // ================= epilogue warps =================
-    const int q = warp & 3;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      const int64_t row = tile * kTileM + q * 32 + lane;
+      consumer_bar_sync();
+      if (ct == 0 && store_z && !(dbg & 4)) {
+        for (int kb = 0; kb < num_kb; ++kb) tma_store_2d(&tmZ, sZ + kb * (kTileM * 128), kb * kKB, (int)(tile * kTileM));
+        tma_store_commit();
+      }
+      // ---- GEMM: rows [64 wg, 64 wg + 64) of the tile x every n block of W0
+      const int64_t row0 = tile * kTileM + wg * 64 + wl * 16 + (lane >> 2);
       for (int nb = 0; nb < n_blks; ++nb) {
-        mbar_wait(&tfull_bar[acc], acc_phase);
-        tc_fence_after();
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * kBN;
-#pragma unroll 1
-        for (int c0 = 0; c0 < kBN; c0 += 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(t_row + c0, r);
-          tmem_ld_wait();
-          const int col0 = nb * kBN + c0;
-          if (!(dbg & 8) && row < B && col0 < N) {
-            __nv_bfloat16* dst = out + row * ldo + col0;
+        float acc[kBN / 2];
 #pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              if (col0 + j < N) {
-                float v[8];
+        for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint64_t adesc = gmma_desc_sw128(smem_u32(sZ + kb * (kTileM * 128) + wg * 64 * 128), 16, 1024);
+          const uint64_t bdesc = gmma_desc_sw128(smem_u32(sB + stage * L::kBStage), 16, 1024);
+          wgmma_fence();
 #pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] = fmaxf(__uint_as_float(r[j + e]) + s_bias[col0 + j + e], 0.f);
-                int4 pk;
-                pk.x = (int)pack_bf16x2(v[0], v[1]); pk.y = (int)pack_bf16x2(v[2], v[3]);
-                pk.z = (int)pack_bf16x2(v[4], v[5]); pk.w = (int)pack_bf16x2(v[6], v[7]);
-                *reinterpret_cast<int4*>(dst + j) = pk;
+          for (int k = 0; k < kKB / 16; ++k) wgmma_bf16<kBN, 0, 0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == kStagesB) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc);
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (!(dbg & 8)) {
+#pragma unroll
+          for (int j = 0; j < kBN / 8; ++j) {
+            const int col = nb * kBN + 8 * j + 2 * (lane & 3);
+            if (col >= N) continue;                       // N is a multiple of 8
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int64_t row = row0 + 8 * h;
+              if (row < B) {
+                const float v0 = fmaxf(acc[4 * j + 2 * h] + s_bias[col], 0.f), v1 = fmaxf(acc[4 * j + 2 * h + 1] + s_bias[col + 1], 0.f);
+                *reinterpret_cast<uint32_t*>(out + row * ldo + col) = pack_bf16x2(v0, v1);
               }
             }
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       }
+      if (ct == 0 && store_z && !(dbg & 4)) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");     // the stores have read the tile
     }
+    if (ct == 0) tma_store_wait_all();
   }
-  if (warp == 1 && lane == 0) tma_store_wait_all();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 256);
 }
 
 }  // namespace
@@ -376,7 +329,7 @@ int dr_cuda_dlrm_inter_gemm(const void* x, int64_t ldx, const void* urow, const 
   static DrPerDeviceOnce attr_once; bool& attr = attr_once();
   if (!attr) { DR_CUDA_CHECK(cudaFuncSetAttribute(k_dlrm_inter_gemm, cudaFuncAttributeMaxDynamicSharedMemorySize, FusedSmem::kTotal)); attr = true; }
   const int64_t ntiles = (B + kTileM - 1) / kTileM;
-  const int grid = (int)(ntiles < kNumSMs ? ntiles : kNumSMs);
+  const int grid = (int)(ntiles < num_sms() ? ntiles : num_sms());
   DrSpSync sy{}; if (sync) sy = *sync;
   DR_PDL_LAUNCH((k_dlrm_inter_gemm), grid, kThreads, FusedSmem::kTotal, s, tw, tz, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)urow, inv, ldinv, T, B, Kz,
                 N, bias, (__nv_bfloat16*)out, ldo, Z ? 1 : 0, sy, fused_dbg());

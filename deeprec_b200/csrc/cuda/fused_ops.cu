@@ -97,8 +97,8 @@ __global__ void k_dice_fwd(const float* __restrict__ x, int64_t rows, int cols, 
   }
 }
 
-inline int grid_rows(int64_t rows) { int64_t b = (rows + 7) / 8; if (b < 1) b = 1; if (b > kNumSMs * 8) b = kNumSMs * 8; return (int)b; }
-inline int grid_el(int64_t n) { int64_t b = (n + 255) / 256; if (b < 1) b = 1; if (b > kNumSMs * 8) b = kNumSMs * 8; return (int)b; }
+inline int grid_rows(int64_t rows) { int64_t b = (rows + 7) / 8; if (b < 1) b = 1; if (b > num_sms() * 8) b = num_sms() * 8; return (int)b; }
+inline int grid_el(int64_t n) { int64_t b = (n + 255) / 256; if (b < 1) b = 1; if (b > num_sms() * 8) b = num_sms() * 8; return (int)b; }
 
 }  // namespace
 

@@ -1,15 +1,8 @@
-// FP8 (E4M3) tcgen05 GEMM for the serving MLP:  D[M,N] = (A_q[M,K] * B_q[N,K]^T) * col_scale[n] + bias[n]  (ReLU)
-//   A_q : activations quantised per tensor (static scale from calibration), B_q : weights quantised per output channel;
-//   col_scale[n] = a_scale * w_scale[n] is folded on the host, so the epilogue is one FMA per element.
-//   The output is either bf16 (last layer / consumers that want bf16) or E4M3 re-quantised with the NEXT layer's activation
-//   scale (out = sat_e4m3(v * out_inv_scale)), so a chain of layers never leaves 8-bit storage between GEMMs.
-// tcgen05.mma kind::f8f6f4 (dense 8-bit peak = 2x bf16), K-major operands, 128B-swizzled TMA tiles: one smem row = 128 B
-// = 128 fp8 elements, so BLOCK_K = 128 and each stage issues 4 MMAs of K = 32.  Same warp-specialised persistent structure
-// as k_gemm_tn (gemm_tcgen05.cu): warp 0 TMA producer, warp 1 MMA issuer, warps 2-5 epilogue, double-buffered TMEM.
+// FP8 (E4M3) quantisation kernels of the serving MLP: activations per tensor (static scale from calibration), weights per output
+// channel, and the abs-max used to calibrate.  The FP8 GEMM that consumes them is dr_cuda_gemm_fp8_tn (gemm_wgmma.cu).
 //
 // SURVEY §2.9 "tools/low_precision_optimize" (BF16/FP16/INT8 model quantisation incl. EV) is the reference's low-precision
 // story -- a graph rewrite that calls library kernels; BASELINE config 5 asks for an fp8 MLP in SessionGroup inference.
-#include <cuda.h>
 #include <cuda_fp8.h>
 
 #include "common.cuh"
@@ -18,240 +11,12 @@ using namespace drc;
 
 namespace {
 
-constexpr int BLOCK_M = 128;
-constexpr int BLOCK_K8 = 128;        // 128 fp8 = 128 B = one swizzle-128B row
-constexpr int UMMA_K8 = 32;
-constexpr int kStages8 = 4;
-constexpr int kThreads8 = 192;
-
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-PFN_encodeTiled get_encode8() {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (PFN_encodeTiled)p;
-  }
-  return fn;
-}
-
-int make_tmap_u8(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, uint64_t pitch_bytes, uint32_t box_inner, uint32_t box_outer) {
-  PFN_encodeTiled enc = get_encode8();
-  if (!enc) return -100;
-  cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {pitch_bytes};
-  cuuint32_t box[2] = {box_inner, box_outer};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : -101 - (int)r;
-}
-
-// InstrDescriptor for kind::f8f6f4: c = f32 (bit 4), a_format = b_format = 0 (E4M3), K-major operands
-__host__ __device__ constexpr uint32_t umma_idesc_e4m3(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_fp8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
 // 4 floats -> 4 packed E4M3 bytes (round-to-nearest, saturate to +-448)
 __device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
   uint16_t lo, hi;
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(b), "f"(a));
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(d), "f"(c));
   return (uint32_t)lo | ((uint32_t)hi << 16);
-}
-
-struct Epi8 {
-  const float* col_scale;   // [N]
-  const float* bias;        // [N] or null
-  void* out;                // bf16 [M, ldc] or e4m3 [M, ldc]
-  int64_t ldc;
-  int relu;
-  int out_fp8;
-  float out_inv_scale;
-};
-
-template <int BLOCK_N>
-struct Smem8 {
-  static constexpr int kABytes = BLOCK_M * BLOCK_K8;
-  static constexpr int kBBytes = BLOCK_N * BLOCK_K8;
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTotal = kStages8 * kStageBytes + 1024 + 256;
-};
-
-template <int BLOCK_N>
-__global__ void __launch_bounds__(kThreads8, 1)
-k_gemm_fp8_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K, Epi8 ep) {
-  using L = Smem8<BLOCK_N>;
-  constexpr int kTmemCols = (2 * BLOCK_N <= 32) ? 32 : (2 * BLOCK_N <= 64) ? 64 : (2 * BLOCK_N <= 128) ? 128 : (2 * BLOCK_N <= 256) ? 256 : 512;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages8 * L::kStageBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + kStages8;
-  uint64_t* tfull_bar = bars + 2 * kStages8;
-  uint64_t* tempty_bar = bars + 2 * kStages8 + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * kStages8 + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-  const int n_tiles = (N + BLOCK_N - 1) / BLOCK_N;
-  const int num_tiles = m_tiles * n_tiles;
-  const int num_kb = (K + BLOCK_K8 - 1) / BLOCK_K8;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < kStages8; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 4); }
-    fence_mbar_init();
-  }
-  if (warp == 1) { tmem_alloc(tmem_ptr, kTmemCols); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * L::kStageBytes;
-          uint8_t* sb = sa + L::kABytes;
-          mbar_expect_tx(&full_bar[stage], L::kStageBytes);
-          tma_load_2d(sa, &tmA, &full_bar[stage], kb * BLOCK_K8, m_blk * BLOCK_M);
-          tma_load_2d(sb, &tmB, &full_bar[stage], kb * BLOCK_K8, n_blk * BLOCK_N);
-          if (++stage == kStages8) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_e4m3(BLOCK_M, BLOCK_N);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * L::kStageBytes);
-          const uint32_t sb = sa + L::kABytes;
-          const uint64_t adesc = umma_desc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = umma_desc_sw128(sb, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K8 / UMMA_K8; ++k)       // +32 B inside the swizzle atom per K = 32 step
-            umma_fp8(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-          umma_commit(&empty_bar[stage]);
-          if (kb == num_kb - 1) umma_commit(&tfull_bar[acc]);
-          if (++stage == kStages8) { stage = 0; phase ^= 1; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const int row = m_blk * BLOCK_M + q * 32 + lane;
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BLOCK_N;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_row + c0, r);
-        tmem_ld_wait();
-        const int col0 = n_blk * BLOCK_N + c0;
-        if (row < M && col0 < N) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            if (col0 + j < N) {
-              const float4 sc = *reinterpret_cast<const float4*>(ep.col_scale + col0 + j);
-              float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (ep.bias) b = *reinterpret_cast<const float4*>(ep.bias + col0 + j);
-              v[j] = fmaf(__uint_as_float(r[j]), sc.x, b.x); v[j + 1] = fmaf(__uint_as_float(r[j + 1]), sc.y, b.y);
-              v[j + 2] = fmaf(__uint_as_float(r[j + 2]), sc.z, b.z); v[j + 3] = fmaf(__uint_as_float(r[j + 3]), sc.w, b.w);
-            } else {
-              v[j] = v[j + 1] = v[j + 2] = v[j + 3] = 0.f;
-            }
-          }
-          if (ep.relu) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-          if (ep.out_fp8) {
-            uint8_t* dst = reinterpret_cast<uint8_t*>(ep.out) + (int64_t)row * ep.ldc + col0;
-            const float s = ep.out_inv_scale;
-#pragma unroll
-            for (int j = 0; j < 32; j += 16) {
-              if (col0 + j < N) {       // N is a multiple of 16 on this path (checked on the host)
-                int4 pk;
-                pk.x = (int)pack_e4m3x4(v[j] * s, v[j + 1] * s, v[j + 2] * s, v[j + 3] * s);
-                pk.y = (int)pack_e4m3x4(v[j + 4] * s, v[j + 5] * s, v[j + 6] * s, v[j + 7] * s);
-                pk.z = (int)pack_e4m3x4(v[j + 8] * s, v[j + 9] * s, v[j + 10] * s, v[j + 11] * s);
-                pk.w = (int)pack_e4m3x4(v[j + 12] * s, v[j + 13] * s, v[j + 14] * s, v[j + 15] * s);
-                *reinterpret_cast<int4*>(dst + j) = pk;
-              }
-            }
-          } else {
-            __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(ep.out) + (int64_t)row * ep.ldc + col0;
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              if (col0 + j < N) {
-                int4 pk;
-                pk.x = (int)pack_bf16x2(v[j], v[j + 1]); pk.y = (int)pack_bf16x2(v[j + 2], v[j + 3]);
-                pk.z = (int)pack_bf16x2(v[j + 4], v[j + 5]); pk.w = (int)pack_bf16x2(v[j + 6], v[j + 7]);
-                *reinterpret_cast<int4*>(dst + j) = pk;
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
-}
-
-template <int BN>
-int launch_fp8(const CUtensorMap& ta, const void* B, int M, int N, int K, int64_t ldb, const Epi8& ep, cudaStream_t s) {
-  using L = Smem8<BN>;
-  CUtensorMap tb;
-  int rc = make_tmap_u8(&tb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, BLOCK_K8, BN);
-  if (rc) return rc;
-  static DrPerDeviceOnce attr_once; bool& attr = attr_once();
-  if (!attr) { DR_CUDA_CHECK(cudaFuncSetAttribute(k_gemm_fp8_tn<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal)); attr = true; }
-  const int tiles = ((M + BLOCK_M - 1) / BLOCK_M) * ((N + BN - 1) / BN);
-  const int grid = tiles < kNumSMs ? tiles : kNumSMs;
-  k_gemm_fp8_tn<BN><<<grid, kThreads8, L::kTotal, s>>>(ta, tb, M, N, K, ep);
-  DR_LAUNCH_CHECK();
-  return 0;
 }
 
 // x [M, C] (fp32 or bf16) * inv_scale -> e4m3 [M, Cp] (zero padded columns), 16 outputs per thread
@@ -302,26 +67,10 @@ __global__ void k_absmax(const __nv_bfloat16* __restrict__ x, int64_t n, float* 
 
 extern "C" {
 
-// out[M,N] = (A[M,K] B[N,K]^T) * col_scale + bias (relu).  A, B: e4m3, K-major, lda/ldb multiples of 16 bytes; N % 16 == 0.
-int dr_cuda_gemm_fp8_tn(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* col_scale, const float* bias,
-                        int relu, void* out, int64_t ldc, int out_fp8, float out_inv_scale, cudaStream_t s) {
-  if (M <= 0 || N <= 0 || K <= 0) return 0;
-  if ((lda % 16) || (ldb % 16) || (N % 16) || (ldc % 8) || (out_fp8 && (ldc % 16))) return -2;
-  CUtensorMap ta;
-  int rc = make_tmap_u8(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BLOCK_K8, BLOCK_M);
-  if (rc) return rc;
-  Epi8 ep{col_scale, bias, out, ldc, relu, out_fp8, out_inv_scale};
-  if (N <= 16) return launch_fp8<16>(ta, B, M, N, K, ldb, ep, s);
-  if (N <= 32) return launch_fp8<32>(ta, B, M, N, K, ldb, ep, s);
-  if (N <= 64) return launch_fp8<64>(ta, B, M, N, K, ldb, ep, s);
-  if (N <= 128 || M <= 128 * kNumSMs / 4) return launch_fp8<128>(ta, B, M, N, K, ldb, ep, s);   // small M: more, narrower tiles fill the SMs
-  return launch_fp8<256>(ta, B, M, N, K, ldb, ep, s);
-}
-
 int dr_cuda_quantize_e4m3(const void* x, int is_bf16, int64_t M, int C, int64_t ldx, void* y, int Cp, float inv_scale, cudaStream_t s) {
   if (Cp % 16) return -2;
   const int64_t total = M * (Cp / 16);
-  int grid = (int)((total + 255) / 256); if (grid < 1) grid = 1; if (grid > kNumSMs * 8) grid = kNumSMs * 8;
+  int grid = (int)((total + 255) / 256); if (grid < 1) grid = 1; if (grid > num_sms() * 8) grid = num_sms() * 8;
   if (is_bf16) k_quantize_e4m3<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, M, C, ldx, (uint8_t*)y, Cp, inv_scale);
   else k_quantize_e4m3<float><<<grid, 256, 0, s>>>((const float*)x, M, C, ldx, (uint8_t*)y, Cp, inv_scale);
   DR_LAUNCH_CHECK();
@@ -337,7 +86,7 @@ int dr_cuda_quantize_weights_e4m3(const float* w, int N, int K, int64_t ldw, voi
 
 int dr_cuda_absmax_bf16(const void* x, int64_t n, float* out, cudaStream_t s) {
   DR_CUDA_CHECK(cudaMemsetAsync(out, 0, 4, s));
-  int grid = (int)((n + 255) / 256); if (grid < 1) grid = 1; if (grid > kNumSMs * 4) grid = kNumSMs * 4;
+  int grid = (int)((n + 255) / 256); if (grid < 1) grid = 1; if (grid > num_sms() * 4) grid = num_sms() * 4;
   k_absmax<<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, n, out);
   DR_LAUNCH_CHECK();
   return 0;

@@ -1,252 +1,10 @@
-// Block-scaled FP8 (MXFP8: E4M3 elements, one UE8M0 scale per 32 elements along K) tcgen05 GEMM for the MLP path:
-//
-//     D[M,N] = sum_kb32 ( 2^(sfa[m,kb32] - 127) * 2^(sfb[n,kb32] - 127) * A_q[m, kb32] . B_q[n, kb32] )  + bias[n]   (ReLU)   -> bf16
-//
-// `tcgen05.mma.kind::mxf8f6f4.block_scale`: the tensor core applies both scale factors per 32-wide k block inside the MMA, so
-// neither operand needs a calibrated per-tensor scale (the static-scale `kind::f8f6f4` path of gemm_fp8.cu does) and the
-// epilogue has no scale multiply.  Scale factors travel global -> shared (one 512 B `cp.async.bulk` per 128 rows per 128-wide
-// k block, on the same mbarrier as the operand tiles) -> TMEM (`tcgen05.cp.32x128b.warpx4`, issued by the MMA thread right before
-// the four MMAs that use them; the 4 bytes of one 32-bit TMEM column are the 4 k sub-blocks, selected by the a_sf_id / b_sf_id
-// fields of the instruction descriptor).  The quantiser (k_quantize_mxfp8) writes the scale words directly in the order the
-// tcgen05.cp wants (word (r % 32) * 4 + r / 32 for row r of a 128-row block), so the GEMM kernel needs no transposer warp.
-//
-// Same warp-specialised persistent structure as k_gemm_fp8_tn: warp 0 TMA producer, warp 1 MMA issuer, warps 2-5 epilogue,
-// double-buffered TMEM accumulators (2 x 128 columns) + 4 columns SFA + 4 columns SFB.
-//
-// Reference: none -- DeepRec's low-precision story is tools/low_precision_optimize (BF16 / FP16 / INT8 graph rewrite over library
-// kernels, SURVEY §2.9); BASELINE.json names block-scaled fp8 on the MLP path as part of the B200 north star.
-// Opt-in; written after the round's GPU budget was spent: first hardware run is tests/test_gpu_zzzzzzz_mxfp8.py.
-#include <cuda.h>
-#include <cuda_fp8.h>
-
+// MXFP8 (block-scaled fp8) quantiser: E4M3 elements with one UE8M0 power-of-two scale per 32 elements along K.  The block-scaled GEMM
+// that consumes its output is dr_cuda_gemm_mxfp8_tn (gemm_wgmma.cu: one m64nNk32 wgmma per scale block, scales applied in registers).
 #include "common.cuh"
 
 using namespace drc;
 
 namespace {
-
-constexpr int BLOCK_M = 128;
-constexpr int BLOCK_N = 128;
-constexpr int BLOCK_KX = 128;        // 128 fp8 = one swizzle-128B row = 4 scale blocks of 32
-constexpr int UMMA_KX = 32;
-constexpr int kStagesX = 5;
-constexpr int kThreadsX = 192;
-constexpr int kSfBytes = 128 * 4;    // one uint32 (4 UE8M0 bytes) per row of a 128-row block per 128-wide k block
-constexpr uint32_t kTmemColsX = 512; // 2 x 128 accumulator columns + 4 (SFA) + 4 (SFB) -> next power of two
-constexpr uint32_t kSfaCol = 2 * BLOCK_N, kSfbCol = 2 * BLOCK_N + 4;
-
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-PFN_encodeTiled get_encode_x() {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (PFN_encodeTiled)p;
-  }
-  return fn;
-}
-
-int make_tmap_x(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, uint64_t pitch_bytes, uint32_t box_inner, uint32_t box_outer) {
-  PFN_encodeTiled enc = get_encode_x();
-  if (!enc) return -100;
-  cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {pitch_bytes};
-  cuuint32_t box[2] = {box_inner, box_outer};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : -101 - (int)r;
-}
-
-// InstrDescriptorBlockScaled (cute/arch/mma_sm100_desc.hpp): [4,6) b_sf_id | [7,10) a_format = 0 (E4M3) | [10,13) b_format = 0 |
-// 15 / 16 a / b major = 0 (K-major) | [17,23) N >> 3 | 23 scale_format = 1 (UE8M0) | [24,29) M >> 4 | [29,31) a_sf_id | 31 k_size = 0 (K = 32)
-__host__ __device__ constexpr uint32_t umma_idesc_mxf8(int M, int N, uint32_t sf_id) {
-  return (sf_id << 4) | ((uint32_t)(N >> 3) << 17) | (1u << 23) | ((uint32_t)(M >> 4) << 24) | (sf_id << 29);
-}
-
-__device__ __forceinline__ void umma_mxf8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate, uint32_t tmem_sfa,
-                                          uint32_t tmem_sfb) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(tmem_sfa), "r"(tmem_sfb) : "memory");
-}
-// shared -> TMEM: 32 rows x 128 bit, replicated into the 4 lane quarters (the scale-factor operand layout)
-__device__ __forceinline__ void tmem_cp_32x128b_warpx4(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-// un-swizzled K-major descriptor of a [32 rows x 16 B] scale block: 8-row atoms of 128 B (SBO), one atom along K (LBO unused)
-__device__ __forceinline__ uint64_t sf_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(128 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
-struct EpiX {
-  const float* bias;   // [N] or null
-  __nv_bfloat16* out;  // [M, ldc]
-  int64_t ldc;
-  int relu;
-};
-
-struct SmemX {
-  static constexpr int kABytes = BLOCK_M * BLOCK_KX;
-  static constexpr int kBBytes = BLOCK_N * BLOCK_KX;
-  static constexpr int kStageBytes = kABytes + kBBytes + 2 * kSfBytes;      // 33792: stage bases stay 1024-aligned
-  static constexpr int kTotal = kStagesX * kStageBytes + 1024 + 256;
-};
-
-__global__ void __launch_bounds__(kThreadsX, 1)
-k_gemm_mxfp8_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const uint32_t* __restrict__ sfa,
-                const uint32_t* __restrict__ sfb, int M, int N, int K, EpiX ep) {
-  using L = SmemX;
-  static_assert(L::kStageBytes % 1024 == 0, "swizzle-128B tiles need 1024 B aligned bases");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStagesX * L::kStageBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + kStagesX;
-  uint64_t* tfull_bar = bars + 2 * kStagesX;
-  uint64_t* tempty_bar = bars + 2 * kStagesX + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * kStagesX + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-  const int n_tiles = (N + BLOCK_N - 1) / BLOCK_N;
-  const int num_tiles = m_tiles * n_tiles;
-  const int num_kb = (K + BLOCK_KX - 1) / BLOCK_KX;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < kStagesX; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 4); }
-    fence_mbar_init();
-  }
-  if (warp == 1) { tmem_alloc(tmem_ptr, kTmemColsX); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ================= producer: operand tiles by TMA, the two scale blocks by 1-D bulk copies, one barrier =================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * L::kStageBytes;
-          uint8_t* sb = sa + L::kABytes;
-          uint8_t* ssfa = sb + L::kBBytes;
-          uint8_t* ssfb = ssfa + kSfBytes;
-          mbar_expect_tx(&full_bar[stage], L::kStageBytes);
-          tma_load_2d(sa, &tmA, &full_bar[stage], kb * BLOCK_KX, m_blk * BLOCK_M);
-          tma_load_2d(sb, &tmB, &full_bar[stage], kb * BLOCK_KX, n_blk * BLOCK_N);
-          bulk_load_1d(ssfa, sfa + ((int64_t)m_blk * num_kb + kb) * 128, kSfBytes, &full_bar[stage]);
-          bulk_load_1d(ssfb, sfb + ((int64_t)n_blk * num_kb + kb) * 128, kSfBytes, &full_bar[stage]);
-          if (++stage == kStagesX) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer: scale blocks smem -> TMEM, then 4 block-scaled MMAs (K = 32 each) per stage =================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * L::kStageBytes);
-          const uint32_t sb = sa + L::kABytes;
-          const uint32_t ssfa = sb + L::kBBytes, ssfb = ssfa + kSfBytes;
-          // tcgen05.cp / tcgen05.mma of one thread execute in issue order: the copies below wait for the previous stage's MMAs
-          // (which read the same TMEM columns) and the MMAs after them see the new scales.
-          tmem_cp_32x128b_warpx4(tmem_base + kSfaCol, sf_desc(ssfa));
-          tmem_cp_32x128b_warpx4(tmem_base + kSfbCol, sf_desc(ssfb));
-          const uint64_t adesc = umma_desc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = umma_desc_sw128(sb, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < BLOCK_KX / UMMA_KX; ++k)       // +32 B inside the swizzle atom per K = 32 step; scale byte k of the column
-            umma_mxf8(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), umma_idesc_mxf8(BLOCK_M, BLOCK_N, (uint32_t)k), (kb | k) != 0,
-                      tmem_base + kSfaCol, tmem_base + kSfbCol);
-          umma_commit(&empty_bar[stage]);
-          if (kb == num_kb - 1) umma_commit(&tfull_bar[acc]);
-          if (++stage == kStagesX) { stage = 0; phase ^= 1; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else {
-    // ================= epilogue: TMEM -> registers -> (+bias)(ReLU) -> bf16 =================
-    const int q = warp & 3;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const int row = m_blk * BLOCK_M + q * 32 + lane;
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BLOCK_N;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(t_row + c0, r);
-        tmem_ld_wait();
-        const int col0 = n_blk * BLOCK_N + c0;
-        if (row < M && col0 < N) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (ep.bias && col0 + j < N) b = *reinterpret_cast<const float4*>(ep.bias + col0 + j);
-            v[j] = __uint_as_float(r[j]) + b.x; v[j + 1] = __uint_as_float(r[j + 1]) + b.y;
-            v[j + 2] = __uint_as_float(r[j + 2]) + b.z; v[j + 3] = __uint_as_float(r[j + 3]) + b.w;
-          }
-          if (ep.relu) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-          __nv_bfloat16* dst = ep.out + (int64_t)row * ep.ldc + col0;
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            if (col0 + j < N) {       // N is a multiple of 8 (checked on the host)
-              int4 pk;
-              pk.x = (int)pack_bf16x2(v[j], v[j + 1]); pk.y = (int)pack_bf16x2(v[j + 2], v[j + 3]);
-              pk.z = (int)pack_bf16x2(v[j + 4], v[j + 5]); pk.w = (int)pack_bf16x2(v[j + 6], v[j + 7]);
-              *reinterpret_cast<int4*>(dst + j) = pk;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemColsX);
-}
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // Quantiser: x [R, C] (fp32 or bf16, row pitch ldx) -> q [R, Kp] E4M3 (Kp = C rounded up to 128, zero padded) + scale words.
@@ -290,6 +48,7 @@ __global__ void k_quantize_mxfp8(const T* __restrict__ x, int64_t R, int C, int6
   if (lane == 0) sf[((r >> 7) * num_kb + kb) * 128 + (r & 31) * 4 + ((r & 127) >> 5)] = b0 | (b1 << 8) | (b2 << 16) | (b3 << 24);
 }
 
+
 }  // namespace
 
 extern "C" {
@@ -305,28 +64,6 @@ int dr_cuda_quantize_mxfp8(const void* x, int is_bf16, int64_t R, int C, int64_t
     k_quantize_mxfp8<__nv_bfloat16><<<(unsigned)blocks, 256, 0, s>>>((const __nv_bfloat16*)x, R, C, ldx, (uint8_t*)q, Kp, (uint32_t*)sf);
   else
     k_quantize_mxfp8<float><<<(unsigned)blocks, 256, 0, s>>>((const float*)x, R, C, ldx, (uint8_t*)q, Kp, (uint32_t*)sf);
-  DR_LAUNCH_CHECK();
-  return 0;
-}
-
-// out[M,N] (bf16, ldc) = blockscaled(A_q[M,Kp], sfa) * blockscaled(B_q[N,Kp], sfb)^T (+bias)(relu).  A_q / B_q: e4m3, K-major, row pitch
-// Kp (multiple of 128); sfa / sfb: scale words in the quantiser's layout; N % 8 == 0.
-int dr_cuda_gemm_mxfp8_tn(const void* A, const void* sfa, const void* B, const void* sfb, int M, int N, int Kp, const float* bias, int relu, void* out,
-                          int64_t ldc, int max_ctas, cudaStream_t s) {
-  if (M <= 0 || N <= 0 || Kp <= 0) return 0;
-  if ((Kp % 128) || (N % 8) || (ldc % 8)) return -2;
-  CUtensorMap ta, tb;
-  int rc = make_tmap_x(&ta, A, (uint64_t)Kp, (uint64_t)M, (uint64_t)Kp, BLOCK_KX, BLOCK_M);
-  if (rc) return rc;
-  rc = make_tmap_x(&tb, B, (uint64_t)Kp, (uint64_t)N, (uint64_t)Kp, BLOCK_KX, BLOCK_N);
-  if (rc) return rc;
-  static DrPerDeviceOnce attr_once; bool& attr = attr_once();
-  if (!attr) { DR_CUDA_CHECK(cudaFuncSetAttribute(k_gemm_mxfp8_tn, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemX::kTotal)); attr = true; }
-  EpiX ep{bias, (__nv_bfloat16*)out, ldc, relu};
-  if (max_ctas <= 0) max_ctas = kNumSMs;
-  const int tiles = ((M + BLOCK_M - 1) / BLOCK_M) * ((N + BLOCK_N - 1) / BLOCK_N);
-  const int grid = tiles < max_ctas ? tiles : max_ctas;
-  k_gemm_mxfp8_tn<<<grid, kThreadsX, SmemX::kTotal, s>>>(ta, tb, (const uint32_t*)sfa, (const uint32_t*)sfb, M, N, Kp, ep);
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -6,7 +6,7 @@
 // modelzoo/din/train.py:143-188.  The interaction is a batch of 27x16 Gram matrices -- 23 kFLOP per sample
 // against 1.6 kB of traffic -- so it is HBM-bound by two orders of magnitude; it reads the embedding rows
 // exactly once, straight from the (peer-written) feature-major receive buffer, and emits the padded bf16
-// activation the tcgen05 top-MLP GEMM consumes through TMA.
+// activation the wgmma top-MLP GEMM consumes through TMA.
 #include "sp_sync.cuh"
 
 using namespace drc;
@@ -182,25 +182,19 @@ __global__ void __launch_bounds__(256) k_fm_bwd(const __nv_bfloat16* __restrict_
 }
 
 
-#ifndef DR_CUDA_EMU   // tcgen05 / TMEM: hardware only (the emulation build runs the SIMT kernels above for every shape)
+#ifndef DR_CUDA_EMU   // warp-level tensor-core MMA: hardware only (the emulation build runs the SIMT kernels above for every shape)
 // =================================================================================================
-// tcgen05 versions (D = 16, T + 1 <= 32): FOUR samples share one 128-row UMMA tile.
-//   forward :  G = A A^T with A[128 x 16] = 4 samples x 32 (padded) feature rows.  One tcgen05.mma (M=128, N=128, K=16)
-//              per 4 samples; warp w reads the w-th diagonal 32x32 block of the accumulator straight out of TMEM
-//              (tcgen05.ld 32x32b: lane i <- row i of its sample's Gram matrix) and emits the strict lower triangle.
-//   backward:  dF = S F with S the symmetric 32x32 gradient matrix of a sample; A = blockdiag(S_0..S_3) [128 x 128],
-//              B = F^T [16 x 128]; eight tcgen05.mma k-steps (M=128, N=16, K=128); lane i of warp w <- dF_i.
-// Operands are written by the warps into NO-SWIZZLE K-major core-matrix layout (8 rows x 16 B core matrices,
-// LBO = next 8-element K chunk, SBO = next 8-row group), accumulators live in TMEM.  The SIMT kernels above remain
-// as the general-shape fallback.
+// Tensor-core versions (D = 16, T + 1 <= 32): one warp per sample, the sample's 32 (padded) feature rows staged in shared memory.
+//   forward :  G = F F^T [32 x 32 x 16] with six mma.sync.m16n8k16 (the 16 x 8 tiles on or below the diagonal); every lane scatters
+//              the strict lower-triangle elements of its accumulator fragments into the sample's Z row.
+//   backward:  dF = S F [32 x 16 x 32] with S the symmetric 32 x 32 gradient matrix of the sample (eight mma.sync.m16n8k16);
+//              lane i then owns dF_i.
+// The SIMT kernels above remain as the general-shape fallback.
 // =================================================================================================
-__device__ __forceinline__ uint64_t umma_desc_noswz(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;            // descriptor version (sm_100)
-  return d;                          // layout_type = 0 (SWIZZLE_NONE)
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 // INDIRECT: `emb` is the requester-side unique-row buffer urow[gs][16] (written by the owners over NVLink) and feature t of sample b
@@ -213,38 +207,23 @@ __global__ void __launch_bounds__(128) k_dot_fwd_tc(const __nv_bfloat16* __restr
   pdl_sync();
   if (INDIRECT) sp_wait_all(sync, SP_CH_ROWS);
   constexpr int D = 16;
-  __shared__ __align__(128) uint8_t sA[128 * 32];          // [16 row-groups][2 K-chunks][8 rows][16 B]
+  __shared__ __align__(16) uint8_t sF[4][32 * 32];           // per warp: [32 feature rows][16 bf16]
   __shared__ __align__(16) __nv_bfloat16 sZ[4][512];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_slot;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int gI = lane >> 2, tI = lane & 3;                    // mma.sync fragment coordinates
   const int F = T + 1;
-  for (int i = threadIdx.x; i < 128 * 32 / 16; i += 128) reinterpret_cast<int4*>(sA)[i] = make_int4(0, 0, 0, 0);
-  if (threadIdx.x == 0) { mbar_init(&bar, 1); fence_mbar_init(); }
-  if (warp == 0) { tmem_alloc(&tmem_slot, 128); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t a_addr = smem_u32(sA);
-  const uint64_t desc = umma_desc_noswz(a_addr, 128, 256);
-  constexpr uint32_t idesc = umma_idesc_bf16(128, 128, 0, 0);
-  const int R = warp * 32 + lane;                                  // my row in the tile
-  uint8_t* my_row = sA + (R >> 3) * 256 + (R & 7) * 16;
-  const int64_t ngroups = (B + 3) / 4;
-  uint32_t phase = 0;
-  // software pipeline: the rows of group g+1 are fetched into registers while group g is in the tensor core / epilogue
+  uint8_t* myF = sF[warp];
+  const int64_t stride = (int64_t)gridDim.x * 4;
+  // software pipeline: the row of sample b + stride is fetched into registers while sample b is in the tensor core / epilogue
   int4 c0 = make_int4(0, 0, 0, 0), c1 = c0;
-  int32_t gsn = -1;                                   // INDIRECT: row index of my feature for the NEXT group to fetch
-  auto fetch_idx = [&](int64_t gg) {
-    const int64_t bb = gg * 4 + warp;
-    gsn = (gg < ngroups && lane >= 1 && lane < F && bb < B) ? inv[bb * ldinv + lane - 1] : -1;
+  int32_t gsn = -1;                                   // INDIRECT: row index of my feature for the NEXT sample to fetch
+  auto fetch_idx = [&](int64_t bb) {
+    gsn = (lane >= 1 && lane < F && bb < B) ? inv[bb * ldinv + lane - 1] : -1;
   };
-  auto fetch = [&](int64_t gg, int4& r0, int4& r1) {
-    const int64_t bb = gg * 4 + warp;
-    if (gg < ngroups && lane < F && bb < B) {
+  auto fetch = [&](int64_t bb, int4& r0, int4& r1) {
+    r0 = r1 = make_int4(0, 0, 0, 0);
+    if (lane < F && bb < B) {
       if (INDIRECT) {
-        r0 = r1 = make_int4(0, 0, 0, 0);
         if (lane == 0) { r0 = ld_nc_v4(x + bb * ldx); r1 = ld_nc_v4(x + bb * ldx + 8); }
         else if (gsn >= 0) { const __nv_bfloat16* src = emb + (int64_t)gsn * D; r0 = ld_v4_volatile(src); r1 = ld_v4_volatile(src + 8); }
       } else {
@@ -253,61 +232,62 @@ __global__ void __launch_bounds__(128) k_dot_fwd_tc(const __nv_bfloat16* __restr
       }
     }
     if (INDIRECT) {
-      fetch_idx(gg + gridDim.x);                      // index of the group after this one: in flight for a whole iteration
+      fetch_idx(bb + stride);                         // index of the sample after this one: in flight for a whole iteration
     } else {
-      // two more groups ahead: L2 prefetch only (one group of register loads per warp cannot cover the DRAM latency)
-      const int64_t pb = (gg + 2 * (int64_t)gridDim.x) * 4 + warp;
+      // two more samples ahead: L2 prefetch only (one sample of register loads per warp cannot cover the DRAM latency)
+      const int64_t pb = bb + 2 * stride;
       if (lane < F && pb < B) prefetch_l2(lane == 0 ? x + pb * ldx : emb + (int64_t)(lane - 1) * emb_stride_t + pb * emb_stride_b);
     }
   };
-  if (INDIRECT) fetch_idx(blockIdx.x);
-  fetch(blockIdx.x, c0, c1);
-  for (int64_t g = blockIdx.x; g < ngroups; g += gridDim.x) {
-    const int64_t b = g * 4 + warp;
-    const bool live = b < B;
-    if (lane < F && live) {
-      *reinterpret_cast<int4*>(my_row) = c0;
-      *reinterpret_cast<int4*>(my_row + 128) = c1;
-      if (lane == 0) { *reinterpret_cast<int4*>(&sZ[warp][0]) = c0; *reinterpret_cast<int4*>(&sZ[warp][8]) = c1; }
-    }
-    fetch(g + gridDim.x, c0, c1);
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      tc_fence_after();
-      umma_bf16(tmem, desc, desc, idesc, 0u);
-      umma_commit(&bar);
-    }
-    mbar_wait(&bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    uint32_t r[32];
-    tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + warp * 32, r);
-    tmem_ld_wait();
-    if (live) {
-      const int base = D + lane * (lane - 1) / 2;
+  const int64_t first = (int64_t)blockIdx.x * 4 + warp;
+  if (INDIRECT) fetch_idx(first);
+  fetch(first, c0, c1);
+  for (int64_t b = first; b < B; b += stride) {
+    *reinterpret_cast<int4*>(myF + lane * 32) = c0;
+    *reinterpret_cast<int4*>(myF + lane * 32 + 16) = c1;
+    if (lane == 0) { *reinterpret_cast<int4*>(&sZ[warp][0]) = c0; *reinterpret_cast<int4*>(&sZ[warp][8]) = c1; }
+    fetch(b + stride, c0, c1);
+    __syncwarp();
+    uint32_t af[2][4], bf[4][2];
 #pragma unroll
-      for (int j = 0; j < 31; ++j)
-        if (j < lane && lane < F) sZ[warp][base + j] = __float2bfloat16(__uint_as_float(r[j]));
-      const int used = D + F * (F - 1) / 2;
-      for (int c = used + lane; c < ldz; c += 32) sZ[warp][c] = __float2bfloat16(0.f);
-      __syncwarp();
-      for (int c = lane * 8; c < ldz; c += 256)
-        *reinterpret_cast<int4*>(Z + b * ldz + c) = *reinterpret_cast<const int4*>(&sZ[warp][c]);
+    for (int mi = 0; mi < 2; ++mi) {
+      const uint8_t* r0 = myF + (16 * mi + gI) * 32 + 4 * tI;
+      af[mi][0] = *reinterpret_cast<const uint32_t*>(r0);
+      af[mi][1] = *reinterpret_cast<const uint32_t*>(r0 + 8 * 32);
+      af[mi][2] = *reinterpret_cast<const uint32_t*>(r0 + 16);
+      af[mi][3] = *reinterpret_cast<const uint32_t*>(r0 + 8 * 32 + 16);
     }
-    tc_fence_before();
-    __syncthreads();          // all TMEM reads + smem tile reads done before the next group overwrites them
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni) {
+      const uint8_t* r0 = myF + (8 * ni + gI) * 32 + 4 * tI;
+      bf[ni][0] = *reinterpret_cast<const uint32_t*>(r0);
+      bf[ni][1] = *reinterpret_cast<const uint32_t*>(r0 + 16);
+    }
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi) {
+#pragma unroll
+      for (int ni = 0; ni < 4; ++ni) {
+        if (8 * ni > 16 * mi + 15) continue;            // tile entirely above the diagonal (compile-time)
+        float c[4] = {0.f, 0.f, 0.f, 0.f};
+        mma_bf16_16816(c, af[mi], bf[ni][0], bf[ni][1]);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int fi = 16 * mi + gI + 8 * (e >> 1), j = 8 * ni + 2 * tI + (e & 1);
+          if (j < fi && fi < F) sZ[warp][D + fi * (fi - 1) / 2 + j] = __float2bfloat16(c[e]);
+        }
+      }
+    }
+    const int used = D + F * (F - 1) / 2;
+    for (int c = used + lane; c < ldz; c += 32) sZ[warp][c] = __float2bfloat16(0.f);
+    __syncwarp();
+    for (int c = lane * 8; c < ldz; c += 256)
+      *reinterpret_cast<int4*>(Z + b * ldz + c) = *reinterpret_cast<const int4*>(&sZ[warp][c]);
+    __syncwarp();                                      // the staging tiles are rewritten by the next sample
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 128);
 }
 
 // INDIRECT: features come from urow[inv[b][t]] (unique-first pipeline); the per-sample gradient rows still go to the feature-major
-// demb buffer, which k_sp_segsum (sparse_pipeline.cu) pre-reduces per distinct key on the side stream.  (A first version reduced
-// them here with shared-memory fp32 atomics: those compile to ATOMS.CAST.SPIN loops and made this kernel 2.6x slower -- see
-// profiles/r2_notes.md.)
+// demb buffer, which k_sp_segsum (sparse_pipeline.cu) pre-reduces per distinct key on the side stream.
 template <bool INDIRECT>
 __global__ void __launch_bounds__(128) k_dot_bwd_tc(const __nv_bfloat16* __restrict__ dZ, int64_t ldz, const __nv_bfloat16* __restrict__ x,
                                                     int64_t ldx, const __nv_bfloat16* __restrict__ emb, int64_t emb_stride_t,
@@ -316,40 +296,24 @@ __global__ void __launch_bounds__(128) k_dot_bwd_tc(const __nv_bfloat16* __restr
                                                     const int32_t* __restrict__ inv, int ldinv) {
   pdl_sync();
   constexpr int D = 16;
-  extern __shared__ __align__(128) uint8_t dyn[];
-  uint8_t* sA = dyn;                                   // blockdiag(S): [16 row-groups][16 K-chunks][8 rows][16 B] = 32 KB
-  uint8_t* sB = dyn + 32768;                           // F^T: [2 d-groups][16 K-chunks][8 d][16 B] = 4 KB
-  __nv_bfloat16* sG = reinterpret_cast<__nv_bfloat16*>(dyn + 32768 + 4096);   // [4][512] dZ rows
-
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(16) __nv_bfloat16 sG[4][512];         // per warp: the sample's dZ row
+  __shared__ __align__(16) __nv_bfloat16 sS[4][32 * 32];     // per warp: S row-major [i][j]
+  __shared__ __align__(16) __nv_bfloat16 sFt[4][16 * 32];    // per warp: F^T [d][j]
+  __shared__ __align__(16) float sO[4][32 * 17];             // per warp: dF [i][d] (padded rows)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int gI = lane >> 2, tI = lane & 3;
   const int F = T + 1;
-  for (int i = threadIdx.x; i < (32768 + 4096) / 16; i += 128) reinterpret_cast<int4*>(dyn)[i] = make_int4(0, 0, 0, 0);
-  if (threadIdx.x == 0) { mbar_init(&bar, 1); fence_mbar_init(); }
-  if (warp == 0) { tmem_alloc(&tmem_slot, 32); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint64_t adesc = umma_desc_noswz(smem_u32(sA), 128, 2048);
-  const uint64_t bdesc = umma_desc_noswz(smem_u32(sB), 128, 2048);
-  constexpr uint32_t idesc = umma_idesc_bf16(128, 16, 0, 0);
-  const int R = warp * 32 + lane;
-  __nv_bfloat16* myG = sG + warp * 512;
-  const int64_t ngroups = (B + 3) / 4;
-  uint32_t phase = 0;
-  // software pipeline: dZ chunks + the feature row of group g+1 are fetched while group g is being processed
+  __nv_bfloat16* myG = sG[warp];
+  const int64_t stride = (int64_t)gridDim.x * 4;
+  // software pipeline: dZ chunks + the feature row of sample b + stride are fetched while sample b is being processed
   int4 pz0 = make_int4(0, 0, 0, 0), pz1 = pz0, pf0 = pz0, pf1 = pz0;
-  int32_t gsn = -1;                                   // INDIRECT: row index of my feature for the NEXT group to fetch
-  auto fetch_idx = [&](int64_t gg) {
-    const int64_t bb = gg * 4 + warp;
-    gsn = (gg < ngroups && lane >= 1 && lane < F && bb < B) ? inv[bb * ldinv + lane - 1] : -1;
+  int32_t gsn = -1;                                   // INDIRECT: row index of my feature for the NEXT sample to fetch
+  auto fetch_idx = [&](int64_t bb) {
+    gsn = (lane >= 1 && lane < F && bb < B) ? inv[bb * ldinv + lane - 1] : -1;
   };
-  auto fetch = [&](int64_t gg) {
-    const int64_t bb = gg * 4 + warp;
+  auto fetch = [&](int64_t bb) {
     pz0 = pz1 = pf0 = pf1 = make_int4(0, 0, 0, 0);
-    if (gg < ngroups && bb < B) {
+    if (bb < B) {
       if (lane * 8 < ldz) pz0 = ld_nc_v4(dZ + bb * ldz + lane * 8);
       if (lane * 8 + 256 < ldz) pz1 = ld_nc_v4(dZ + bb * ldz + lane * 8 + 256);
       if (lane < F) {
@@ -365,37 +329,32 @@ __global__ void __launch_bounds__(128) k_dot_bwd_tc(const __nv_bfloat16* __restr
         }
       }
     }
-    if (INDIRECT) fetch_idx(gg + gridDim.x);
-    // two more groups ahead: L2 prefetch only (one group of register loads per warp cannot cover the DRAM latency)
-    const int64_t pb = (gg + 2 * (int64_t)gridDim.x) * 4 + warp;
+    if (INDIRECT) fetch_idx(bb + stride);
+    // two more samples ahead: L2 prefetch only (one sample of register loads per warp cannot cover the DRAM latency)
+    const int64_t pb = bb + 2 * stride;
     if (pb < B) {
       if (lane * 8 < ldz) prefetch_l2(dZ + pb * ldz + lane * 8);
       if (lane * 8 + 256 < ldz) prefetch_l2(dZ + pb * ldz + lane * 8 + 256);
       if (!INDIRECT && lane < F) prefetch_l2(lane == 0 ? x + pb * ldx : emb + (int64_t)(lane - 1) * emb_stride_t + pb * emb_stride_b);
     }
   };
-  if (INDIRECT) fetch_idx(blockIdx.x);
-  fetch(blockIdx.x);
-  for (int64_t g = blockIdx.x; g < ngroups; g += gridDim.x) {
-    const int64_t b = g * 4 + warp;
-    const bool live = b < B;
-    // ---- stage dZ row and F^T from the prefetched registers
+  const int64_t first = (int64_t)blockIdx.x * 4 + warp;
+  if (INDIRECT) fetch_idx(first);
+  fetch(first);
+  for (int64_t b = first; b < B; b += stride) {
+    // ---- stage the dZ row and F^T from the prefetched registers (lanes >= F hold zeros)
     if (lane * 8 < ldz) *reinterpret_cast<int4*>(myG + lane * 8) = pz0;
     if (lane * 8 + 256 < ldz) *reinterpret_cast<int4*>(myG + lane * 8 + 256) = pz1;
-    if (lane < F) {
+    {
       const int4 c0 = pf0, c1 = pf1;
       const uint32_t w[8] = {(uint32_t)c0.x, (uint32_t)c0.y, (uint32_t)c0.z, (uint32_t)c0.w, (uint32_t)c1.x, (uint32_t)c1.y, (uint32_t)c1.z, (uint32_t)c1.w};
-      // B[n = d][k = R] at (d/8)*2048 + (R/8)*128 + (d%8)*16 + (R%8)*2
-      uint8_t* colbase = sB + (R >> 3) * 128 + (R & 7) * 2;
+      uint16_t* ft = reinterpret_cast<uint16_t*>(sFt[warp]);
 #pragma unroll
-      for (int d = 0; d < 16; ++d) {
-        const uint16_t v = (d & 1) ? (uint16_t)(w[d >> 1] >> 16) : (uint16_t)(w[d >> 1] & 0xFFFF);
-        *reinterpret_cast<uint16_t*>(colbase + (d >> 3) * 2048 + (d & 7) * 16) = v;
-      }
+      for (int d = 0; d < 16; ++d) ft[d * 32 + lane] = (d & 1) ? (uint16_t)(w[d >> 1] >> 16) : (uint16_t)(w[d >> 1] & 0xFFFF);
     }
-    fetch(g + gridDim.x);
+    fetch(b + stride);
     __syncwarp();
-    // ---- my row of S (32 columns of the diagonal block): S[i][j] = dG[max][min], zero on the diagonal / padding
+    // ---- my row of S: S[i][j] = dG[max][min], zero on the diagonal / padding
     {
       uint32_t packed[16];
 #pragma unroll
@@ -408,32 +367,36 @@ __global__ void __launch_bounds__(128) k_dot_bwd_tc(const __nv_bfloat16* __restr
         }
         packed[jj] = lo | (hi << 16);
       }
-      // A[R][C = 32*warp + j] at (R/8)*2048 + (C/8)*128 + (R%8)*16 + (C%8)*2
-      uint8_t* rowbase = sA + (R >> 3) * 2048 + (warp * 4) * 128 + (R & 7) * 16;
+      int4* row = reinterpret_cast<int4*>(sS[warp] + lane * 32);
 #pragma unroll
-      for (int c = 0; c < 4; ++c)
-        *reinterpret_cast<int4*>(rowbase + c * 128) = make_int4((int)packed[4 * c], (int)packed[4 * c + 1], (int)packed[4 * c + 2], (int)packed[4 * c + 3]);
+      for (int c = 0; c < 4; ++c) row[c] = make_int4((int)packed[4 * c], (int)packed[4 * c + 1], (int)packed[4 * c + 2], (int)packed[4 * c + 3]);
     }
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      tc_fence_after();
+    __syncwarp();
+    // ---- dF = S F on the tensor cores
+    const uint8_t* S8 = reinterpret_cast<const uint8_t*>(sS[warp]);
+    const uint8_t* Ft8 = reinterpret_cast<const uint8_t*>(sFt[warp]);
 #pragma unroll
-      for (int k = 0; k < 8; ++k)     // 16 K elements = 2 chunks = 256 B  -> +16 in the (addr >> 4) field
-        umma_bf16(tmem, adesc + (uint64_t)(k * 16), bdesc + (uint64_t)(k * 16), idesc, k != 0);
-      umma_commit(&bar);
+    for (int mi = 0; mi < 2; ++mi) {
+#pragma unroll
+      for (int ni = 0; ni < 2; ++ni) {
+        float c[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int ki = 0; ki < 2; ++ki) {
+          const uint8_t* a0 = S8 + (16 * mi + gI) * 64 + 32 * ki + 4 * tI;
+          const uint32_t a[4] = {*reinterpret_cast<const uint32_t*>(a0), *reinterpret_cast<const uint32_t*>(a0 + 8 * 64),
+                                 *reinterpret_cast<const uint32_t*>(a0 + 16), *reinterpret_cast<const uint32_t*>(a0 + 8 * 64 + 16)};
+          const uint8_t* b0 = Ft8 + (8 * ni + gI) * 64 + 32 * ki + 4 * tI;
+          mma_bf16_16816(c, a, *reinterpret_cast<const uint32_t*>(b0), *reinterpret_cast<const uint32_t*>(b0 + 16));
+        }
+#pragma unroll
+        for (int e = 0; e < 4; ++e) sO[warp][(16 * mi + gI + 8 * (e >> 1)) * 17 + 8 * ni + 2 * tI + (e & 1)] = c[e];
+      }
     }
-    mbar_wait(&bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    uint32_t r[16];
-    tmem_ld_32x16(tmem + ((uint32_t)(warp * 32) << 16), r);
-    tmem_ld_wait();
-    if (live && lane < F) {
+    __syncwarp();
+    if (b < B && lane < F) {
       float acc[16];
 #pragma unroll
-      for (int d = 0; d < 16; ++d) acc[d] = __uint_as_float(r[d]);
+      for (int d = 0; d < 16; ++d) acc[d] = sO[warp][lane * 17 + d];
       if (lane == 0) {
 #pragma unroll
         for (int d = 0; d < 16; ++d) acc[d] += __bfloat162float(myG[d]);
@@ -442,17 +405,13 @@ __global__ void __launch_bounds__(128) k_dot_bwd_tc(const __nv_bfloat16* __restr
         store_row_bf16<16>(demb + (int64_t)(lane - 1) * demb_stride_t + b * demb_stride_b, acc);
       }
     }
-    tc_fence_before();
-    __syncthreads();
+    __syncwarp();                                      // the staging tiles are rewritten by the next sample
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 32);
 }
 
 #endif  // DR_CUDA_EMU
 
-inline int grid_for(int64_t n, int block, int max_blocks = kNumSMs * 8) {
+inline int grid_for(int64_t n, int block, int max_blocks = num_sms() * 8) {
   int64_t b = (n + block - 1) / block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -478,7 +437,7 @@ int dr_cuda_dot_interaction_fwd_u(const void* x, int64_t ldx, const void* urow, 
 #ifdef DR_CUDA_EMU
   return -100;
 #else
-  int g = grid_for((B + 3) / 4, 1, kNumSMs * 4);
+  int g = grid_for((B + 3) / 4, 1, num_sms() * 4);
   DR_PDL_LAUNCH((k_dot_fwd_tc<true>), g, 128, 0, s, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)urow, 0, 0, T, B, (__nv_bfloat16*)Z, ldz, inv, ldinv, *sync);
   DR_LAUNCH_CHECK();
   return 0;
@@ -492,11 +451,8 @@ int dr_cuda_dot_interaction_bwd_u(const void* dZ, int64_t ldz, const void* x, in
 #ifdef DR_CUDA_EMU
   return -100;
 #else
-  constexpr int kSmem = 32768 + 4096 + 4 * 1024;
-  static DrPerDeviceOnce attr_once; bool& attr = attr_once();
-  if (!attr) { DR_CUDA_CHECK(cudaFuncSetAttribute(k_dot_bwd_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem)); attr = true; }
-  int g = grid_for((B + 3) / 4, 1, kNumSMs * 4);
-  DR_PDL_LAUNCH((k_dot_bwd_tc<true>), g, 128, kSmem, s, (const __nv_bfloat16*)dZ, ldz, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)urow, 0, 0, T, B,
+  int g = grid_for((B + 3) / 4, 1, num_sms() * 4);
+  DR_PDL_LAUNCH((k_dot_bwd_tc<true>), g, 128, 0, s, (const __nv_bfloat16*)dZ, ldz, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)urow, 0, 0, T, B,
                 (__nv_bfloat16*)dx, lddx, (__nv_bfloat16*)demb, demb_stride_t, demb_stride_b, inv, ldinv);
   DR_LAUNCH_CHECK();
   return 0;
@@ -508,14 +464,14 @@ int dr_cuda_dot_interaction_fwd(const void* x, int64_t ldx, const void* emb, int
   if (T + 1 > 32 || ldz > 512 || ldz % 8 || D + (T + 1) * T / 2 > ldz) return -2;
 #ifndef DR_CUDA_EMU
   if (D == 16 && !dot_force_simt()) {
-    int g = grid_for((B + 3) / 4, 1, kNumSMs * 4);
+    int g = grid_for((B + 3) / 4, 1, num_sms() * 4);
     DR_PDL_LAUNCH((k_dot_fwd_tc<false>), g, 128, 0, s, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)emb, emb_stride_t, emb_stride_b, T, B, (__nv_bfloat16*)Z, ldz,
                   (const int32_t*)nullptr, 0, DrSpSync{});
     DR_LAUNCH_CHECK();
     return 0;
   }
 #endif
-  int grid = grid_for((B + 7) / 8, 1, kNumSMs * 6);
+  int grid = grid_for((B + 7) / 8, 1, num_sms() * 6);
   switch (D) {
     case 8: k_dot_fwd<8><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)emb, emb_stride_t, emb_stride_b, T, B, (__nv_bfloat16*)Z, ldz); break;
     case 16: k_dot_fwd<16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)emb, emb_stride_t, emb_stride_b, T, B, (__nv_bfloat16*)Z, ldz); break;
@@ -532,17 +488,14 @@ int dr_cuda_dot_interaction_bwd(const void* dZ, int64_t ldz, const void* x, int6
   if (T + 1 > 32 || ldz > 512 || ldz % 8) return -2;
 #ifndef DR_CUDA_EMU
   if (D == 16 && !dot_force_simt()) {
-    constexpr int kSmem = 32768 + 4096 + 4 * 1024;
-    static DrPerDeviceOnce attr_once; bool& attr = attr_once();
-    if (!attr) { DR_CUDA_CHECK(cudaFuncSetAttribute(k_dot_bwd_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem)); attr = true; }
-    int g = grid_for((B + 3) / 4, 1, kNumSMs * 4);
-    DR_PDL_LAUNCH((k_dot_bwd_tc<false>), g, 128, kSmem, s, (const __nv_bfloat16*)dZ, ldz, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)emb, emb_stride_t, emb_stride_b, T, B,
+    int g = grid_for((B + 3) / 4, 1, num_sms() * 4);
+    DR_PDL_LAUNCH((k_dot_bwd_tc<false>), g, 128, 0, s, (const __nv_bfloat16*)dZ, ldz, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)emb, emb_stride_t, emb_stride_b, T, B,
                                        (__nv_bfloat16*)dx, lddx, (__nv_bfloat16*)demb, demb_stride_t, demb_stride_b, (const int32_t*)nullptr, 0);
     DR_LAUNCH_CHECK();
     return 0;
   }
 #endif
-  int grid = grid_for((B + 7) / 8, 1, kNumSMs * 6);
+  int grid = grid_for((B + 7) / 8, 1, num_sms() * 6);
 #define BWD(DD) k_dot_bwd<DD><<<grid, 256, 0, s>>>((const __nv_bfloat16*)dZ, ldz, (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)emb, emb_stride_t, emb_stride_b, T, B, (__nv_bfloat16*)dx, lddx, (__nv_bfloat16*)demb, demb_stride_t, demb_stride_b)
   switch (D) { case 8: BWD(8); break; case 16: BWD(16); break; case 32: BWD(32); break; default: return -3; }
 #undef BWD

@@ -213,7 +213,7 @@ int dr_nvls_allreduce_apply(const void* mc_ptr, float* w, float* s0, float* s1, 
   if (n % 4) return -2;
   int64_t b = (n / 4 + 255) / 256;
   if (b < 1) b = 1;
-  if (b > kNumSMs * 4) b = kNumSMs * 4;
+  if (b > num_sms() * 4) b = num_sms() * 4;
   DrSpSync sy{}; if (sync) sy = *sync;
   DR_PDL_LAUNCH((k_nvls_allreduce_apply), (int)b, 256, 0, s, (const float*)mc_ptr, w, s0, s1, n / 4, hp_dev, reduced_out, sy);
   DR_LAUNCH_CHECK();
@@ -229,14 +229,14 @@ int dr_nvls_allreduce_2phase(void* mc_ptr, const float* local_ptr, int rank, int
   const int64_t n4 = n / 4, per = (n4 + W - 1) / W;
   int64_t b = (per + 255) / 256;
   if (b < 1) b = 1;
-  if (b > kNumSMs * 4) b = kNumSMs * 4;
+  if (b > num_sms() * 4) b = num_sms() * 4;
   DrSpSync sy{}; if (sync) sy = *sync;
   DR_PDL_LAUNCH((k_nvls_reduce_bcast), (int)b, 256, 0, s, (float*)mc_ptr, n4, rank, W, sy);
   DR_LAUNCH_CHECK();
   if (w) {
     if (!sync) return -3;
     int64_t b2 = (n4 + 255) / 256;
-    if (b2 > kNumSMs * 4) b2 = kNumSMs * 4;
+    if (b2 > num_sms() * 4) b2 = num_sms() * 4;
     DR_PDL_LAUNCH((k_nvls_apply_local), (int)b2, 256, 0, s, local_ptr, w, s0, s1, n4, hp_dev, sy);
     DR_LAUNCH_CHECK();
   }

@@ -1,5 +1,5 @@
 // Op-program serving on the GPU: the non-GEMM ops of an exported inference graph (serving/export.py::export_saved_model_program) over
-// bf16 [B, ld] activation buffers.  The LINEAR ops run on the tcgen05 GEMM (gemm_tcgen05.cu, bias + ReLU in its epilogue); everything
+// bf16 [B, ld] activation buffers.  The LINEAR ops run on the wgmma GEMM (gemm_wgmma.cu, bias + ReLU in its epilogue); everything
 // here is bandwidth-trivial glue between them (a DeepFM forward at batch 2048 moves < 4 MB through these kernels).
 //
 // Reference: the processor runs ANY SavedModel graph per session on the session's device (serving/processor/serving/model_session.cc:377-386,
@@ -217,7 +217,7 @@ __global__ void __launch_bounds__(256) k_prog_sigmoid_cols(const __nv_bfloat16* 
 }
 
 // ---- recurrent / transformer sequence models (DIEN, BST) -------------------------------------------------------------------------------------
-// GRU recurrence over the pre-computed input projection gi [B * L, 3H] (the tcgen05 GEMM x W_ih^T + b_ih): one block per sample, W_hh^T in
+// GRU recurrence over the pre-computed input projection gi [B * L, 3H] (the wgmma GEMM x W_ih^T + b_ih): one block per sample, W_hh^T in
 // shared memory ([k][j]: consecutive threads read consecutive gate columns), two barriers per time step.  PyTorch gate order r, z, n:
 //   r = s(gi_r + W_hr h + b_hr), z = s(gi_z + W_hz h + b_hz), n = tanh(gi_n + r (W_hn h + b_hn)), h' = (1 - z) n + z h
 __global__ void __launch_bounds__(256) k_prog_gru(const __nv_bfloat16* __restrict__ gi, int64_t ldg, const float* __restrict__ whh /* [3H][H] */,
@@ -314,7 +314,7 @@ __global__ void __launch_bounds__(256) k_prog_mha(const __nv_bfloat16* __restric
   }
 }
 
-inline int grid_el(int64_t n) { const int64_t b = (n + 255) / 256; return (int)(b < 1 ? 1 : b > kNumSMs * 8 ? kNumSMs * 8 : b); }
+inline int grid_el(int64_t n) { const int64_t b = (n + 255) / 256; return (int)(b < 1 ? 1 : b > num_sms() * 8 ? num_sms() * 8 : b); }
 inline int grid_rows(int64_t rows) { return grid_el(rows * 32); }
 
 }  // namespace
@@ -422,7 +422,7 @@ int dr_prog_gru(const void* gi, int64_t ldg, const float* whh, const float* bhh,
   if (bytes > 200 * 1024) return -1;                                // W_hh must fit in shared memory (H <= 126)
   static DrPerDeviceOnce attr_once; bool& attr = attr_once();
   if (!attr) { DR_CUDA_CHECK(cudaFuncSetAttribute(k_prog_gru, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
-  k_prog_gru<<<(int)(B < kNumSMs * 4 ? B : kNumSMs * 4), 256, bytes, s>>>((const __nv_bfloat16*)gi, ldg, whh, bhh, L, H, (__nv_bfloat16*)y, ldy, B);
+  k_prog_gru<<<(int)(B < num_sms() * 4 ? B : num_sms() * 4), 256, bytes, s>>>((const __nv_bfloat16*)gi, ldg, whh, bhh, L, H, (__nv_bfloat16*)y, ldy, B);
   DR_LAUNCH_CHECK();
   return 0;
 }
@@ -445,7 +445,7 @@ int dr_prog_mha(const void* qkv, int64_t ldq, const void* valid, int64_t ldv, in
   if (bytes > 200 * 1024) return -1;
   static DrPerDeviceOnce attr_once; bool& attr = attr_once();
   if (!attr) { DR_CUDA_CHECK(cudaFuncSetAttribute(k_prog_mha, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
-  k_prog_mha<<<(int)(B < kNumSMs * 4 ? B : kNumSMs * 4), 256, bytes, s>>>((const __nv_bfloat16*)qkv, ldq, (const __nv_bfloat16*)valid, ldv, S, E, heads, (__nv_bfloat16*)y, ldy, B);
+  k_prog_mha<<<(int)(B < num_sms() * 4 ? B : num_sms() * 4), 256, bytes, s>>>((const __nv_bfloat16*)qkv, ldq, (const __nv_bfloat16*)valid, ldv, S, E, heads, (__nv_bfloat16*)y, ldy, B);
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -9,7 +9,7 @@
 //     old one reaped when its last request finishes (shared_ptr refcount); new DELTA -> patch rows of the live tables +
 //     swap the (small) dense parameter block, no warm-up (model_instance.cc:406-446); invalid versions are skipped.
 //   Tracer: per-request stage timings, dumped every N requests (serving/tracer.h).
-// The reference embeds the TF runtime and runs a SavedModel graph; here inference is the sm_100a kernel sequence of the
+// The reference embeds the TF runtime and runs a SavedModel graph; here inference is the sm_90a kernel sequence of the
 // flagship engine (BatchNorm folded at load time, read-only probes), so a request is ~16 kernel launches on the
 // session's stream.
 #include <dlfcn.h>
@@ -172,7 +172,7 @@ template <typename T> static bool Upload(DevBuf& b, const std::vector<T>& h) {
 
 // Op program (saved_model.json "arch": "program", serving/export.py::export_saved_model_program): the inference graph of a Criteo-style model
 // other than DLRM as a list of ops over [B, width] buffers; buffer 0 = dense inputs, buffer 1 = embeddings [B, T * D].  Same format and
-// op set as the CPU runtime (csrc/host/cpu_serving.cc); here LINEAR runs on the tcgen05 GEMM and the rest on program_kernels.cu.
+// op set as the CPU runtime (csrc/host/cpu_serving.cc); here LINEAR runs on the wgmma GEMM and the rest on program_kernels.cu.
 enum POpKind { P_CONCAT, P_LINEAR, P_AFFINE, P_FM, P_CROSS, P_MUL_ADD, P_ADD, P_LAYERNORM, P_MUL, P_SLICE,
                P_VALID_MASK, P_SEQ_ZIP, P_SEQ_MASK, P_SEQ_SUM, P_DIN_ATT, P_PRELU, P_SOFTMAX, P_COSINE, P_TILE, P_GRU, P_SEQ_LAST, P_MHA, P_SEQ_MEAN, P_NUM_OPS };     // sequence-model ops: see cpu_serving.cc
 // rows1 / P_TILE: sample-aware graph compression (serving/export.py::compress_sample_aware): user-side ops run once per request on row 0
@@ -661,7 +661,7 @@ struct Session {
       void* out = buf(op.out); const int W = dp.width[(size_t)op.out]; const int64_t ldo = ld(op.out);
       const void* a0 = buf(op.in[0]); const int w0 = dp.width[(size_t)op.in[0]]; const int64_t ld0 = ld(op.in[0]);
       switch (op.kind) {
-        case P_LINEAR:                                               // tcgen05 GEMM, bias (+ ReLU) in the epilogue; N padded to 8 with zero rows
+        case P_LINEAR:                                               // wgmma GEMM, bias (+ ReLU) in the epilogue; N padded to 8 with zero rows
           if (op.len > 1)                                            // sequence form: [B, S * K] is a [B * S, K] matrix (un-padded buffers, checked at load)
             rc |= dr_cuda_gemm_tn_ex(a0, pd.L.K, pd.L.w_bf16.p, pd.L.Kp, B * op.len, pd.L.Np, pd.L.Kp, pd.L.bias.as<float>(), op.relu ? 1 : 0, nullptr, 0, 0, out, pd.L.N,
                                      nullptr, nullptr, nullptr, 0, 0, s);

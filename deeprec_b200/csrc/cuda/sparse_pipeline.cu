@@ -1,4 +1,4 @@
-// "Unique-first" model-parallel embedding pipeline over NVLink peer memory (sm_100a).
+// "Unique-first" model-parallel embedding pipeline over NVLink peer memory (sm_90a).
 //
 // The reference dedups ids before every EmbeddingVariable lookup / apply (python/training/optimizer.py:91,
 // kernels/unique_ali_op_gpu.cu.cc: cub radix sort + adjacent-diff + scan) and SOK moves ids, vectors and gradients with three
@@ -13,8 +13,10 @@
 //                             probes / inserts / admits in the device EmbeddingVariable, claims the per-step unique index, and
 //                             stores the bf16 row straight into the SOURCE's urow[gs] (P2P stores).  Last block raises ROWS.
 //   (interaction kernels gather urow[inv[b][c]] -- L2-resident, 32 B rows)
-//   k_sp_segsum  (requester)  pre-reduces the per-sample gradient rows per distinct key into ugrad[gs] (fp32) with in-warp
-//                             match.any combining, so only UNIQUE rows ever cross NVLink.  Last block raises GRAD.
+//   k_sp_segsum  (requester)  pre-reduces the per-sample gradient rows per distinct key into ugrad[gs] with in-warp match.any
+//                             combining, so only UNIQUE rows ever cross NVLink.  Last block raises GRAD.  ugrad holds 64-bit fixed
+//                             point (units of 2^-40): integer addition is associative, so a key's sum does not depend on the order
+//                             in which warps add to it, and a training step computes the same gradients on every run.
 //   k_sp_grad    (owner)      waits per source on its GRAD flag, pulls ugrad rows over NVLink and reduces the <= W contributions
 //                             per key into gsum[unique]; the row-wise optimizer (k_apply) follows on the same stream.
 //   k_sp_reset   (requester)  clears the touched scratch slots through the bucket lists (no 50 MB memset per step).
@@ -22,6 +24,12 @@
 // With the bench's id distribution only ~15 % of the ids of a batch are distinct: NVLink traffic, owner-side probes and
 // owner-side atomics all shrink by that factor, and what is left on the requester is perfectly balanced across ranks.
 #include "sp_sync.cuh"
+
+namespace {
+constexpr float kUgradScale = 1099511627776.f;        // 2^40: |row sum| < 8e6, resolution 9e-13 (finer than a bf16 gradient of 1e-9)
+__device__ __forceinline__ unsigned long long ugrad_fix(float v) { return (unsigned long long)(long long)rintf(v * kUgradScale); }
+__device__ __forceinline__ float ugrad_float(unsigned long long q) { return (float)(long long)q * (1.f / kUgradScale); }
+}  // namespace
 #include "table.cuh"
 
 using namespace drc;
@@ -55,7 +63,7 @@ __global__ void __launch_bounds__(256) k_sp_dedup(const int64_t* __restrict__ id
                                                   int32_t* __restrict__ inv /* [B][ldinv] */, int32_t* __restrict__ invT /* [C][B] or null */,
                                                   int64_t* __restrict__ bkt_key,
                                                   int32_t* __restrict__ bkt_gs, int32_t* __restrict__ bcnt /* [T][W] */,
-                                                  float* __restrict__ ugrad, DrSpSync sync) {
+                                                  unsigned long long* __restrict__ ugrad, DrSpSync sync) {
   pdl_sync();
   extern __shared__ int32_t s_inv[];                         // [32][ldinv + 1]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -116,8 +124,8 @@ __global__ void __launch_bounds__(256) k_sp_dedup(const int64_t* __restrict__ id
         bkt_key[slot] = key;
         bkt_gs[slot] = gs;
         if (ugrad) {
-          float4* z = reinterpret_cast<float4*>(ugrad + (int64_t)gs * g.dim);
-          for (int q = 0; q < g.dim / 4; ++q) z[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+          int4* z = reinterpret_cast<int4*>(ugrad + (int64_t)gs * g.dim);
+          for (int q = 0; q < g.dim / 2; ++q) z[q] = make_int4(0, 0, 0, 0);
         }
       }
       s_inv[lane * lds + c] = gs;
@@ -300,7 +308,7 @@ __global__ void __launch_bounds__(256) k_sp_lookup(const DrDeviceTable* __restri
 // -----------------------------------------------------------------------------------------------------------------
 template <int LPR /* dim / 4 */>
 __global__ void __launch_bounds__(256) k_sp_segsum(const __nv_bfloat16* __restrict__ demb /* [C][B][dim] */, const int32_t* __restrict__ invT /* [C][B] */,
-                                                   DrSpGeom g, float* __restrict__ ugrad, DrSpSync sync) {
+                                                   DrSpGeom g, unsigned long long* __restrict__ ugrad, DrSpSync sync) {
   pdl_sync();
   constexpr int dim = 4 * LPR;
   constexpr int V = dim / 8;                                   // int4 (8 bf16) chunks per row
@@ -337,9 +345,9 @@ __global__ void __launch_bounds__(256) k_sp_segsum(const __nv_bfloat16* __restri
             for (int e = 0; e < 4; ++e) { const float2 f = unpack_bf16x2(w[e]); acc[8 * v + 2 * e] += f.x; acc[8 * v + 2 * e + 1] += f.y; }
           }
         }
-        float* dst = ugrad + (int64_t)gs * dim;
+        unsigned long long* dst = ugrad + (int64_t)gs * dim;
 #pragma unroll
-        for (int d = 0; d < dim; d += 4) red_add_v4_f32(dst + d, acc[d], acc[d + 1], acc[d + 2], acc[d + 3]);
+        for (int d = 0; d < dim; ++d) atomicAdd(dst + d, ugrad_fix(acc[d]));
       }
     }
     __syncwarp();
@@ -398,7 +406,8 @@ __global__ void __launch_bounds__(256) k_sp_grad(const DrDeviceTable* __restrict
       const int32_t p = own_pos[own_off];
       if (p < 0) continue;
       // the peer row does not depend on the tag: both loads are in flight together
-      const float4 v = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(ugrad.ptr[s]) + (int64_t)own_gs[own_off] * dim + 4 * lane);
+      const unsigned long long* q = reinterpret_cast<const unsigned long long*>(ugrad.ptr[s]) + (int64_t)own_gs[own_off] * dim + 4 * lane;
+      const float4 v = make_float4(ugrad_float(q[0]), ugrad_float(q[1]), ugrad_float(q[2]), ugrad_float(q[3]));
       const int32_t u = tables[table_map[t]].slots[p].tag;
       if (u < 0) continue;
       if (W == 1) *reinterpret_cast<float4*>(gsum + (int64_t)u * dim + 4 * lane) = v;     // one contribution per key: plain store (gsum is zero)
@@ -464,7 +473,7 @@ __global__ void k_sp_stats(DrSpGeom g, const int32_t* __restrict__ bcnt, int64_t
 }
 
 inline int sp_grid(int64_t blocks) {
-  const int64_t cap = (int64_t)kNumSMs * sparse_blocks_per_sm();
+  const int64_t cap = (int64_t)num_sms() * sparse_blocks_per_sm();
   if (blocks < 1) blocks = 1;
   return (int)(blocks > cap ? cap : blocks);
 }
@@ -474,26 +483,26 @@ inline int sp_grid(int64_t blocks) {
 extern "C" {
 
 int dr_sp_init_scratch(void* scr, int64_t n, cudaStream_t s) {
-  k_sp_init_scratch<<<kNumSMs * 4, 256, 0, s>>>((DrSpSlot*)scr, n);
+  k_sp_init_scratch<<<num_sms() * 4, 256, 0, s>>>((DrSpSlot*)scr, n);
   DR_LAUNCH_CHECK();
   return 0;
 }
 
 int dr_sp_dedup(const int64_t* ids, const DrSpGeom* g, void* scr, int32_t* inv, int32_t* invT, int64_t* bkt_key, int32_t* bkt_gs, int32_t* bcnt,
-                float* ugrad, const DrSpSync* sync, cudaStream_t s) {
+                void* ugrad, const DrSpSync* sync, cudaStream_t s) {
   if (g->ldinv % 4 || g->ldinv < g->C || g->dim % 4) return -2;
   const size_t smem = (size_t)32 * (g->ldinv + 1) * 4;
   if (smem > 48 * 1024) return -3;
-  DR_PDL_LAUNCH((k_sp_dedup), sp_grid((g->B + 31) / 32), 256, smem, s, ids, *g, (DrSpSlot*)scr, inv, invT, bkt_key, bkt_gs, bcnt, ugrad, *sync);
+  DR_PDL_LAUNCH((k_sp_dedup), sp_grid((g->B + 31) / 32), 256, smem, s, ids, *g, (DrSpSlot*)scr, inv, invT, bkt_key, bkt_gs, bcnt, (unsigned long long*)ugrad, *sync);
   DR_LAUNCH_CHECK();
   return 0;
 }
 
 // demb: bf16 [C][B][dim] per-sample gradient rows (feature-major); accumulates into ugrad and raises the GRAD flags
-int dr_sp_segsum(const void* demb, const int32_t* invT, const DrSpGeom* g, float* ugrad, const DrSpSync* sync, cudaStream_t s) {
+int dr_sp_segsum(const void* demb, const int32_t* invT, const DrSpGeom* g, void* ugrad, const DrSpSync* sync, cudaStream_t s) {
   const int64_t units = ((g->B + 31) / 32) * g->C;
   const int grid = sp_grid((units + 7) / 8);
-#define SPS(L) DR_PDL_LAUNCH((k_sp_segsum<L>), grid, 256, 0, s, (const __nv_bfloat16*)demb, invT, *g, ugrad, *sync)
+#define SPS(L) DR_PDL_LAUNCH((k_sp_segsum<L>), grid, 256, 0, s, (const __nv_bfloat16*)demb, invT, *g, (unsigned long long*)ugrad, *sync)
   switch (g->dim / 4) {
     case 2: SPS(2); break; case 4: SPS(4); break; case 8: SPS(8); break; case 16: SPS(16); break;
     default: return -3;

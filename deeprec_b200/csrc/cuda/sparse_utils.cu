@@ -1,4 +1,4 @@
-// Sparse utility kernels of the input / embedding front-end, sm_100a.  One C entry per op, every data-dependent size stays on the device
+// Sparse utility kernels of the input / embedding front-end, sm_90a.  One C entry per op, every data-dependent size stays on the device
 // (the python wrapper reads the count once, where the reference blocks on a D2H copy of the cub select result).
 //
 // Reference kernels replaced (SURVEY §2.14 K14 / K16):
@@ -23,7 +23,7 @@ using namespace drc;
 
 namespace {
 
-inline int grid_el(int64_t n, int block = 256) { const int64_t b = (n + block - 1) / block; return (int)(b < 1 ? 1 : b > kNumSMs * 8 ? kNumSMs * 8 : b); }
+inline int grid_el(int64_t n, int block = 256) { const int64_t b = (n + block - 1) / block; return (int)(b < 1 ? 1 : b > num_sms() * 8 ? num_sms() * 8 : b); }
 inline size_t align256(size_t n) { return (n + 255) / 256 * 256; }
 
 // ---------------------------------------------------------------------------------------------- prune + fill-empty-rows

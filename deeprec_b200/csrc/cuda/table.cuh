@@ -14,7 +14,7 @@
 
 extern "C" {
 // One hash-table slot = ONE 32-byte DRAM sector: the probe that finds the key has also fetched every piece of metadata the
-// lookup / claim / apply kernels need (an SoA layout costs 4-5 random sectors per key; measured in profiles/ncu_summary.md).
+// lookup / claim / apply kernels need (an SoA layout costs 4-5 random sectors per key).
 struct __align__(32) DrSlot {
   int64_t key;             // kEmptyKey / kTombKey / key
   int32_t freq;

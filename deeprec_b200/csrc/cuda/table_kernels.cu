@@ -1,4 +1,4 @@
-// sm_100a kernels for the device EmbeddingVariable: fused find-or-insert (+admission, frequency,
+// sm_90a kernels for the device EmbeddingVariable: fused find-or-insert (+admission, frequency,
 // version, dedup claim), row gather, metadata queries, rehash, eviction scan, snapshot, import.
 //
 // Reference kernels replaced: K1-K5 of SURVEY §2.14 (gpu_hash_table.cu.cc:187-658).
@@ -315,7 +315,7 @@ __global__ void k_fill_i64(int64_t* p, int64_t v, int64_t n) {
 }
 
 inline int grid_for(int64_t n, int block, int max_blocks = 0) {
-  if (max_blocks <= 0) max_blocks = kNumSMs * sparse_blocks_per_sm();
+  if (max_blocks <= 0) max_blocks = num_sms() * sparse_blocks_per_sm();
   int64_t b = (n + block - 1) / block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -327,7 +327,7 @@ inline int grid_for(int64_t n, int block, int max_blocks = 0) {
 extern "C" {
 
 int dr_cuda_table_init_slots(void* slots, int64_t n, cudaStream_t s) {
-  k_init_slots<<<grid_for(n, 256, kNumSMs * 8), 256, 0, s>>>((DrSlot*)slots, n);
+  k_init_slots<<<grid_for(n, 256, num_sms() * 8), 256, 0, s>>>((DrSlot*)slots, n);
   DR_LAUNCH_CHECK();
   return 0;
 }

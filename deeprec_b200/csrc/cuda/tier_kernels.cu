@@ -245,7 +245,7 @@ struct TierManager {
 
 template <typename T> int alloc_pinned(T** p, size_t n) { return (int)cudaHostAlloc((void**)p, n * sizeof(T), cudaHostAllocMapped); }
 template <typename T> int alloc_dev(T** p, size_t n) { return (int)cudaMalloc((void**)p, n * sizeof(T)); }
-inline int grid_of(int64_t n) { int64_t b = (n + 255) / 256; if (b < 1) b = 1; const int64_t cap = (int64_t)kNumSMs * sparse_blocks_per_sm(); return (int)(b > cap ? cap : b); }
+inline int grid_of(int64_t n) { int64_t b = (n + 255) / 256; if (b < 1) b = 1; const int64_t cap = (int64_t)num_sms() * sparse_blocks_per_sm(); return (int)(b > cap ? cap : b); }
 
 }  // namespace
 

@@ -7,7 +7,7 @@ get_version, export, sparse_read, lookup_tier), ``MultiHashVariable`` (:986),
 
 A table lives in one of two native engines behind the same interface:
   * host  -- csrc/host/host_engine.cc (CPU training / DRAM tier), storage DRAM
-  * device -- csrc/cuda/table_kernels.cu (sm_100a hash table + slab rows), storage HBM / HBM_DRAM
+  * device -- csrc/cuda/table_kernels.cu (sm_90a hash table + slab rows), storage HBM / HBM_DRAM
 Forward lookups never insert (post-2306 semantics, embedding_var.h:202-219): unseen keys read
 their default row; creation, admission, frequency and version stamping happen in the apply.
 """

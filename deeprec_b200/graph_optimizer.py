@@ -2,14 +2,14 @@
 ``do_op_fusion``), grappler fusions (dice_fusion.cc, concat_cast_fusing.cc) and the inference-time BatchNorm folding of
 tools/low_precision_optimize -- re-thought for an eager PyTorch framework: the "graph" is the ``nn.Module`` tree, a *template* matches
 a run of consecutive children of an ``nn.Sequential`` (or a single module anywhere) and replaces it by one module backed by a fused
-sm_100a kernel.  Fused modules keep the ORIGINAL ``nn.Parameter`` objects, so optimizers / checkpoints created before or after the
+sm_90a kernel.  Fused modules keep the ORIGINAL ``nn.Parameter`` objects, so optimizers / checkpoints created before or after the
 rewrite see the same tensors.
 
     report = deeprec_b200.graph_optimizer.optimize(model, OptimizerOptions(do_op_fusion=True))
     enable_sample_awared_graph_compression(...)            # re-exported from serving.sample_aware
 
 Templates (``register_template`` adds more):
-  LinearReluChain      Linear [ReLU] Linear [ReLU] ...      -> nn.FusedMLP      (tcgen05 GEMMs, bias+ReLU epilogue, one autograd node)
+  LinearReluChain      Linear [ReLU] Linear [ReLU] ...      -> nn.FusedMLP      (wgmma GEMMs, bias+ReLU epilogue, one autograd node)
   LinearBatchNormFold  Linear BatchNorm1d   (eval only)     -> Linear           (W' = diag(s) W, b' = s b + t; no normalisation pass)
   LayerNorm            nn.LayerNorm                         -> FusedLayerNorm   (one pass, fused mean/var/scale; fused_layer_norm op)
   Gelu                 nn.GELU                              -> FusedGelu
@@ -39,7 +39,7 @@ class OptimizerOptions:
     fold_batchnorm: bool = True          # only applied to modules in eval mode
     min_chain: int = 1                   # Linear layers a chain needs before it is rewritten
     min_width: int = 8                   # narrower layers (e.g. the final logit) stay plain Linear: no GEMM tile to fill
-    mxfp8_inference: bool = False        # eval-mode Linear(+ReLU) -> block-scaled fp8 layer (ops/mxfp8.py: tcgen05 kind::mxf8f6f4.block_scale)
+    mxfp8_inference: bool = False        # eval-mode Linear(+ReLU) -> block-scaled fp8 layer (ops/mxfp8.py: e4m3 wgmma per 32-element scale block)
 
 
 @dataclass
@@ -145,7 +145,7 @@ class LinearReluChain(FusionTemplate):
 
 class LinearToMXFP8(FusionTemplate):
     """Inference-only: Linear (+ReLU) in eval mode -> MXFP8Linear (weights quantised once with one power-of-two scale per 32 inputs,
-    activations per call; the tensor core applies both scales).  The low-precision rewrite of tools/low_precision_optimize, B200 form."""
+    activations per call; the GEMM applies both scales per 32-element block).  The low-precision rewrite of tools/low_precision_optimize."""
     name = "LinearToMXFP8"
 
     def enabled(self, opts):

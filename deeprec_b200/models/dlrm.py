@@ -104,7 +104,7 @@ class DLRM(nn.Module):
             embs = torch.stack([(t.lookup(ids[i]) if isinstance(t, EmbeddingVariable) else t(ids[i])).to(x.device) for i, t in enumerate(self.tables)], dim=1)
         if self.interaction_op == "dot":
             if self.fused_kernels:
-                from ..nn import dot_interaction as fused_dot   # tcgen05 kernel on CUDA (bf16), the expression above on CPU
+                from ..nn import dot_interaction as fused_dot   # tensor-core kernel on CUDA (bf16), the expression above on CPU
                 z = fused_dot(x, embs)
             else:
                 z = dot_interaction(x, embs)                    # fp32 oracle path

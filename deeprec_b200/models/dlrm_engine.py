@@ -1,15 +1,15 @@
-"""DLRMEngine -- the fused B200 training/inference step for DLRM (the flagship benchmark path).
+"""DLRMEngine -- the fused H100 training/inference step for DLRM (the flagship benchmark path).
 
 Model (modelzoo/dlrm/train.py:68-243): bottom MLP [512,256,64,16] (Dense+ReLU+BatchNorm each), 26
 EmbeddingVariable tables of dim 16, 'dot' interaction (strict lower triangle of the 27x27 Gram
 matrix, concatenated with the bottom output), top MLP [512,256] (Dense+ReLU), logits Dense(1),
 sigmoid + binary cross-entropy, one optimizer for dense and sparse parameters.
 
-Execution design (B200-first; nothing here is a translation of the TF graph):
+Execution design (GPU-first; nothing here is a translation of the TF graph):
   * static buffers + ONE CUDA graph per step (~75 kernel nodes), embedding branch forked onto a
     second stream inside the graph so probes/gathers overlap the bottom MLP;
-  * every GEMM is the hand-written tcgen05/TMEM/TMA kernel (csrc/cuda/gemm_tcgen05.cu) with bias,
-    ReLU and ReLU-backward masks fused in the epilogue; weight gradients are split-K tcgen05 GEMMs
+  * every GEMM is the hand-written wgmma/TMA kernel (csrc/cuda/gemm_wgmma.cu) with bias,
+    ReLU and ReLU-backward masks fused in the epilogue; weight gradients are split-K wgmma GEMMs
     reading both operands MN-major straight from the activations (no transposes);
   * embeddings are model-parallel (every table row-sharded by hash(key) % world) and the dense net
     data-parallel.  The sparse path is "unique-first" (parallel/sparse_pipeline.py): the requester
@@ -69,10 +69,10 @@ class DLRMConfig:
     seed: int = 1234
     overlap_embedding: bool = True              # fork the embedding branch onto a side stream inside the graph
     sparse_blocks_per_sm: int = 4               # resident-block budget of the side-stream sparse kernels (overlap with the GEMMs)
-    gemm_v1: bool = False                       # A/B switch: direct-store GEMM epilogue + separate statistics passes
-    # combine + dot interaction + top-MLP layer 0 in ONE tcgen05 kernel (csrc/cuda/fused_interaction_gemm.cu).  Validated against the
-    # unfused path and the fp32 oracle, but measured SLOWER at B = 65536 (215 us vs 64 + 35 us: the per-SM builder phase cannot overlap
-    # the GEMM phase with a single 96 KB Z tile in shared memory -- profiles/r2_notes.md), so the default step keeps the two kernels.
+    gemm_v1: bool = False                       # A/B switch: separate statistics passes instead of the statistics fused into the GEMM epilogue
+    # combine + dot interaction + top-MLP layer 0 in ONE tensor-core kernel (csrc/cuda/fused_interaction_gemm.cu).  Opt-in: the builder
+    # phase and the GEMM phase of a tile share one 96 KB Z tile in shared memory and run one after the other, so the default step keeps
+    # the two kernels.
     fuse_interaction_gemm: bool = False
 
 
@@ -163,7 +163,7 @@ class DLRMEngine:
         self.s0 = torch.full((self.P,), cfg.initial_accumulator_value if self.kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0,
                              dtype=torch.float32, device=dev) if ns > 0 else None
         self.s1 = torch.zeros(self.P, dtype=torch.float32, device=dev) if ns > 1 else None
-        # bf16 shadows for the tcgen05 GEMMs: W [N, Kp] and W^T [Kp, Np]
+        # bf16 shadows for the wgmma GEMMs: W [N, Kp] and W^T [Kp, Np]
         for L in self.bot + self.top:
             L.w_bf16 = torch.zeros(L.N, L.Kp, dtype=torch.bfloat16, device=dev)
             L.wt_bf16 = torch.zeros(L.Kp, L.Np, dtype=torch.bfloat16, device=dev)
@@ -320,7 +320,7 @@ class DLRMEngine:
 
     def _gemm(self, A, lda, Bm, ldb, M, N, K, bias, relu, mask, ldm, out, ldc, aux_mode=None, S1=None, S2=None):
         """out[M,N] = A[M,K] Bm[N,K]^T (+bias)(relu); aux ``mask`` with aux_mode 1 = ReLU-backward mask, 2 = S2 partner;
-        S1/S2 = column statistics fused into the epilogue (tcgen05 v2 epilogue)."""
+        S1/S2 = column statistics fused into the epilogue (fused GEMM epilogue)."""
         mode = aux_mode if aux_mode is not None else (1 if mask is not None else 0)
         self._call(self.lib.dr_cuda_gemm_tn_ex, ptr(A), lda, ptr(Bm), ldb, M, N, K, ptr(bias) if bias is not None else None, int(relu),
                    ptr(mask) if mask is not None else None, ldm, mode, ptr(out), ldc, None, ptr(S1) if S1 is not None else None,
@@ -605,7 +605,7 @@ class DLRMEngine:
 
     def l2_flush(self) -> None:
         if self._l2_scratch is None:
-            self._l2_scratch = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=self.dev)   # 256 MB > 126 MB L2
+            self._l2_scratch = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=self.dev)   # 256 MB > 50 MB L2
         self._call(self.lib.dr_cuda_l2_flush, ptr(self._l2_scratch), self._l2_scratch.numel(), 0.0)
 
     def state_dict(self) -> Dict[str, torch.Tensor]:

@@ -8,7 +8,7 @@ rest of the model zoo (DeepFM: BASELINE config #3, DIN: config #4, and any ``nn.
     probed / inserted / admitted by their owners, rows pushed over NVLink, gradients pre-reduced per key and pulled by the owners,
     row-wise optimizer on the device table (``parallel/sparse_pipeline.py``) -- sequence features are just more id columns of the
     same table (``col_table``), padding ids (-1) produce zero rows and no statistics;
-  * dense net: the module's own autograd graph (``nn.FusedMLP`` -> tcgen05 GEMMs), parameters and gradients re-pointed into ONE flat
+  * dense net: the module's own autograd graph (``nn.FusedMLP`` -> wgmma GEMMs), parameters and gradients re-pointed into ONE flat
     fp32 buffer each, so the optimizer is one fused kernel -- with ``world > 1`` the in-kernel-synchronised one-shot all-reduce +
     optimizer of ``parallel/p2p.py`` over the symmetric gradient buffer;
   * the whole step (forward, backward, both optimizers, flag protocol) is captured into ONE CUDA graph after three eager warm-up
@@ -311,7 +311,7 @@ def criteo_engine(model, batch_size: int, table_rows: Optional[Sequence[int]] = 
     dense_net = _StripTables(model)
 
     def fwd(net, dense, emb, ids):
-        # bf16 activations end to end (tcgen05 FusedMLP in / out, BatchNorm, FM kernel); fp32 master weights; the loss is taken in fp32
+        # bf16 activations end to end (wgmma FusedMLP in / out, BatchNorm, FM kernel); fp32 master weights; the loss is taken in fp32
         with torch.autocast(emb.device.type, dtype=torch.bfloat16):
             return net.inner.logits(dense["dense"].to(torch.bfloat16), emb)
     return FusedRecEngine(dense_net, fwd, list(range(T)), rows, batch_size, embedding_dim=model.emb_dim,

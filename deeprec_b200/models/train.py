@@ -2,7 +2,7 @@
 --ev --ev_filter {counter,cbf} --ev_elimination {l2,gstep} --emb_fusion --op_fusion --smartstaged --optimizer {adam,adamasync,
 adagraddecay,adagrad,gradientdescent,ftrl} --bf16 --incremental_ckpt --workqueue --parquet_dataset --group_embedding
 --adaptive_emb --dynamic_ev --micro_batch --timeline --steps --batch_size --learning_rate --checkpoint.
-Synthetic Criteo / Taobao data (no datasets offline); ``--engine`` runs DLRM through the fused B200 engine."""
+Synthetic Criteo / Taobao data (no datasets offline); ``--engine`` runs DLRM through the fused GPU engine."""
 from __future__ import annotations
 
 import argparse
@@ -51,7 +51,7 @@ def get_arg_parser():
                         "roles with `python -m deeprec_b200.parallel.ps_train`")
     p.add_argument("--timeline", type=int, default=0)
     p.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
-    p.add_argument("--engine", action="store_true", help="fused sm_100a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / DIN through FusedRecEngine (models/rec_engine.py)")
+    p.add_argument("--engine", action="store_true", help="fused sm_90a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / DIN through FusedRecEngine (models/rec_engine.py)")
     p.add_argument("--log_every", type=int, default=20)
     p.add_argument("--watchdog", type=float, default=0, help="seconds without a finished step before the job dumps stacks and exits 86")
     return p

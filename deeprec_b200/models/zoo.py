@@ -25,14 +25,14 @@ from .dlrm import DLRM
 
 
 def _use_fused(device) -> bool:
-    """CUDA models run their MLPs on the tcgen05 kernels (deeprec_b200.nn) unless DEEPREC_FUSED_NN=0."""
+    """CUDA models run their MLPs on the tensor-core kernels (deeprec_b200.nn) unless DEEPREC_FUSED_NN=0."""
     import os
     return device is not None and torch.device(device).type == "cuda" and os.environ.get("DEEPREC_FUSED_NN", "1") != "0"
 
 
 def _fast_onehot() -> bool:
     """DEEPREC_FAST_ONEHOT=1: one-hot group lookups skip the bag construction (ops/device_table.group_lookup_dense_device).  Off by
-    default until it has been validated and measured on a B200 (written after the round's GPU budget was spent)."""
+    default."""
     import os
     return os.environ.get("DEEPREC_FAST_ONEHOT", "0") == "1"
 

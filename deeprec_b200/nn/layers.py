@@ -1,7 +1,7 @@
-"""torch.nn layers on the hand-written sm_100a kernels -- the building blocks the model zoo uses on a GPU.
+"""torch.nn layers on the hand-written sm_90a kernels -- the building blocks the model zoo uses on a GPU.
 
-  * ``FusedMLP`` / ``FusedLinear``: a chain of Linear(+ReLU) layers as ONE autograd node.  Forward = tcgen05/TMEM/TMA GEMM with
-    bias + ReLU in the epilogue (csrc/cuda/gemm_tcgen05.cu); backward = split-K tcgen05 weight-gradient GEMMs reading both
+  * ``FusedMLP`` / ``FusedLinear``: a chain of Linear(+ReLU) layers as ONE autograd node.  Forward = wgmma/TMA GEMM with
+    bias + ReLU in the epilogue (csrc/cuda/gemm_wgmma.cu); backward = split-K wgmma weight-gradient GEMMs reading both
     operands MN-major, and dX GEMMs whose epilogue applies the previous layer's ReLU mask and reduces its bias gradient,
     i.e. the same dataflow as models/dlrm_engine.py but usable from any nn.Module.  Master weights stay fp32; bf16 shadows
     are re-packed every forward by one small kernel per layer.
@@ -148,7 +148,7 @@ class _FusedMLPFn(torch.autograd.Function):
 
 
 class FusedMLP(nn.Module):
-    """Linear+ReLU chain on the tcgen05 GEMM kernels (CUDA) with an identical-math torch fallback (CPU).
+    """Linear+ReLU chain on the wgmma GEMM kernels (CUDA) with an identical-math torch fallback (CPU).
 
     ``sizes`` are the layer widths; ``last_act`` says whether the last layer is followed by ReLU."""
 
@@ -188,7 +188,7 @@ class FusedMLP(nn.Module):
 
 
 class FusedLinear(FusedMLP):
-    """One Linear (optionally + ReLU) on the tcgen05 GEMM."""
+    """One Linear (optionally + ReLU) on the wgmma GEMM."""
 
     def __init__(self, in_features: int, out_features: int, relu: bool = False, bias: bool = True, device=None):
         super().__init__(in_features, [out_features], last_act=relu, bias=bias, device=device)
@@ -225,7 +225,7 @@ class _DotInteraction(torch.autograd.Function):
 
 
 def dot_interaction(x: torch.Tensor, emb: torch.Tensor) -> torch.Tensor:
-    """DLRM 'dot' interaction (modelzoo/dlrm/train.py:163-236).  CUDA: tcgen05 kernel (D = 16) / SIMT kernel (D = 8, 32)."""
+    """DLRM 'dot' interaction (modelzoo/dlrm/train.py:163-236).  CUDA: tensor-core kernel (D = 16, mma.sync) / SIMT kernel (D = 8, 32)."""
     if x.is_cuda and emb.shape[1] + 1 <= 32 and emb.shape[2] in (8, 16, 32) and _pad8(emb.shape[2] + (emb.shape[1] + 1) * emb.shape[1] // 2) <= 512:
         return _DotInteraction.apply(x, emb)
     feats = torch.cat([x.unsqueeze(1), emb], 1)

@@ -1,6 +1,6 @@
 """Device-resident EmbeddingVariable storage (HBM tier) and the fused multi-table lookup.
 
-Python owns the buffers (torch tensors, so HBM goes through one allocator); the sm_100a kernels in
+Python owns the buffers (torch tensors, so HBM goes through one allocator); the sm_90a kernels in
 csrc/cuda/{table,embedding,optimizer}_kernels.cu receive POD ``DrDeviceTable`` descriptors.
 Parity: GPUHashTable / GPUHashMapKV / HbmStorage (framework/embedding/gpu_hash_table.h:33-133,
 gpu_hash_map_kv.h:29-340, single_tier_storage.h HbmStorage) and the GPU Kv* ops

@@ -3,7 +3,7 @@
 ``SparseIds`` is the SparseTensor analogue: flat ``values`` [nnz] with ``row_ids`` [nnz]
 (sorted by row) and ``batch_size``; optional per-id ``weights``.
 
-On CUDA tensors the combiner runs in the fused sm_100a multi-table kernel
+On CUDA tensors the combiner runs in the fused sm_90a multi-table kernel
 (csrc/cuda/embedding_kernels.cu -- one launch for all tables of a group); on CPU it is
 index_add over the host engine's gather.
 """

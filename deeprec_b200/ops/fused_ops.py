@@ -1,5 +1,5 @@
 """Fused LayerNorm / L2-normalize / GELU / Dice (kernels/fused_layer_norm, fused_l2_normalize, gelu_op*, dice_fusion in the reference).
-CUDA tensors run the sm_100a kernels (csrc/cuda/fused_ops.cu); CPU tensors use the equivalent torch expression."""
+CUDA tensors run the sm_90a kernels (csrc/cuda/fused_ops.cu); CPU tensors use the equivalent torch expression."""
 from __future__ import annotations
 
 import ctypes as C

@@ -1,16 +1,15 @@
-"""MXFP8 (block-scaled fp8) for the MLP path: E4M3 elements with one UE8M0 power-of-two scale per 32 elements along K, multiplied by
-`tcgen05.mma.kind::mxf8f6f4.block_scale` (csrc/cuda/gemm_mxfp8.cu) -- the tensor core applies the scales, so there is no calibration
-pass and no per-tensor scale to go stale when a model is hot-swapped.
+"""MXFP8 (block-scaled fp8) for the MLP path: E4M3 elements with one UE8M0 power-of-two scale per 32 elements along K.  On H100 the
+GEMM (dr_cuda_gemm_mxfp8_tn, csrc/cuda/gemm_wgmma.cu) issues one m64nNk32 e4m3 wgmma per 32-element scale block and promotes its product
+into the fp32 accumulator with the two scales, so there is no calibration pass and no per-tensor scale to go stale when a model is
+hot-swapped.
 
 `quantize_mxfp8_reference` / `dequantize_mxfp8` are plain torch (run anywhere; the CPU tests pin the format and the scale-word layout
 with them); `quantize_mxfp8` and `mxfp8_gemm` call the CUDA kernels; `MXFP8Linear` is the inference layer built from them.
 
-Scale-word layout (what `tcgen05.cp.32x128b.warpx4` wants, so the GEMM needs no in-kernel transpose): rows are grouped in blocks of 128,
-K in blocks of 128; the uint32 of row r and k block kb sits at ``((r // 128) * num_kb + kb) * 128 + (r % 32) * 4 + (r % 128) // 32`` and
-its byte j is the scale of elements ``kb * 128 + 32 j .. + 31``.
+Scale-word layout: rows are grouped in blocks of 128, K in blocks of 128; the uint32 of row r and k block kb sits at
+``((r // 128) * num_kb + kb) * 128 + (r % 32) * 4 + (r % 128) // 32`` and its byte j is the scale of elements ``kb * 128 + 32 j .. + 31``.
 
-Reference parity: DeepRec quantises models offline with tools/low_precision_optimize (BF16 / FP16 / INT8, SURVEY §2.9); block-scaled fp8
-is the B200 form BASELINE.json's north star names.
+Reference parity: DeepRec quantises models offline with tools/low_precision_optimize (BF16 / FP16 / INT8, SURVEY §2.9).
 """
 from __future__ import annotations
 
@@ -47,7 +46,7 @@ def block_exponents(x: torch.Tensor) -> torch.Tensor:
 
 
 def quantize_mxfp8_reference(x: torch.Tensor):
-    """x [R, C] -> (q uint8 [R, Kp] holding E4M3 bits, sf int32 [sf_words] in the tcgen05.cp layout).  Bit-exact model of k_quantize_mxfp8."""
+    """x [R, C] -> (q uint8 [R, Kp] holding E4M3 bits, sf int32 [sf_words] in the scale-word layout above).  Bit-exact model of k_quantize_mxfp8."""
     R, Cc = x.shape
     Kp = padded_k(Cc)
     xf = torch.zeros(R, Kp, dtype=torch.float32, device=x.device)
@@ -97,7 +96,7 @@ def quantize_mxfp8(x: torch.Tensor):
 
 
 def mxfp8_gemm(aq, sfa, bq, sfb, n: int, bias=None, relu: bool = False, max_ctas: int = 0) -> torch.Tensor:
-    """out [M, N] bf16 = blockscaled(aq [M, Kp]) @ blockscaled(bq [>= N, Kp])^T (+bias)(ReLU) on the tcgen05 block-scaled tensor-core path."""
+    """out [M, N] bf16 = blockscaled(aq [M, Kp]) @ blockscaled(bq [>= N, Kp])^T (+bias)(ReLU) on the block-scaled wgmma path."""
     M, Kp = aq.shape
     assert bq.shape[1] == Kp and bq.shape[0] >= n and n % 8 == 0
     out = torch.empty(M, n, dtype=torch.bfloat16, device=aq.device)

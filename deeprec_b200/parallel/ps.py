@@ -21,7 +21,7 @@ PS -> PS (rows + optimizer slots + freq / version: ``ExportAndRemove`` / ``Resto
 server definition; other workers notice the bumped definition version on their next pull / push (the PS rejects requests made
 under a stale definition) and re-route transparently.
 
-The synchronous NVLink path (parallel/p2p.py) is the fast path on a B200 box; this module is the functional equivalent of the
+The synchronous NVLink path (parallel/p2p.py) is the fast path on an H100 box; this module is the functional equivalent of the
 PS mode for CPU clusters / heterogeneous setups and for the reference's async-training semantics (stale reads, lock-free rows).
 """
 from __future__ import annotations

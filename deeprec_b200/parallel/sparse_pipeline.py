@@ -76,7 +76,7 @@ def bind(lib):
     }
     for name, args in sigs.items():
         if not hasattr(lib, name) and _native.emu_active():
-            continue                             # tcgen05 translation units are not part of the emulation build
+            continue                             # wgmma translation units are not part of the emulation build
         fn = getattr(lib, name)
         fn.argtypes, fn.restype = args, INT
     lib._sp_bound = True
@@ -148,13 +148,13 @@ class SparsePipeline:
         # ---- peer-visible (requester side)
         self.scr_buf = sym(self.Htot * 16)
         self.urow_buf = sym(self.Htot * dim * 2)
-        self.ugrad_buf = sym(self.Htot * dim * 4) if with_grad else None
+        self.ugrad_buf = sym(self.Htot * dim * 8) if with_grad else None       # int64 fixed point (csrc/cuda/sparse_pipeline.cu)
         self.bkt_key_buf = sym(self.Btot * world * 8)
         self.bkt_gs_buf = sym(self.Btot * world * 4)
         self.bcnt_buf = sym(max(64, num_tables * world) * 4)
         self.flags_buf = sym(8 * 16 * 4)
         self.urow = self.urow_buf.tensor(torch.bfloat16, (self.Htot, dim))
-        self.ugrad = self.ugrad_buf.tensor(torch.float32, (self.Htot, dim)) if with_grad else None
+        self.ugrad = self.ugrad_buf.tensor(torch.int64, (self.Htot, dim)) if with_grad else None
         self.bcnt = self.bcnt_buf.tensor(i32t, (num_tables, world))
         # ---- local
         self.state = torch.zeros(16, dtype=i32t, device=dev)
@@ -213,6 +213,10 @@ class SparsePipeline:
         assert demb.shape == (self.C, self.B, self.dim) and demb.dtype == torch.bfloat16
         _chk(self.lib.dr_sp_segsum(ptr(demb), ptr(self.invT), self.geom_ref(), ptr(self.ugrad), self.sync_ref(), self._s()), "segsum")
         self.launches += 1
+
+    def ugrad_rows(self) -> torch.Tensor:
+        """The pre-reduced per-key gradient rows as fp32 (ugrad holds them in 64-bit fixed point, units of 2^-40)."""
+        return (self.ugrad.double() * 2.0 ** -40).float()
 
     def grad(self, ctx, table_map: torch.Tensor) -> None:
         """Owner side: pull the sources' pre-reduced gradient rows into gsum[unique] (k_apply follows)."""

@@ -588,7 +588,7 @@ def export_saved_model_program(model, export_dir: str, version: int, root: Optio
                                sample_aware: Optional[dict] = None) -> str:
     """Full export of a zoo model (Criteo-style ``WDL``, ``DeepFM``, ``DCN``, ``DCNv2``, ``MaskNet``; sequence model ``DIN`` with ``max_len`` history
     positions -- request ids = the ``[3 + 2 L, B]`` block of ``models.rec_engine.din_ids`` and one dummy dense column) as an op program + EmbeddingVariable tables; loaded by
-    ``Processor(dir, cfg)`` (GPU runtime: tcgen05 GEMMs + csrc/cuda/program_kernels.cu; ``device="cpu"``: the host interpreter) exactly like a DLRM
+    ``Processor(dir, cfg)`` (GPU runtime: wgmma GEMMs + csrc/cuda/program_kernels.cu; ``device="cpu"``: the host interpreter) exactly like a DLRM
     export (same ModelConfig, update protocol, request formats)."""
     was_training = model.training
     model.eval()

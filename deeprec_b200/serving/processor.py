@@ -56,7 +56,7 @@ class _Abi:
 
 
 class Processor:
-    """``device="cuda"``: the GPU runtime (csrc/cuda/serving_runtime.cu: device tables, bf16 / fp8 tcgen05 MLP; DLRM exports and op-program
+    """``device="cuda"``: the GPU runtime (csrc/cuda/serving_runtime.cu: device tables, bf16 / fp8 wgmma MLP; DLRM exports and op-program
     exports of the other Criteo-style models);
     ``device="cpu"``: the CPU runtime (csrc/host/cpu_serving.cc: host tables, fp32 MLP on the OpenMP pool).  Same saved-model directory,
     request encodings, ModelConfig keys and hot-swap protocol.  Default: cuda when a GPU is visible, else cpu."""
@@ -71,7 +71,7 @@ class Processor:
         if device is None:
             import torch
             # both runtimes interpret op-program exports (DeepFM, DCN, WDL, ... -- export_saved_model_program): the GPU one runs the LINEAR ops
-            # on the tcgen05 GEMM and the glue ops on csrc/cuda/program_kernels.cu, the CPU one is csrc/host/cpu_serving.cc::RunProgram
+            # on the wgmma GEMM and the glue ops on csrc/cuda/program_kernels.cu, the CPU one is csrc/host/cpu_serving.cc::RunProgram
             device = "cuda" if torch.cuda.is_available() else "cpu"
         self.device, self.program = device, program
         if device == "cpu":

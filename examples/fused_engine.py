@@ -1,4 +1,4 @@
-"""FusedRecEngine: any dense net over the unique-first sparse pipeline, the whole training step as one CUDA graph on a B200 -- shown here on the
+"""FusedRecEngine: any dense net over the unique-first sparse pipeline, the whole training step as one CUDA graph on an H100 -- shown here on the
 CUDA-on-CPU emulation of the same kernels (``_native.cuda_emulation()``), so it runs anywhere.  Multi-tier tables (HBM cache over host DRAM),
 auto micro-batch, full + incremental training checkpoints.  On a GPU: drop the ``with`` line, build the model on ``cuda`` and call
 ``eng.capture()`` after the first batch; with torchrun + ``parallel.p2p.P2PComm`` the same code runs model-parallel on 1-8 GPUs."""

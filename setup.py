@@ -1,5 +1,5 @@
 """``pip install --no-build-isolation -e .`` (or ``python setup.py build_ext --inplace``): builds the two C-ABI libraries in-tree
-(``deeprec_b200/lib/libdeeprec_host.so`` with g++, ``libdeeprec_cuda.so`` with nvcc for sm_100a -- skipped with a warning when nvcc is
+(``deeprec_b200/lib/libdeeprec_host.so`` with g++, ``libdeeprec_cuda.so`` with nvcc for sm_90a -- skipped with a warning when nvcc is
 absent) through ``deeprec_b200/build.py`` and installs the python package around them."""
 import os
 import sys
@@ -45,7 +45,7 @@ class BuildPy(build_py):
 setup(
     name="deeprec_b200",
     version="0.1.0",
-    description="Blackwell (B200) native sparse-recommender training and serving engine",
+    description="Hopper (H100) native sparse-recommender training and serving engine",
     packages=find_packages(include=["deeprec_b200", "deeprec_b200.*"]),
     package_data={"deeprec_b200": ["lib/*.so", "csrc/**/*", "csrc/*/*"]},
     python_requires=">=3.10",

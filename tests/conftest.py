@@ -7,7 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `pytest -m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with `pytest -m gpu`")
 
 
 def pytest_collection_modifyitems(config, items):

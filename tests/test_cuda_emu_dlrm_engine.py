@@ -1,6 +1,6 @@
-"""The flagship DLRMEngine on the CUDA-on-CPU emulation: the hand-scheduled training step that bench.py and smoke() run on a B200 -- unique-first
+"""The flagship DLRMEngine on the CUDA-on-CPU emulation: the hand-scheduled training step that bench.py and smoke() run on an H100 -- unique-first
 sparse pipeline, BatchNorm-folded bottom MLP with statistics out of the GEMM epilogue, indirect dot interaction, top MLP, fused head, backward, fused
-optimizers -- executes in the CPU test tier with the SIMT kernels compiled for the host and the tcgen05 GEMMs replaced by host loops with the real
+optimizers -- executes in the CPU test tier with the SIMT kernels compiled for the host and the wgmma GEMMs replaced by host loops with the real
 wrappers' argument contracts (csrc/cuda/emu/emu_stubs.cu).  Same fp32 oracle and tolerances as tests/test_gpu_table_engine.py; plus the engine's
 checkpoint round trip and the model-parallel step with the ranks as threads."""
 import threading

@@ -1,6 +1,6 @@
 """The GPU Processor's op-program interpreter (csrc/cuda/serving_runtime.cu::Session::RunProgram), its glue kernels (program_kernels.cu), the
 device-table kernels and the fused DIN attention kernel, executed on the CUDA-on-CPU emulation (``Processor(device="cuda_emu")``: one host
-thread per CUDA thread; the tcgen05 GEMM entry point replaced by a host loop with the same argument contract).  Same assertions as
+thread per CUDA thread; the wgmma GEMM entry point replaced by a host loop with the same argument contract).  Same assertions as
 tests/test_gpu_zzz_program_serving.py at batch sizes a CPU box can afford: a GPU-less CI catches interpreter / indexing / layout bugs before
 the kernels ever reach hardware."""
 import os

@@ -1,4 +1,4 @@
-"""FP8 (E4M3) tcgen05 GEMM + quantisation kernels against fp32 references."""
+"""FP8 (E4M3) wgmma GEMM + quantisation kernels against fp32 references."""
 import ctypes as C
 
 import pytest

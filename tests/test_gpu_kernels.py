@@ -1,4 +1,4 @@
-"""GPU numerics: every hand-written sm_100a kernel against a plain PyTorch fp32 reference of the same op."""
+"""GPU numerics: every hand-written sm_90a kernel against a plain PyTorch fp32 reference of the same op."""
 import ctypes as C
 
 import pytest

@@ -1,4 +1,4 @@
-"""deeprec_b200.nn layers (tcgen05 GEMM chain, fused interactions) against plain fp32 PyTorch."""
+"""deeprec_b200.nn layers (wgmma GEMM chain, fused interactions) against plain fp32 PyTorch."""
 import pytest
 import torch
 

@@ -81,7 +81,7 @@ def test_python_session_group_round_robin():
 
 
 def test_processor_fp8_mlp_close_to_bf16(tmp_path):
-    """mlp_dtype=fp8: E4M3 tcgen05 GEMMs with calibrated static activation scales; predictions stay close to the bf16 runtime,
+    """mlp_dtype=fp8: E4M3 wgmma GEMMs with calibrated static activation scales; predictions stay close to the bf16 runtime,
     and a delta update re-quantises the dense block while keeping the calibration."""
     from deeprec_b200.serving import Processor, export_delta, export_saved_model
     eng, cards = _engine()

@@ -1,12 +1,9 @@
-"""Fused DIN attention kernel vs the composite fp32 PyTorch reference.
-(File name sorts last: added after the round's GPU budget was spent.)"""
+"""Fused DIN attention kernel vs the composite fp32 PyTorch reference."""
 import os
 import pytest
 import torch
 import torch.nn as nn
 
-# Never run on hardware yet (written after the round's GPU budget was spent): opt-in, so that the round-end `pytest -m gpu` stays on
-# validated ground (a wrong mbarrier protocol would hang, not fail).  `benchmarks/ab_validate.sh` runs them under `timeout`.
 pytestmark = pytest.mark.gpu
 
 

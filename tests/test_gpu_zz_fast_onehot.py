@@ -1,11 +1,8 @@
-"""One-hot group lookup fast path (DEEPREC_FAST_ONEHOT=1) == the generic bag-building path, forward and after training steps.
-(File name sorts last: added after the round's GPU budget was spent.)"""
+"""One-hot group lookup fast path (DEEPREC_FAST_ONEHOT=1) == the generic bag-building path, forward and after training steps."""
 import os
 import pytest
 import torch
 
-# Never run on hardware yet (written after the round's GPU budget was spent): opt-in, so that the round-end `pytest -m gpu` stays on
-# validated ground (a wrong mbarrier protocol would hang, not fail).  `benchmarks/ab_validate.sh` runs them under `timeout`.
 pytestmark = pytest.mark.gpu
 
 

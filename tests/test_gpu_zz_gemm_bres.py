@@ -1,14 +1,11 @@
-"""B-resident (weight-stationary) variant of the tcgen05 GEMM (DEEPREC_GEMM_BRES / dr_cuda_set_gemm_bres): same results as the
-streaming kernel and as the fp32 reference, for every epilogue mode.  Opt-in, default off.
-(File name sorts last: written after the round's GPU budget was spent; first validation happens in the next round.)"""
+"""B-resident (weight-stationary) variant of the wgmma GEMM (DEEPREC_GEMM_BRES / dr_cuda_set_gemm_bres): same results as the
+streaming kernel and as the fp32 reference, for every epilogue mode.  Opt-in, default off."""
 import os
 import ctypes as C
 
 import pytest
 import torch
 
-# Never run on hardware yet (written after the round's GPU budget was spent): opt-in, so that the round-end `pytest -m gpu` stays on
-# validated ground (a wrong mbarrier protocol would hang, not fail).  `benchmarks/ab_validate.sh` runs them under `timeout`.
 pytestmark = pytest.mark.gpu
 
 

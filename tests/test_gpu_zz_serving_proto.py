@@ -1,13 +1,11 @@
 """Native Processor: protobuf PredictRequest (reference predict.proto wire format) through ``process()`` gives the same
-probabilities as the compact wire format.  (File name sorts last: added after the round's GPU budget was spent.)"""
+probabilities as the compact wire format."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
-# Never run on hardware yet (written after the round's GPU budget was spent): opt-in, so that the round-end `pytest -m gpu` stays on
-# validated ground (a wrong mbarrier protocol would hang, not fail).  `benchmarks/ab_validate.sh` runs them under `timeout`.
 pytestmark = pytest.mark.gpu
 
 

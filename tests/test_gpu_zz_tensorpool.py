@@ -1,13 +1,10 @@
-"""GPU TensorPool as PyTorch's CUDA allocator (subprocess: the allocator must be installed before the first CUDA allocation).
-(File name sorts last: added after the round's GPU budget was spent.)"""
+"""GPU TensorPool as PyTorch's CUDA allocator (subprocess: the allocator must be installed before the first CUDA allocation)."""
 import os
 import subprocess
 import sys
 
 import pytest
 
-# Never run on hardware yet (written after the round's GPU budget was spent): opt-in, so that the round-end `pytest -m gpu` stays on
-# validated ground (a wrong mbarrier protocol would hang, not fail).  `benchmarks/ab_validate.sh` runs them under `timeout`.
 pytestmark = pytest.mark.gpu
 
 SCRIPT = r"""

@@ -1,5 +1,5 @@
 """GPU serving of op-program models (WDL / DeepFM / DCN / DCNv2 / MaskNet) -- csrc/cuda/serving_runtime.cu::Session::RunProgram: the LINEAR ops
-on the tcgen05 GEMM, the glue ops on csrc/cuda/program_kernels.cu.  Oracle: the module's own fp32 predictions and the CPU Processor
+on the wgmma GEMM, the glue ops on csrc/cuda/program_kernels.cu.  Oracle: the module's own fp32 predictions and the CPU Processor
 (fp32 interpreter of the SAME exported program).  Written after the round's GPU budget was spent: this file sorts last on purpose.
 
 Reference behaviour: any SavedModel graph runs per session on the session's device (serving/processor/serving/model_session.cc:377-386)."""

@@ -1,10 +1,9 @@
-"""CTA-pair (`cta_group::2`, thread-block cluster of 2) variant of the tcgen05 GEMM (DEEPREC_GEMM_2CTA / dr_cuda_set_gemm_2cta):
-same results as the single-CTA kernels and as the fp32 reference for the direct-store epilogue modes (bias + ReLU, ReLU-backward mask,
-fp32 copy), M / N tails, odd numbers of 128-row blocks (the second CTA of the last pair is all out of bounds).
+"""CTA-pair (thread-block cluster of 2, B tile multicast to both CTAs) variant of the wgmma GEMM (DEEPREC_GEMM_2CTA /
+dr_cuda_set_gemm_2cta): same results as the single-CTA kernels and as the fp32 reference for the epilogue modes (bias + ReLU,
+ReLU-backward mask, fp32 copy), M / N tails, odd numbers of 128-row blocks (the second CTA of the last pair is all out of bounds).
 
-Written after the round's GPU budget was spent, so this is its FIRST run on hardware: the file sorts last in `pytest -m gpu`, and the
-kernel runs in a child process under a timeout -- a wrong mbarrier / cluster protocol hangs instead of failing, and the hang must cost
-one test, not the session."""
+The kernel runs in a child process under a timeout: a wrong mbarrier / cluster protocol hangs instead of failing, and the hang must
+cost one test, not the session."""
 import os
 import subprocess
 import sys

@@ -1,9 +1,8 @@
-"""Block-scaled fp8 GEMM (`tcgen05.mma.kind::mxf8f6f4.block_scale`, csrc/cuda/gemm_mxfp8.cu): the CUDA quantiser equals the torch model of
-the format bit for bit (elements and scale words), and the GEMM equals the fp32 product of the DEQUANTISED operands (so any error left is
-the bf16 output rounding -- a wrong scale-factor layout / sf_id would be off by powers of two), for M / N / K tails and many tiles per CTA.
-
-Written after the round's GPU budget was spent: FIRST run on hardware.  Sorts last; runs in a child process under a timeout (a wrong
-mbarrier transaction count hangs instead of failing)."""
+"""Block-scaled fp8 GEMM (dr_cuda_gemm_mxfp8_tn: one e4m3 wgmma per 32-element scale block, scales applied in registers) and its quantiser
+(csrc/cuda/gemm_mxfp8.cu): the CUDA quantiser equals the torch model of the format bit for bit (elements and scale words), and the GEMM
+equals the fp32 product of the DEQUANTISED operands (so any error left is the bf16 output rounding -- a wrong scale-word layout would be
+off by powers of two), for M / N / K tails and many tiles per CTA.  Runs in a child process under a timeout (a wrong mbarrier protocol
+hangs instead of failing)."""
 import os
 import subprocess
 import sys
@@ -49,8 +48,11 @@ for M, N, K in shapes:
         rs = r.abs().amax(1, keepdim=True) + 1e-6
         e = ((out - r).abs() / rs).max().item()
         assert e < 1e-2, (M, N, K, relu, mc, "vs dequantised operands", e)
-        e2 = ((out - f).abs() / (f.abs().amax(1, keepdim=True) + 1e-6)).max().item()
-        assert e2 < 8e-2, (M, N, K, relu, mc, "vs fp32", e2)
+        # vs fp32: the kernel adds no error beyond what the e4m3 format itself costs (the dequantised product's own distance to fp32)
+        fs = f.abs().amax(1, keepdim=True) + 1e-6
+        e2 = ((out - f).abs() / fs).max().item()
+        e_fmt = ((r - f).abs() / fs).max().item()
+        assert e2 < e_fmt + 1e-2, (M, N, K, relu, mc, "vs fp32", e2, e_fmt)
     print("ok", M, N, K, flush=True)
 # ---- the layer
 lin = torch.nn.Linear(368, 500).cuda()

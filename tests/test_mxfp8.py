@@ -1,6 +1,5 @@
 """MXFP8 format helpers (ops/mxfp8.py): the torch model of the block-scaled quantiser pins the number format (E4M3 elements, UE8M0 scale per
-32 along K, smallest power of two that keeps the block inside +-448) and the scale-word layout the tcgen05.cp copy needs; the GPU test
-(tests/test_gpu_zzzzzzz_mxfp8.py) checks the CUDA quantiser bit for bit against it and the block-scaled GEMM against its dequantisation."""
+32 along K, smallest power of two that keeps the block inside +-448) and the scale-word layout."""
 import torch
 
 from deeprec_b200.ops import mxfp8
