@@ -12,7 +12,8 @@ inline float bf(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
 extern "C" {
 
-// gemm_wgmma.cu::dr_cuda_gemm_tn_ex: out[M,N] = A[M,K](lda) * B[N,K](ldb)^T (+bias)(relu)(*mask); bf16 in / out, fp32 accumulate
+// gemm_wgmma.cu::dr_cuda_gemm_tn_ex: out[M,N] = A[M,K](lda) * B[N,K](ldb)^T (+bias)(relu)(*mask); bf16 in / out, fp32 accumulate.
+// Same return codes, out_f32 pitch (ldc) and statistics (fp32 epilogue values before the bf16 rounding) as the hardware entry.
 int dr_cuda_gemm_tn_ex(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* bias, int relu, const void* mask_src,
                        int64_t ld_mask, int aux_mode, void* out, int64_t ldc, float* out_f32, float* S1, float* S2, int max_ctas, int force_v1, cudaStream_t) {
   (void)max_ctas; (void)force_v1;
@@ -20,8 +21,7 @@ int dr_cuda_gemm_tn_ex(const void* A, int64_t lda, const void* B, int64_t ldb, i
   if ((lda % 8) || (ldb % 8) || (ldc % 8) || (N % 8)) return -2;
   if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)out) & 15) return -3;                 // TMA: 16-byte aligned global addresses
   if (lda < K || ldb < K || ldc < N) return -5;
-  const bool v2 = !force_v1 && N > 32 && out_f32 == nullptr;
-  if (!v2 && (S1 || S2 || aux_mode == 2)) return -4;
+  if ((S2 && !S1) || (aux_mode == 2 && !mask_src)) return -4;
   const __nv_bfloat16* a = (const __nv_bfloat16*)A; const __nv_bfloat16* b = (const __nv_bfloat16*)B;
   const __nv_bfloat16* mk = (const __nv_bfloat16*)mask_src;
   __nv_bfloat16* o = (__nv_bfloat16*)out;
@@ -31,11 +31,11 @@ int dr_cuda_gemm_tn_ex(const void* A, int64_t lda, const void* B, int64_t ldb, i
       for (int k = 0; k < K; ++k) acc += bf(a + (int64_t)m * lda + k) * bf(b + (int64_t)n * ldb + k);
       if (bias) acc += bias[n];
       if (relu && acc < 0.f) acc = 0.f;
-      if (mk && aux_mode == 1 && !(bf(mk + (int64_t)m * ld_mask + n) > 0.f)) acc = 0.f;
-      const __nv_bfloat16 r = __float2bfloat16(acc);
-      if (o) o[(int64_t)m * ldc + n] = r;
-      if (out_f32) out_f32[(int64_t)m * N + n] = acc;
-      if (S1) { const float v = __bfloat162float(r); S1[n] += v; if (S2) S2[n] += v * v; }
+      const float w = mk ? bf(mk + (int64_t)m * ld_mask + n) : 0.f;
+      if (mk && aux_mode == 1 && !(w > 0.f)) acc = 0.f;
+      if (o) o[(int64_t)m * ldc + n] = __float2bfloat16(acc);
+      if (out_f32) out_f32[(int64_t)m * ldc + n] = acc;
+      if (S1) { S1[n] += acc; if (S2) S2[n] += acc * (aux_mode == 2 ? w : acc); }
     }
   return 0;
 }

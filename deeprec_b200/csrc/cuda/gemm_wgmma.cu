@@ -548,17 +548,25 @@ int dr_cuda_gemm_tn(const void* A, int64_t lda, const void* B, int64_t ldb, int 
 
 // Extended entry: aux_mode 1 = ReLU-backward mask, 2 = statistics partner; S1/S2 = fused column statistics.  force_v1 is accepted for
 // callers that select the unfused-statistics path; every shape runs the same kernel.
+// Contract (the emulation stand-in in emu/emu_stubs.cu checks and computes the same):
+//   -2  lda, ldb, ldc or N not a multiple of 8;  -3  A, B or out not 16-byte aligned;  -5  lda < K, ldb < K or ldc < N;
+//   -4  S2 without S1, or aux_mode 2 without mask_src.
+//   out and out_f32 share the row pitch ldc.  S1 / S2 are accumulated into (+=) and sum the fp32 epilogue values (after bias, ReLU and
+//   mask, before the bf16 rounding of `out`) of rows < M only; S2 multiplies by the aux value in aux_mode 2, by the value itself otherwise.
+//   Any N (a multiple of 8) may carry statistics, with or without out_f32.
 int dr_cuda_gemm_tn_ex(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* bias, int relu,
                        const void* mask_src, int64_t ld_mask, int aux_mode, void* out, int64_t ldc, float* out_f32, float* S1, float* S2,
                        int max_ctas, int force_v1, cudaStream_t s) {
   (void)force_v1;
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if ((lda % 8) || (ldb % 8) || (ldc % 8) || (N % 8)) return -2;
+  if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)out) & 15) return -3;
+  if (lda < K || ldb < K || ldc < N) return -5;
+  if ((S2 && !S1) || (aux_mode == 2 && !mask_src)) return -4;
   if (max_ctas <= 0) max_ctas = num_sms();
   CUtensorMap ta;
   int rc = make_tmap(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BLOCK_K, BLOCK_M);
   if (rc) return rc;
-  if (S2 && !S1) return -4;
   const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
   float* ws = nullptr;
   if (S1) {

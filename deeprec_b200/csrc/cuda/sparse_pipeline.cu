@@ -26,8 +26,17 @@
 #include "sp_sync.cuh"
 
 namespace {
-constexpr float kUgradScale = 1099511627776.f;        // 2^40: |row sum| < 8e6, resolution 9e-13 (finer than a bf16 gradient of 1e-9)
-__device__ __forceinline__ unsigned long long ugrad_fix(float v) { return (unsigned long long)(long long)rintf(v * kUgradScale); }
+// 2^40: resolution 9e-13 (finer than a bf16 gradient of 1e-9).  A key's gradient sum must stay below 2^22 (4.2e6) in magnitude; the
+// engines scale the loss by 1 / (global batch) (DLRMEngine._head), so a per-sample gradient is O(1 / batch) and a key's sum O(1).
+// A 32-row partial beyond +-2^22 is clamped to it (a defined saturation instead of an out-of-range float -> integer conversion, which
+// is undefined on the host); NaN converts to 0 as the device cvt does.  The 64-bit sum of the partials itself wraps beyond 2^23.
+constexpr float kUgradScale = 1099511627776.f;
+constexpr float kUgradMax = 4611686018427387904.f;           // 2^22 * 2^40 = 2^62
+__device__ __forceinline__ unsigned long long ugrad_fix(float v) {
+  float x = v * kUgradScale;
+  if (!(fabsf(x) <= kUgradMax)) x = x != x ? 0.f : copysignf(kUgradMax, x);
+  return (unsigned long long)(long long)rintf(x);
+}
 __device__ __forceinline__ float ugrad_float(unsigned long long q) { return (float)(long long)q * (1.f / kUgradScale); }
 }  // namespace
 #include "table.cuh"
