@@ -64,7 +64,7 @@ def _bind(lib):
     _sig(lib, "dr_cuda_sparse_accumulate", [P, P, INT, INT, P, P, i64, i64, P, INT, i64, i64, INT, P, P, P, S])
     _sig(lib, "dr_cuda_sparse_apply", [P, P, P, i64, P, INT, P, i64, INT, S])
     _sig(lib, "dr_cuda_advance_hyper", [P, S])
-    _sig(lib, "dr_cuda_dense_apply", [P, P, P, P, i64, P, f32, INT, P, S])
+    _sig(lib, "dr_cuda_dense_apply", [P, P, P, P, i64, P, f32, P, S])
     _sig(lib, "dr_cuda_combine_fwd", [P, P, INT, i64, INT, P, P, P, P, P, P, INT, i64, i64, P, P, S])
     _sig(lib, "dr_cuda_unique", [P, i64, P, P, i64, P, P, P, P, P, S])
     _sig(lib, "dr_cuda_segment_sum", [P, P, i64, INT, P, S])

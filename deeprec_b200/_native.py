@@ -47,7 +47,7 @@ class OptHyper(C.Structure):
         ("beta1_power", f32), ("beta2_power", f32), ("weight_decay", f32),
         ("l1", f32), ("l2", f32), ("l2_shrinkage", f32), ("lr_power", f32),
         ("decay_rate", f32), ("decay_baseline", f32), ("init_accum", f32),
-        ("decay_step", i64), ("global_step", i64),
+        ("decay_step", i64), ("global_step", i64), ("dense_decay_power", i64),
     ]
 
 

@@ -194,7 +194,12 @@ def _load_dense(eng, prefix0: str) -> None:
     rd = BundleReader(prefix0)
     for k, v in _dense_state(eng).items():
         if rd.has(k):
-            v.copy_(rd.read(k).to(v.device).view_as(v))
+            x = rd.read(k).to(v.device)
+            if k == "dense/hyper" and x.numel() < v.numel():     # written before dense_decay_power joined DrOptHyper: it restarts at 0
+                v.zero_()
+                v[:x.numel()].copy_(x.view(-1))
+            else:
+                v.copy_(x.view_as(v))
     rd.close()
     if hasattr(eng, "_pack_weights"):
         eng._pack_weights()                                        # bf16 shadows of the restored fp32 master weights

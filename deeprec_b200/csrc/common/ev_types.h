@@ -77,6 +77,7 @@ struct DrOptHyper {
   float init_accum;
   int64_t decay_step;               // AdagradDecay
   int64_t global_step;
+  int64_t dense_decay_power;        // AdagradDecay: decays applied to the dense accumulators so far (advanced on the device)
 };
 
 }  // extern "C"
@@ -105,7 +106,8 @@ DR_HD int dr_opt_num_slots(int kind) {
 // engine is the numerics oracle for the CUDA kernels). `w` is the embedding element,
 // `s0`/`s1` the two slot elements, `g` the (already de-duplicated, summed) gradient.
 // Adam-family `alpha` = lr*sqrt(1-b2^t)/(1-b1^t) is precomputed by the caller.
-// FTRL is row-coupled (group-lasso on ||linear||) and handled by dr_ftrl_* below.
+// FTRL here is the element-wise dense form (dr_ftrl_dense_elem); EmbeddingVariable rows use the
+// row-coupled form (group-lasso on ||linear||) of dr_ftrl_linear / dr_ftrl_weight below.
 // ---------------------------------------------------------------------------------------
 DR_HD float dr_rsqrtf(float x) {
 #if defined(__CUDA_ARCH__)
@@ -120,6 +122,35 @@ DR_HD float dr_sqrtf(float x) {
 #else
   return __builtin_sqrtf(x);
 #endif
+}
+
+DR_HD float dr_powf(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return powf(a, b);
+#else
+  return __builtin_powf(a, b);
+#endif
+}
+
+// Dense FTRL-proximal, ApplyFtrlV2 (training_ops.cc:370-396): the l2-shrinkage gradient enters `linear` only; new_accum and
+// the stored accumulator use the raw gradient.  (The EmbeddingVariable op puts the shrinkage gradient in new_accum: dr_ftrl_linear.)
+DR_HD void dr_ftrl_dense_elem(const DrOptHyper& hp, float g, float& w, float& accum, float& linear) {
+  const float gs = g + 2.0f * hp.l2_shrinkage * w;
+  const float na = accum + g * g;
+  const bool half = hp.lr_power == -0.5f;
+  const float pw_new = half ? dr_sqrtf(na) : dr_powf(na, -hp.lr_power);
+  const float pw_old = half ? dr_sqrtf(accum) : dr_powf(accum, -hp.lr_power);
+  linear += gs - (pw_new - pw_old) / hp.lr * w;
+  const float quad = pw_new / hp.lr + 2.0f * hp.l2;
+  const float l1_signed = linear < 0.0f ? -hp.l1 : hp.l1;
+  w = (linear > hp.l1 || -linear > hp.l1) ? (l1_signed - linear) / quad : 0.0f;
+  accum = na;
+}
+
+// AdagradDecay on dense variables (ApplyAdagradDecayOp, training_ali_ops.cc:946-950): decay once when global_step / decay_step
+// exceeds the decay power.  k_advance_hyper then advances hp.dense_decay_power, so a captured CUDA graph decays on the right steps.
+DR_HD bool dr_dense_decay_now(const DrOptHyper& hp) {
+  return hp.kind == DR_OPT_ADAGRAD_DECAY && hp.decay_step > 0 && hp.global_step / hp.decay_step > hp.dense_decay_power;
 }
 
 DR_HD void dr_apply_elem(int kind, const DrOptHyper& hp, float alpha, bool decay_now,
@@ -166,6 +197,9 @@ DR_HD void dr_apply_elem(int kind, const DrOptHyper& hp, float alpha, bool decay
       s0 = s0 * hp.beta1 + dr_rsqrtf(s1 + hp.epsilon) * hp.lr * g;
       w -= s0;
       break;
+    case DR_OPT_FTRL:
+      dr_ftrl_dense_elem(hp, g, w, s0, s1);
+      break;
     default:
       break;
   }
@@ -173,14 +207,6 @@ DR_HD void dr_apply_elem(int kind, const DrOptHyper& hp, float alpha, bool decay
 
 DR_HD float dr_adam_alpha(const DrOptHyper& hp) {
   return hp.lr * dr_sqrtf(1.0f - hp.beta2_power) / (1.0f - hp.beta1_power);
-}
-
-DR_HD float dr_powf(float a, float b) {
-#if defined(__CUDA_ARCH__)
-  return powf(a, b);
-#else
-  return __builtin_powf(a, b);
-#endif
 }
 
 // FTRL phase 1: update `linear` (slot1) for one element, return its new value; accum (slot0)

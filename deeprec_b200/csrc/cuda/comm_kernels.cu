@@ -46,6 +46,7 @@ __global__ void __launch_bounds__(256) k_allreduce_apply(DrPeers grad_peers, int
   DrOptHyper hp = {};
   if (hp_dev) hp = *hp_dev;
   const float alpha = hp_dev ? dr_adam_alpha(hp) : 0.f;
+  const bool decay_now = dr_dense_decay_now(hp);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int r = 0; r < W; ++r) {
@@ -57,10 +58,10 @@ __global__ void __launch_bounds__(256) k_allreduce_apply(DrPeers grad_peers, int
       float4 wv = reinterpret_cast<float4*>(w)[i];
       float4 a = s0 ? reinterpret_cast<float4*>(s0)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
       float4 b = s1 ? reinterpret_cast<float4*>(s1)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-      dr_apply_elem(hp.kind, hp, alpha, false, g.x, wv.x, a.x, b.x);
-      dr_apply_elem(hp.kind, hp, alpha, false, g.y, wv.y, a.y, b.y);
-      dr_apply_elem(hp.kind, hp, alpha, false, g.z, wv.z, a.z, b.z);
-      dr_apply_elem(hp.kind, hp, alpha, false, g.w, wv.w, a.w, b.w);
+      dr_apply_elem(hp.kind, hp, alpha, decay_now, g.x, wv.x, a.x, b.x);
+      dr_apply_elem(hp.kind, hp, alpha, decay_now, g.y, wv.y, a.y, b.y);
+      dr_apply_elem(hp.kind, hp, alpha, decay_now, g.z, wv.z, a.z, b.z);
+      dr_apply_elem(hp.kind, hp, alpha, decay_now, g.w, wv.w, a.w, b.w);
       reinterpret_cast<float4*>(w)[i] = wv;
       if (s0) reinterpret_cast<float4*>(s0)[i] = a;
       if (s1) reinterpret_cast<float4*>(s1)[i] = b;

@@ -55,6 +55,7 @@ __global__ void __launch_bounds__(256) k_nvls_allreduce_apply(const float* __res
   DrOptHyper hp = {};
   if (hp_dev) hp = *hp_dev;
   const float alpha = hp_dev ? dr_adam_alpha(hp) : 0.f;
+  const bool decay_now = dr_dense_decay_now(hp);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     float4 g;
     asm volatile("multimem.ld_reduce.relaxed.sys.global.add.v4.f32 {%0,%1,%2,%3}, [%4];"
@@ -64,10 +65,10 @@ __global__ void __launch_bounds__(256) k_nvls_allreduce_apply(const float* __res
       float4 wv = reinterpret_cast<float4*>(w)[i];
       float4 a = s0 ? reinterpret_cast<float4*>(s0)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
       float4 b = s1 ? reinterpret_cast<float4*>(s1)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-      dr_apply_elem(hp.kind, hp, alpha, false, g.x, wv.x, a.x, b.x);
-      dr_apply_elem(hp.kind, hp, alpha, false, g.y, wv.y, a.y, b.y);
-      dr_apply_elem(hp.kind, hp, alpha, false, g.z, wv.z, a.z, b.z);
-      dr_apply_elem(hp.kind, hp, alpha, false, g.w, wv.w, a.w, b.w);
+      dr_apply_elem(hp.kind, hp, alpha, decay_now, g.x, wv.x, a.x, b.x);
+      dr_apply_elem(hp.kind, hp, alpha, decay_now, g.y, wv.y, a.y, b.y);
+      dr_apply_elem(hp.kind, hp, alpha, decay_now, g.z, wv.z, a.z, b.z);
+      dr_apply_elem(hp.kind, hp, alpha, decay_now, g.w, wv.w, a.w, b.w);
       reinterpret_cast<float4*>(w)[i] = wv;
       if (s0) reinterpret_cast<float4*>(s0)[i] = a;
       if (s1) reinterpret_cast<float4*>(s1)[i] = b;
@@ -100,16 +101,17 @@ __global__ void __launch_bounds__(256) k_nvls_apply_local(const float* __restric
   if (sync.state) sp_wait_all(sync, SP_CH_REDUCED);      // every slice owner has broadcast its reduced slice into my buffer
   const DrOptHyper hp = *hp_dev;
   const float alpha = dr_adam_alpha(hp);
+  const bool decay_now = dr_dense_decay_now(hp);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     const int4 raw = ld_v4_volatile(reinterpret_cast<const float4*>(g_local) + i);     // written by the switch: bypass L1
     const float4 g = make_float4(__int_as_float(raw.x), __int_as_float(raw.y), __int_as_float(raw.z), __int_as_float(raw.w));
     float4 wv = reinterpret_cast<float4*>(w)[i];
     float4 a = s0 ? reinterpret_cast<float4*>(s0)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
     float4 b = s1 ? reinterpret_cast<float4*>(s1)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-    dr_apply_elem(hp.kind, hp, alpha, false, g.x, wv.x, a.x, b.x);
-    dr_apply_elem(hp.kind, hp, alpha, false, g.y, wv.y, a.y, b.y);
-    dr_apply_elem(hp.kind, hp, alpha, false, g.z, wv.z, a.z, b.z);
-    dr_apply_elem(hp.kind, hp, alpha, false, g.w, wv.w, a.w, b.w);
+    dr_apply_elem(hp.kind, hp, alpha, decay_now, g.x, wv.x, a.x, b.x);
+    dr_apply_elem(hp.kind, hp, alpha, decay_now, g.y, wv.y, a.y, b.y);
+    dr_apply_elem(hp.kind, hp, alpha, decay_now, g.z, wv.z, a.z, b.z);
+    dr_apply_elem(hp.kind, hp, alpha, decay_now, g.w, wv.w, a.w, b.w);
     reinterpret_cast<float4*>(w)[i] = wv;
     if (s0) reinterpret_cast<float4*>(s0)[i] = a;
     if (s1) reinterpret_cast<float4*>(s1)[i] = b;

@@ -201,9 +201,11 @@ __global__ void k_reset_counter(int32_t* c) {
   *c = 0;
 }
 
-// end-of-step bookkeeping on the device: global_step += 1, Adam-family beta powers advance
+// end-of-step bookkeeping on the device: the dense AdagradDecay power follows the decay this step's dense apply made,
+// global_step += 1, Adam-family beta powers advance
 __global__ void k_advance_hyper(DrOptHyper* hp) {
   pdl_sync();
+  if (dr_dense_decay_now(*hp)) hp->dense_decay_power += 1;
   hp->global_step += 1;
   if (hp->kind == DR_OPT_ADAM || hp->kind == DR_OPT_ADAMW || hp->kind == DR_OPT_ADAM_ASYNC || hp->kind == DR_OPT_ADAM_ASYNC_RMSPROP) {
     hp->beta1_power *= hp->beta1;
@@ -217,28 +219,17 @@ __global__ void k_advance_hyper(DrOptHyper* hp) {
 // -----------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_dense_apply(float* __restrict__ w, const float* __restrict__ grad,
                                                      float* __restrict__ s0, float* __restrict__ s1, int64_t n,
-                                                     const DrOptHyper* __restrict__ hp_dev, float grad_scale, int decay_now,
+                                                     const DrOptHyper* __restrict__ hp_dev, float grad_scale,
                                                      __nv_bfloat16* __restrict__ w_bf16) {
   pdl_sync();
   const DrOptHyper hp = *hp_dev;
   const float alpha = dr_adam_alpha(hp);
+  const bool decay_now = dr_dense_decay_now(hp);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     float g = grad[i] * grad_scale;
     float wv = w[i];
     float a = s0 ? s0[i] : 0.f, b = s1 ? s1[i] : 0.f;
-    if (hp.kind == DR_OPT_FTRL) {
-      // element-wise FTRL-proximal for dense parameters
-      float gs = g + 2.f * hp.l2_shrinkage * wv;
-      float na = a + gs * gs;
-      float pw_new = hp.lr_power == -0.5f ? sqrtf(na) : powf(na, -hp.lr_power);
-      float pw_old = hp.lr_power == -0.5f ? sqrtf(a) : powf(a, -hp.lr_power);
-      b += gs - (pw_new - pw_old) / hp.lr * wv;
-      float quad = pw_new / hp.lr + 2.f * hp.l2;
-      wv = fabsf(b) > hp.l1 ? (copysignf(hp.l1, b) - b) / quad : 0.f;
-      a += g * g;
-    } else {
-      dr_apply_elem(hp.kind, hp, alpha, decay_now != 0, g, wv, a, b);
-    }
+    dr_apply_elem(hp.kind, hp, alpha, decay_now, g, wv, a, b);
     w[i] = wv;
     if (s0) s0[i] = a;
     if (s1) s1[i] = b;
@@ -305,9 +296,9 @@ int dr_cuda_advance_hyper(DrOptHyper* hp_dev, cudaStream_t s) {
 }
 
 int dr_cuda_dense_apply(float* w, const float* grad, float* s0, float* s1, int64_t n, const DrOptHyper* hp_dev, float grad_scale,
-                        int decay_now, void* w_bf16, cudaStream_t s) {
+                        void* w_bf16, cudaStream_t s) {
   if (n == 0) return 0;
-  DR_PDL_LAUNCH((k_dense_apply), grid_for(n, 256), 256, 0, s, w, grad, s0, s1, n, hp_dev, grad_scale, decay_now, (__nv_bfloat16*)w_bf16);
+  DR_PDL_LAUNCH((k_dense_apply), grid_for(n, 256), 256, 0, s, w, grad, s0, s1, n, hp_dev, grad_scale, (__nv_bfloat16*)w_bf16);
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -515,7 +515,7 @@ class DLRMEngine:
             self.comm.dense_allreduce_update(self)
         else:
             self._call(lib.dr_cuda_dense_apply, ptr(self.params), ptr(self.grads), ptr(self.s0) if self.s0 is not None else None,
-                       ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, 0, None)
+                       ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, None)
         self._pack_weights()
         self._call(lib.dr_cuda_advance_hyper, ptr(self.hp_dev))
         if self.uf:

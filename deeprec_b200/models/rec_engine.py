@@ -214,7 +214,7 @@ class FusedRecEngine:
             self.comm.dense_allreduce_update(self)
         else:
             _chk(self.lib.dr_cuda_dense_apply(ptr(self.params), ptr(self.grads), ptr(self.s0) if self.s0 is not None else None,
-                                              ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, 0, None, self._s()), "dense_apply")
+                                              ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, None, self._s()), "dense_apply")
             self.launches += 1
         _chk(self.lib.dr_cuda_advance_hyper(ptr(self.hp_dev), self._s()), "advance_hyper")
         self.sp.step_end()

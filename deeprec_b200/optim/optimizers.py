@@ -369,13 +369,14 @@ class FtrlOptimizer(DeepRecOptimizer):
         return [self._init_acc, 0.0]
 
     def _dense_update(self, p, g, state, group, hp):
-        # dense FTRL-proximal (element-wise l1 shrinkage, stock tf.train.FtrlOptimizer)
+        # dense FTRL-proximal, ApplyFtrlV2 (training_ops.cc:370-396): element-wise l1 shrinkage; the l2-shrinkage gradient enters
+        # `linear` only, the accumulator takes the raw gradient (same rule as csrc/common/ev_types.h::dr_ftrl_dense_elem)
         if "accum" not in state:
             state["accum"] = torch.full_like(p, group["initial_accumulator_value"]); state["linear"] = torch.zeros_like(p)
         acc, lin = state["accum"], state["linear"]
         lr, l1, l2, lp = group["lr"], group["l1"], group["l2"], group["lr_power"]
         gs = g + 2 * group["l2_shrinkage"] * p
-        new_acc = acc + gs * gs
+        new_acc = acc + g * g
         lin.add_(gs - (new_acc.pow(-lp) - acc.pow(-lp)) / lr * p)
         quad = new_acc.pow(-lp) / lr + 2 * l2
         p.copy_(torch.where(lin.abs() > l1, (l1 * lin.sign() - lin) / quad, torch.zeros_like(p)))

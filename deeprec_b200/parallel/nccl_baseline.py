@@ -114,7 +114,7 @@ class NcclComm:
             dist.all_reduce(eng.grads, group=self.group)                                                                              # C1
         s = torch.cuda.current_stream(self.dev).cuda_stream
         _chk(self.lib.dr_cuda_dense_apply(ptr(eng.params), ptr(eng.grads), ptr(eng.s0) if eng.s0 is not None else None,
-                                          ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), 1.0, 0, None, s), "dense_apply")
+                                          ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), 1.0, None, s), "dense_apply")
         eng.launches += 2
 
 

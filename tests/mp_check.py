@@ -26,7 +26,7 @@ def gathered_rows(eng, t, probe, dev):
     return rows, freq, cnt
 
 
-def main():
+def main(optimizer: str = "adagrad"):
     rank, world, lr = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(lr)
     dev = torch.device("cuda", lr)
@@ -52,7 +52,7 @@ def main():
 
     # ---- 2. DLRM engine: unique-first P2P pipeline vs NCCL (SOK) dataflow, same seeds / batches
     cards = [50, 1000, 7, 300] + [97] * 21 + [200000]
-    cfg = DLRMConfig(batch_size=2048, cardinalities=cards, optimizer="adagrad", learning_rate=0.05)
+    cfg = DLRMConfig(batch_size=2048, cardinalities=cards, optimizer=optimizer, learning_rate=0.05)
     nsteps = 5
     batches = [criteo_batch(cfg.batch_size, 13, cards, seed=100 * rank + s) for s in range(nsteps)]
     results = {}
@@ -91,9 +91,9 @@ def main():
     dist.broadcast(ref, 0)
     assert torch.equal(ref, p1), "dense parameters diverged across ranks"
     if rank == 0:
-        print(f"MP_CHECK_OK world={world} losses={['%.4f' % x for x in l1]} distinct_keys={n1}")
+        print(f"MP_CHECK_OK world={world} optimizer={optimizer} losses={['%.4f' % x for x in l1]} distinct_keys={n1}")
     dist.destroy_process_group()
 
 
 if __name__ == "__main__":
-    main()
+    main(*sys.argv[1:2])

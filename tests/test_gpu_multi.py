@@ -10,16 +10,18 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _run(n):
+def _run(n, optimizer="adagrad"):
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={n}", "--master-addr", "127.0.0.1",
-           "--master-port", "29533", os.path.join(ROOT, "tests", "mp_check.py")]
+           "--master-port", "29533", os.path.join(ROOT, "tests", "mp_check.py"), optimizer]
     r = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT)
     assert r.returncode == 0 and "MP_CHECK_OK" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
-def test_p2p_matches_nccl_2gpu():
-    _run(2)
+@pytest.mark.parametrize("optimizer", ["adagrad", "adam", "ftrl"])
+def test_p2p_matches_nccl_2gpu(optimizer):
+    """The fused P2P / NVLS all-reduce + dense update against the NCCL arm's all-reduce + dr_cuda_dense_apply, per optimizer."""
+    _run(2, optimizer)
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 8, reason="needs 8 GPUs")
