@@ -11,6 +11,8 @@ hooks ``core/kernels/save_restore_v2_ops.cc:158-360``, ``IncrSave`` / ``IndicesI
   * delta save  = only rows whose dirty bit was set by the apply kernel since the last (full or delta) save + the dense block.
   * restore     = any world size: every rank scans every shard file and imports the keys it owns under the CURRENT world
                   (``hash(key) % world`` -- the sharding function of the sparse pipeline), then replays the delta chain in order.
+  * linear group = the dim-4 tables of ``FusedRecEngine(linear=True)`` are saved as ``linear/<t>-...`` with the same tensors as ``table/<t>-...``
+                  (and restored the same way), their optimizer's hyper-parameters as ``linear/hyper``.
   * multi-tier  = tables of ``FusedRecEngine(tiered=...)`` save BOTH tiers (the HBM cache and the DRAM tier; rows demoted since the last save
                   carry their dirty bit into the DRAM tier, so delta saves stay complete) and restore each into its tier.
 """
@@ -73,6 +75,16 @@ def _dense_state(eng) -> Dict[str, torch.Tensor]:
     if net is not None:
         for k, v in net.named_buffers():
             out["buffer/" + k] = v
+    if getattr(eng, "linear", False):                    # FusedRecEngine's linear group: its own optimizer step / beta powers / decay
+        out["linear/hyper"] = eng.lin_hp_dev
+    return out
+
+
+def _groups(eng):
+    """(name, tables, tiers) of every embedding group: the engine's tables, and FusedRecEngine's linear group (single-tier)."""
+    out = [("table", eng.tables, getattr(eng, "tiers", None) or {})]
+    if getattr(eng, "linear", False):
+        out.append(("linear", eng.lin_tables, {}))
     return out
 
 
@@ -98,32 +110,33 @@ def save_engine(eng, save_path: str, incremental: bool = False, max_to_keep: int
         for k, v in _dense_state(eng).items():
             w.add(k, v)
     sfx = "sparse_incr_" if incremental else ""
-    tiers = getattr(eng, "tiers", None) or {}
-    for t, tbl in eng.tables.items():
-        if not incremental and (tbl.cfg.steps_to_live > 0 or tbl.cfg.l2_weight_threshold >= 0):
-            tbl.shrink(step)                                      # eviction happens inside a full save (single_tier_storage.h:235-261)
-        if t in tiers:
-            # multi-tier table: the HBM tier is a cache -- rows demoted to the DRAM tier are training state too (hbm_dram_storage.h:
-            # Save() walks both tiers).  In-flight promotions / demotions finish first; the HBM copy of a key wins on restore (imported last).
-            mgr = tiers[t][0]
-            mgr.drain()
-            hs = mgr.host.snapshot(dirty_only=incremental)
-            w.add(f"table/{t}-host-{sfx}keys", hs["keys"]); w.add(f"table/{t}-host-{sfx}values", hs["rows"])
-            w.add(f"table/{t}-host-{sfx}freqs", hs["freqs"]); w.add(f"table/{t}-host-{sfx}versions", hs["versions"])
-        s = tbl.snapshot(dirty_only=incremental)
-        w.add(f"table/{t}-{sfx}keys", s["keys"]); w.add(f"table/{t}-{sfx}values", s["rows"])
-        w.add(f"table/{t}-{sfx}freqs", s["freqs"]); w.add(f"table/{t}-{sfx}versions", s["versions"])
-        w.add(f"table/{t}-{'incr_' if incremental else ''}partition_offset", s["partition_offset"])
-        w.add(f"table/{t}-{sfx}keys_filtered", s["keys_filtered"]); w.add(f"table/{t}-{sfx}freqs_filtered", s["freqs_filtered"])
-        w.add(f"table/{t}-{sfx}versions_filtered", s["versions_filtered"])
-        bloom = tbl.bloom_state()
-        if bloom is not None and not incremental:
-            w.add(f"table/{t}-bloom", bloom)
+    for grp, tables, tiers in _groups(eng):
+        for t, tbl in tables.items():
+            if not incremental and (tbl.cfg.steps_to_live > 0 or tbl.cfg.l2_weight_threshold >= 0):
+                tbl.shrink(step)                                      # eviction happens inside a full save (single_tier_storage.h:235-261)
+            if t in tiers:
+                # multi-tier table: the HBM tier is a cache -- rows demoted to the DRAM tier are training state too (hbm_dram_storage.h:
+                # Save() walks both tiers).  In-flight promotions / demotions finish first; the HBM copy of a key wins on restore (imported last).
+                mgr = tiers[t][0]
+                mgr.drain()
+                hs = mgr.host.snapshot(dirty_only=incremental)
+                w.add(f"{grp}/{t}-host-{sfx}keys", hs["keys"]); w.add(f"{grp}/{t}-host-{sfx}values", hs["rows"])
+                w.add(f"{grp}/{t}-host-{sfx}freqs", hs["freqs"]); w.add(f"{grp}/{t}-host-{sfx}versions", hs["versions"])
+            s = tbl.snapshot(dirty_only=incremental)
+            w.add(f"{grp}/{t}-{sfx}keys", s["keys"]); w.add(f"{grp}/{t}-{sfx}values", s["rows"])
+            w.add(f"{grp}/{t}-{sfx}freqs", s["freqs"]); w.add(f"{grp}/{t}-{sfx}versions", s["versions"])
+            w.add(f"{grp}/{t}-{'incr_' if incremental else ''}partition_offset", s["partition_offset"])
+            w.add(f"{grp}/{t}-{sfx}keys_filtered", s["keys_filtered"]); w.add(f"{grp}/{t}-{sfx}freqs_filtered", s["freqs_filtered"])
+            w.add(f"{grp}/{t}-{sfx}versions_filtered", s["versions_filtered"])
+            bloom = tbl.bloom_state()
+            if bloom is not None and not incremental:
+                w.add(f"{grp}/{t}-bloom", bloom)
     w.close()
-    for tbl in eng.tables.values():
-        tbl.clear_dirty()                                         # the recorder restarts at every (full or delta) save
-    for mgr, _ in tiers.values():
-        mgr.host.clear_dirty()
+    for _, tables, tiers in _groups(eng):
+        for tbl in tables.values():
+            tbl.clear_dirty()                                     # the recorder restarts at every (full or delta) save
+        for mgr, _ in tiers.values():
+            mgr.host.clear_dirty()
     if W > 1:
         import torch.distributed as dist
         dist.barrier()
@@ -151,41 +164,41 @@ def latest_engine_step(directory: str, base: str, incremental: bool = False) -> 
 def _load_tables(eng, prefixes: List[str], incremental: bool) -> int:
     W, r = eng.world, eng.rank
     sfx = "sparse_incr_" if incremental else ""
-    tiers = getattr(eng, "tiers", None) or {}
     n = 0
     for p in prefixes:
         rd = BundleReader(p)
-        for t, tbl in eng.tables.items():
-            hk = f"table/{t}-host-{sfx}keys"
-            if rd.has(hk):                                        # DRAM-tier rows of a multi-tier table
-                hkeys = rd.read(hk)
-                if hkeys.numel():
-                    mine = sp_owner(hkeys, W) == r
+        for grp, tables, tiers in _groups(eng):
+            for t, tbl in tables.items():
+                hk = f"{grp}/{t}-host-{sfx}keys"
+                if rd.has(hk):                                    # DRAM-tier rows of a multi-tier table
+                    hkeys = rd.read(hk)
+                    if hkeys.numel():
+                        mine = sp_owner(hkeys, W) == r
+                        if bool(mine.any()):
+                            rows, fr, ve = rd.read(f"{grp}/{t}-host-{sfx}values")[mine], rd.read(f"{grp}/{t}-host-{sfx}freqs")[mine], rd.read(f"{grp}/{t}-host-{sfx}versions")[mine]
+                            if t in tiers:
+                                if incremental:                   # demoted since the base checkpoint: the HBM copy an earlier bundle restored is
+                                    tbl.remove(hkeys[mine])       # stale, and the HBM tier is authoritative -- drop it before the DRAM-tier import
+                                n += tiers[t][0].host.import_(hkeys[mine], rows, fr, ve)
+                            else:                                 # restored into an engine without the DRAM tier: everything lives in HBM
+                                n += tbl.import_(hkeys[mine], rows, fr, ve)
+                kk = f"{grp}/{t}-{sfx}keys"
+                if not rd.has(kk):
+                    continue
+                keys = rd.read(kk)
+                if keys.numel():
+                    mine = sp_owner(keys, W) == r
                     if bool(mine.any()):
-                        rows, fr, ve = rd.read(f"table/{t}-host-{sfx}values")[mine], rd.read(f"table/{t}-host-{sfx}freqs")[mine], rd.read(f"table/{t}-host-{sfx}versions")[mine]
-                        if t in tiers:
-                            if incremental:                       # demoted since the base checkpoint: the HBM copy an earlier bundle restored is
-                                tbl.remove(hkeys[mine])           # stale, and the HBM tier is authoritative -- drop it before the DRAM-tier import
-                            n += tiers[t][0].host.import_(hkeys[mine], rows, fr, ve)
-                        else:                                     # restored into an engine without the DRAM tier: everything lives in HBM
-                            n += tbl.import_(hkeys[mine], rows, fr, ve)
-            kk = f"table/{t}-{sfx}keys"
-            if not rd.has(kk):
-                continue
-            keys = rd.read(kk)
-            if keys.numel():
-                mine = sp_owner(keys, W) == r
-                if bool(mine.any()):
-                    n += tbl.import_(keys[mine], rd.read(f"table/{t}-{sfx}values")[mine], rd.read(f"table/{t}-{sfx}freqs")[mine],
-                                     rd.read(f"table/{t}-{sfx}versions")[mine])
-            fk = rd.read(f"table/{t}-{sfx}keys_filtered")
-            if fk.numel():
-                mine = sp_owner(fk, W) == r
-                if bool(mine.any()):
-                    tbl.import_(fk[mine], None, rd.read(f"table/{t}-{sfx}freqs_filtered")[mine], rd.read(f"table/{t}-{sfx}versions_filtered")[mine])
-            if rd.has(f"table/{t}-bloom") and len(prefixes) == W:      # counting-Bloom state is per shard: only same-world restores reuse it
-                if p.endswith(f"-part{r:05d}-of-{W:05d}"):
-                    tbl.load_bloom_state(rd.read(f"table/{t}-bloom"))
+                        n += tbl.import_(keys[mine], rd.read(f"{grp}/{t}-{sfx}values")[mine], rd.read(f"{grp}/{t}-{sfx}freqs")[mine],
+                                         rd.read(f"{grp}/{t}-{sfx}versions")[mine])
+                fk = rd.read(f"{grp}/{t}-{sfx}keys_filtered")
+                if fk.numel():
+                    mine = sp_owner(fk, W) == r
+                    if bool(mine.any()):
+                        tbl.import_(fk[mine], None, rd.read(f"{grp}/{t}-{sfx}freqs_filtered")[mine], rd.read(f"{grp}/{t}-{sfx}versions_filtered")[mine])
+                if rd.has(f"{grp}/{t}-bloom") and len(prefixes) == W:      # counting-Bloom state is per shard: only same-world restores reuse it
+                    if p.endswith(f"-part{r:05d}-of-{W:05d}"):
+                        tbl.load_bloom_state(rd.read(f"{grp}/{t}-bloom"))
         rd.close()
     return n
 
@@ -228,7 +241,8 @@ def restore_engine(eng, save_path: str, step: Optional[int] = None, replay_incre
             _load_dense(eng, sh[0])
             n += _load_tables(eng, sh, incremental=True)
             last = s
-    for tbl in eng.tables.values():
-        tbl.clear_dirty()
+    for _, tables, _ in _groups(eng):
+        for tbl in tables.values():
+            tbl.clear_dirty()
     _native_device_sync(eng.dev)
     return last

@@ -20,6 +20,8 @@
 //   k_sp_grad    (owner)      waits per source on its GRAD flag, pulls ugrad rows over NVLink and reduces the <= W contributions
 //                             per key into gsum[unique]; the row-wise optimizer (k_apply) follows on the same stream.
 //   k_sp_reset   (requester)  clears the touched scratch slots through the bucket lists (no 50 MB memset per step).
+//   k_sp_linear_fwd / k_sp_linear_bwd (requester)  a linear (wide) embedding group: the per-sample sum of element 0 of the unique rows,
+//                             and its fp32 gradient scattered into element 0 of ugrad -- in place of gather / segsum.
 //
 // With the bench's id distribution only ~15 % of the ids of a batch are distinct: NVLink traffic, owner-side probes and
 // owner-side atomics all shrink by that factor, and what is left on the requester is perfectly balanced across ranks.
@@ -386,6 +388,64 @@ __global__ void __launch_bounds__(256) k_sp_gather(const __nv_bfloat16* __restri
 }
 
 // -----------------------------------------------------------------------------------------------------------------
+// k_sp_linear_fwd (requester): out[b] = sum_c float(urow[inv[b][c]][0])  -- the linear (wide) logit of a sample, read in place from the
+// unique rows instead of gathering a [B, C, dim] activation.  One thread per sample adds its columns in order in fp32, so the result is
+// the sequential float sum whatever the launch geometry.  Padding (inv < 0) adds nothing.  Waits in-kernel for every owner's ROWS flag.
+// -----------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_sp_linear_fwd(const __nv_bfloat16* __restrict__ urow, const int32_t* __restrict__ inv, int ldinv, int C,
+                                                       int64_t B, int dim, float* __restrict__ out, DrSpSync sync) {
+  pdl_sync();
+  sp_wait_all(sync, SP_CH_ROWS);
+  for (int64_t b = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; b < B; b += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t* ib = inv + b * ldinv;
+    float acc = 0.f;
+    for (int c = 0; c < C; ++c) {
+      const int32_t gs = ib[c];
+      if (gs < 0) continue;
+      uint2 v;
+      DR_LD_V2_VOLATILE_U32(v, urow + (int64_t)gs * dim);       // peer-written row: bypass L1, as k_sp_gather does
+      acc += unpack_bf16x2(v.x).x;
+    }
+    out[b] = acc;
+  }
+}
+
+// -----------------------------------------------------------------------------------------------------------------
+// k_sp_linear_bwd (requester): ugrad[gs][0] += fix(dlogit[b]) for every (c, b) with gs = invT[c][b] >= 0.  The per-sample gradient is
+// fp32 and each term is converted to 64-bit fixed point before anything is combined, so a key's sum is exactly the integer sum of its
+// terms whatever the grid or warp layout.  One warp = 32 consecutive samples of one column; lanes holding the same key are combined
+// with match.any so a hot key costs one atomic per warp.  Elements 1..dim-1 keep the zero k_sp_dedup wrote.  Last block raises GRAD.
+// -----------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_sp_linear_bwd(const float* __restrict__ dlogit, const int32_t* __restrict__ invT, DrSpGeom g,
+                                                       unsigned long long* __restrict__ ugrad, DrSpSync sync) {
+  pdl_sync();
+  __shared__ uint64_t s_q[8][32];                             // (one-token type: the emulation build gives it per-block storage)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t tiles = (g.B + 31) / 32;
+  const int64_t units = tiles * g.C;
+  for (int64_t u = (int64_t)blockIdx.x * 8 + warp; u < units; u += (int64_t)gridDim.x * 8) {
+    const int c = (int)(u / tiles);
+    const int64_t b = (u % tiles) * 32 + lane;
+    int32_t gs = -1;
+    if (b < g.B) gs = invT[(int64_t)c * g.B + b];
+    const bool live = gs >= 0;
+    const unsigned lm = __ballot_sync(0xffffffffu, live);
+    if (live) s_q[warp][lane] = ugrad_fix(dlogit[b]);
+    __syncwarp();
+    if (live) {
+      const unsigned same = __match_any_sync(lm, gs);
+      if (lane == __ffs(same) - 1) {                            // leader of this key inside the tile: integer sum of its members' terms
+        unsigned long long sum = 0;
+        for (unsigned m = same; m; m &= m - 1) sum += s_q[warp][__ffs(m) - 1];
+        atomicAdd(ugrad + (int64_t)gs * g.dim, sum);
+      }
+    }
+    __syncwarp();
+  }
+  sp_signal_last_block(sync, SP_CH_GRAD);
+}
+
+// -----------------------------------------------------------------------------------------------------------------
 // k_sp_grad (owner): gsum[tag(pos)] += ugrad_of_source[gs]      (fp32 rows, pre-reduced per key on the source)
 // -----------------------------------------------------------------------------------------------------------------
 template <int LPR>
@@ -530,7 +590,7 @@ int dr_sp_lookup(const DrDeviceTable* tables_dev, const int32_t* table_map, cons
   const int grid = sp_grid(chunks);
 #define SPL(L) DR_PDL_LAUNCH((k_sp_lookup<L>), grid, 256, 0, s, tables_dev, table_map, *g, P, train, own_pos, own_gs, own_cnt, ulist, nunique, ulist_cap, *sync)
   switch (g->dim / 4) {
-    case 2: SPL(2); break; case 4: SPL(4); break; case 8: SPL(8); break; case 16: SPL(16); break; case 32: SPL(32); break;
+    case 1: SPL(1); break; case 2: SPL(2); break; case 4: SPL(4); break; case 8: SPL(8); break; case 16: SPL(16); break; case 32: SPL(32); break;
     default: return -3;
   }
 #undef SPL
@@ -541,13 +601,13 @@ int dr_sp_lookup(const DrDeviceTable* tables_dev, const int32_t* table_map, cons
 int dr_sp_grad(const DrDeviceTable* tables_dev, const int32_t* table_map, const DrSpGeom* g, int64_t max_bcap, const DrPeers* ugrad,
                const int32_t* own_pos, const int32_t* own_gs, const int32_t* own_cnt, float* gsum, const DrSpSync* sync, cudaStream_t s) {
   const int lpr = g->dim / 4;
-  if (lpr < 2 || lpr > 32 || (lpr & (lpr - 1))) return -3;
+  if (lpr < 1 || lpr > 32 || (lpr & (lpr - 1))) return -3;
   const int ipc = 256 / lpr;
   const int64_t chunks = (int64_t)g->T * g->W * ((max_bcap + ipc - 1) / ipc);
   const int grid = sp_grid(chunks);
 #define SPG(L) DR_PDL_LAUNCH((k_sp_grad<L>), grid, 256, 0, s, tables_dev, table_map, *g, *ugrad, own_pos, own_gs, own_cnt, gsum, *sync)
   switch (lpr) {
-    case 2: SPG(2); break; case 4: SPG(4); break; case 8: SPG(8); break; case 16: SPG(16); break; case 32: SPG(32); break;
+    case 1: SPG(1); break; case 2: SPG(2); break; case 4: SPG(4); break; case 8: SPG(8); break; case 16: SPG(16); break; case 32: SPG(32); break;
     default: return -3;
   }
 #undef SPG
@@ -565,6 +625,23 @@ int dr_sp_gather(const void* urow, const int32_t* inv, const DrSpGeom* g, void* 
     default: return -3;
   }
 #undef SPGA
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// out_f32[b] = sum_c float(urow[inv[b][c]][0]): the linear logit of every local sample (fp32 [B]); waits for every owner's ROWS flag
+int dr_sp_linear_fwd(const void* urow, const int32_t* inv, const DrSpGeom* g, float* out_f32, const DrSpSync* sync, cudaStream_t s) {
+  if (g->dim % 4 || g->dim <= 0 || g->ldinv < g->C) return -2;
+  DR_PDL_LAUNCH((k_sp_linear_fwd), sp_grid((g->B + 255) / 256), 256, 0, s, (const __nv_bfloat16*)urow, inv, g->ldinv, g->C, g->B, g->dim, out_f32, *sync);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// dlogit_f32: fp32 [B] gradient of the linear logits; adds it to element 0 of ugrad[invT[c][b]] for every live id and raises the GRAD flags
+int dr_sp_linear_bwd(const float* dlogit_f32, const int32_t* invT, const DrSpGeom* g, void* ugrad, const DrSpSync* sync, cudaStream_t s) {
+  if (g->dim % 4 || g->dim <= 0) return -2;
+  const int64_t units = ((g->B + 31) / 32) * g->C;
+  DR_PDL_LAUNCH((k_sp_linear_bwd), sp_grid((units + 7) / 8), 256, 0, s, dlogit_f32, invT, *g, (unsigned long long*)ugrad, *sync);
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -1,7 +1,7 @@
 """FusedRecEngine -- one CUDA-graph training step for ANY dense network over the unique-first sparse pipeline.
 
 :class:`models.dlrm_engine.DLRMEngine` hand-schedules DLRM's dense net; this engine generalises the same execution design to the
-rest of the model zoo (DeepFM: BASELINE config #3, DIN: config #4, and any ``nn.Module`` that maps ``(dense inputs, embeddings
+rest of the model zoo (DeepFM: BASELINE config #3, DIN: config #4, WDL, and any ``nn.Module`` that maps ``(dense inputs, embeddings
 [B, C, D])`` to logits):
 
   * embeddings: every table row-sharded over the ranks (hash(key) % world), id columns deduplicated on the requester, distinct keys
@@ -11,6 +11,10 @@ rest of the model zoo (DeepFM: BASELINE config #3, DIN: config #4, and any ``nn.
   * dense net: the module's own autograd graph (``nn.FusedMLP`` -> wgmma GEMMs), parameters and gradients re-pointed into ONE flat
     fp32 buffer each, so the optimizer is one fused kernel -- with ``world > 1`` the in-kernel-synchronised one-shot all-reduce +
     optimizer of ``parallel/p2p.py`` over the symmetric gradient buffer;
+  * optional linear group (``linear=True``, Wide & Deep's wide part, reference modelzoo/wide_and_deep/train.py:271-288): dim-4 tables over the
+    same id columns on a second pipeline with its own optimizer; the per-sample sum of element 0 of the rows is read in place from the unique
+    rows (``k_sp_linear_fwd``) and handed to the dense net as ``linear=`` (fp32 [B]); its gradient goes straight back into the per-key
+    fixed-point sums (``k_sp_linear_bwd``) -- no [B, C, 4] activation, no bf16 rounding of the per-sample gradient;
   * the whole step (forward, backward, both optimizers, flag protocol) is captured into ONE CUDA graph after three eager warm-up
     steps -- per-module Python / launch overhead, the reason the framework-API path ran DeepFM at 0.70 M samples/s, disappears.
 
@@ -42,7 +46,8 @@ class FusedRecEngine:
                  embedding_dim: int = 16, dense_inputs: Optional[Dict[str, tuple]] = None, optimizer: str = "adagrad", learning_rate: float = 0.01,
                  initial_accumulator_value: float = 0.1, filter_freq: int = 0, steps_to_live: int = 0, pad_key: int = -1, seed: int = 1234,
                  max_rows_per_table: int = 1 << 25, device=None, rank: int = 0, world_size: int = 1, comm=None, loss_fn: Optional[Callable] = None,
-                 tiered: Optional[Dict[int, dict]] = None, micro_batch_num: int = 1):
+                 tiered: Optional[Dict[int, dict]] = None, micro_batch_num: int = 1, linear: bool = False, linear_optimizer: Optional[str] = None,
+                 linear_learning_rate: Optional[float] = None):
         """net: dense module (its parameters are trained); forward_fn(net, dense: dict of static tensors, emb [B, C, D] bf16, ids [C, B]) -> logits [B].
         col_table[c]: table of id column c; table_rows[t]: expected distinct keys of table t (pre-sizing hint, tables grow).
         tiered: {table: {"cache_rows": R, "strategy": 0 (LFU) | 1 (LRU)}} -- those tables keep at most ~R rows PER RANK in HBM over a host DRAM tier
@@ -51,7 +56,12 @@ class FusedRecEngine:
         k_tier_publish / k_tier_wait / k_tier_miss_list_mp) -- ``prefetch`` is then a collective, like ``train_step``.
         micro_batch_num: auto micro-batch (graph_execution_state.cc:635-729, ConfigProto.micro_batch_num): the DENSE net's forward + backward run
         over M slices of the batch inside the same step (same CUDA graph), parameter gradients accumulate, one optimizer step -- peak activation
-        memory / M.  The sparse pipeline still runs ONCE per step on the whole batch: dedup gets better with batch size, and its buffers are static."""
+        memory / M.  The sparse pipeline still runs ONCE per step on the whole batch: dedup gets better with batch size, and its buffers are static.
+        linear: a second, linear embedding group (the wide part of Wide & Deep): one dim-4 table per table of ``col_table`` over the same id columns,
+        of which element 0 is the weight of an id.  Every step computes the per-sample sum of those weights in fp32 (``linear_fwd``, read in place from
+        the unique rows) and hands it to ``forward_fn`` as the keyword ``linear=`` (fp32 [B], a leaf whose gradient trains the group); without the
+        group forward_fn is called without it.  The group has its own optimizer: ``linear_optimizer`` / ``linear_learning_rate`` (None: the same as
+        the deep tables), e.g. FTRL at 0.2 as the reference trains Wide & Deep's linear part.  Linear tables are single-tier."""
         self.net, self.forward_fn = net, forward_fn
         self.rank, self.world, self.comm = rank, world_size, comm
         self.emu = _native.emu_active()              # CPU CI: the same step on the CUDA-on-CPU emulation of the kernels (eager, no CUDA graph)
@@ -71,34 +81,8 @@ class FusedRecEngine:
         # ---- tables: this rank's hash(key) % world shard of every table
         self.ctx = get_context(dev, self.D, owner=id(self) & 0x7FFFFFFF)
         ns = _OPT_SLOTS[self.kind]
-        slot_init = [initial_accumulator_value if self.kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0, 0.0, 0.0, 0.0]
-        self.tables: Dict[int, DeviceTable] = {}
-        g = torch.Generator()
-        for t, card in enumerate(table_rows):
-            card = int(card)
-            if world_size > 1:
-                card = card // world_size + card // (8 * world_size) + 1024
-            c = EvConfig()
-            c.dim, c.num_slots, c.has_scalars = self.D, ns, int(self.kind == OPT_ADAGRAD_DECAY)
-            c.init_capacity = card
-            c.filter_type, c.filter_freq = (1, filter_freq) if filter_freq > 0 else (0, 0)
-            c.bloom_counter_bits = 32
-            c.steps_to_live, c.l2_weight_threshold = steps_to_live, -1.0
-            c.default_value_dim, c.default_value_no_permission = 4096, 0.0
-            c.record_freq = c.record_version = 1
-            c.storage_type = 1
-            for i in range(4):
-                c.slot_init[i] = slot_init[i]
-            g.manual_seed(seed + 17 + 1000 * t)
-            dm = torch.empty(4096, self.D).normal_(0.0, 1.0 / math.sqrt(self.D), generator=g)
-            rows = max(1024, min(card, max_rows_per_table))
-            if tiered and t in tiered:            # HBM tier = cache: R rows + head-room for the keys two steps can create before an eviction lands
-                ncols_t = sum(1 for ct in col_table if ct == t)
-                # (world > 1: a rank owns ~1/W of the W batches' keys -- the same expectation, plus slack for the imbalance of hash(key) % W)
-                rows = int(tiered[t]["cache_rows"]) + (2 if world_size == 1 else 3) * ncols_t * batch_size + 4096
-                card = rows
-            cap = _next_pow2(max(2048, 2 * min(card, rows)))
-            self.tables[t] = DeviceTable(c, dm, dev, capacity=cap, row_capacity=rows, owner=id(self) & 0x7FFFFFFF)
+        self.tables = self._make_tables(self.D, self.kind, id(self) & 0x7FFFFFFF, seed + 17, col_table, table_rows, tiered, filter_freq, steps_to_live,
+                                        max_rows_per_table)
         self.tmap = torch.tensor([self.tables[t].gid for t in range(self.T)], dtype=torch.int32, device=dev)
         self.tiers = {}
         if tiered:
@@ -153,16 +137,73 @@ class FusedRecEngine:
         self.s0 = torch.full((self.P,), initial_accumulator_value if self.kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0,
                              dtype=torch.float32, device=dev) if ns > 0 else None
         self.s1 = torch.zeros(self.P, dtype=torch.float32, device=dev) if ns > 1 else None
+        self.ctx.set_hyper(self._hyper(self.kind, learning_rate))
+        self.hp_dev = self.ctx.hp_dev
+        # ---- linear group: its own tables, step context (owner key distinct from the deep group's, whatever its dim), optimizer and pipeline
+        self.linear = bool(linear)
+        if self.linear:
+            self.lin_kind = _OPT_KIND[(linear_optimizer or optimizer).lower()]
+            self.lin_lr = learning_rate if linear_learning_rate is None else linear_learning_rate
+            lin_owner = -1 - (id(self) & 0x7FFFFFFF)
+            self.lin_ctx = get_context(dev, 4, owner=lin_owner)
+            self.lin_tables = self._make_tables(4, self.lin_kind, lin_owner, seed + 29, col_table, table_rows, None, filter_freq, steps_to_live,
+                                                max_rows_per_table)
+            self.lin_tmap = torch.tensor([self.lin_tables[t].gid for t in range(self.T)], dtype=torch.int32, device=dev)
+            self.lin_sp = SparsePipeline(dev, rank, world_size, list(col_table), self.T, batch_size, 4, comm=comm, pad_key=pad_key)
+            self.lin_out = torch.zeros(batch_size, dtype=torch.float32, device=dev)
+            self.lin_dlogit = torch.zeros(batch_size, dtype=torch.float32, device=dev)
+            self.lin_max_unique = max(1, self.lin_sp.Btot * min(world_size, 2))
+            self.lin_ctx.ensure(self.lin_max_unique)
+            self.lin_ctx.claimed_upper = 0
+            self.lin_ctx.set_hyper(self._hyper(self.lin_kind, self.lin_lr))
+            self.lin_hp_dev = self.lin_ctx.hp_dev
+        _native.device_sync(dev)
+
+    def _hyper(self, kind: int, lr: float) -> OptHyper:
         hp = OptHyper()
-        hp.kind, hp.lr = self.kind, learning_rate
+        hp.kind, hp.lr = kind, lr
         hp.beta1, hp.beta2, hp.epsilon = 0.9, 0.999, 1e-8
         hp.beta1_power, hp.beta2_power = 0.9, 0.999
         hp.weight_decay, hp.l1, hp.l2, hp.l2_shrinkage, hp.lr_power = 0.0, 0.0, 0.0, 0.0, -0.5
-        hp.decay_rate, hp.decay_baseline, hp.init_accum = 0.9, initial_accumulator_value, initial_accumulator_value
+        hp.decay_rate, hp.decay_baseline, hp.init_accum = 0.9, self.init_acc, self.init_acc
         hp.decay_step, hp.global_step = 100000, 0
-        self.ctx.set_hyper(hp)
-        self.hp_dev = self.ctx.hp_dev
-        _native.device_sync(dev)
+        return hp
+
+    def _make_tables(self, dim: int, kind: int, owner: int, seed: int, col_table, table_rows, tiered, filter_freq: int, steps_to_live: int,
+                     max_rows_per_table: int) -> Dict[int, DeviceTable]:
+        """This rank's hash(key) % world shard of every table of one embedding group (default rows: normal(0, 1/sqrt(dim)), seeded per table)."""
+        world_size, batch_size = self.world, self.B
+        ns = _OPT_SLOTS[kind]
+        ia = self.init_acc
+        slot_init = [ia if kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0, 0.0, 0.0, 0.0]
+        tables: Dict[int, DeviceTable] = {}
+        g = torch.Generator()
+        for t, card in enumerate(table_rows):
+            card = int(card)
+            if world_size > 1:
+                card = card // world_size + card // (8 * world_size) + 1024
+            c = EvConfig()
+            c.dim, c.num_slots, c.has_scalars = dim, ns, int(kind == OPT_ADAGRAD_DECAY)
+            c.init_capacity = card
+            c.filter_type, c.filter_freq = (1, filter_freq) if filter_freq > 0 else (0, 0)
+            c.bloom_counter_bits = 32
+            c.steps_to_live, c.l2_weight_threshold = steps_to_live, -1.0
+            c.default_value_dim, c.default_value_no_permission = 4096, 0.0
+            c.record_freq = c.record_version = 1
+            c.storage_type = 1
+            for i in range(4):
+                c.slot_init[i] = slot_init[i]
+            g.manual_seed(seed + 1000 * t)
+            dm = torch.empty(4096, dim).normal_(0.0, 1.0 / math.sqrt(dim), generator=g)
+            rows = max(1024, min(card, max_rows_per_table))
+            if tiered and t in tiered:            # HBM tier = cache: R rows + head-room for the keys two steps can create before an eviction lands
+                ncols_t = sum(1 for ct in col_table if ct == t)
+                # (world > 1: a rank owns ~1/W of the W batches' keys -- the same expectation, plus slack for the imbalance of hash(key) % W)
+                rows = int(tiered[t]["cache_rows"]) + (2 if world_size == 1 else 3) * ncols_t * batch_size + 4096
+                card = rows
+            cap = _next_pow2(max(2048, 2 * min(card, rows)))
+            tables[t] = DeviceTable(c, dm, self.dev, capacity=cap, row_capacity=rows, owner=owner)
+        return tables
 
     # ------------------------------------------------------------------------------------------------------------------
     def _s(self):
@@ -173,6 +214,19 @@ class FusedRecEngine:
         self.sp.lookup(self.ctx, self.tmap, train)
         self.sp.gather(self.emb_out)                  # waits for every owner's ROWS flag in-kernel
         self.launches += 3
+        if self.linear:
+            self.lin_sp.dedup(self.ids)
+            self.lin_sp.lookup(self.lin_ctx, self.lin_tmap, train)
+            self.lin_sp.linear_fwd(self.lin_out)      # waits for every owner's ROWS flag in-kernel
+            self.launches += 3
+
+    def _linear_rendezvous(self) -> None:
+        """world > 1: the linear pipeline's DENSE flags, raised and awaited once per step as the deep pipeline's are -- no rank starts its next
+        linear dedup (which zeroes the ugrad rows the owners pull) before every owner has finished this step's pull."""
+        if self.linear and self.world > 1:
+            self.lin_sp.signal(3)
+            self.comm.wait_dense(self.lin_sp)
+            self.launches += 2
 
     def _sparse_backward(self) -> None:
         self.sp.segsum(self.demb)
@@ -181,6 +235,29 @@ class FusedRecEngine:
         _chk(self.lib.dr_cuda_sparse_apply(ptr(self.ctx.structs()), ptr(self.ctx.ulist), ptr(self.ctx.nuniq), self.ctx.ulist.numel(), ptr(self.ctx.gsum),
                                            self.D, ptr(self.hp_dev), self.max_unique, 1, self._s()), "sparse_apply")
         self.launches += 5
+        if self.linear:
+            self.lin_sp.linear_bwd(self.lin_dlogit)
+            self.lin_sp.reset()
+            self.lin_sp.grad(self.lin_ctx, self.lin_tmap)
+            _chk(self.lib.dr_cuda_sparse_apply(ptr(self.lin_ctx.structs()), ptr(self.lin_ctx.ulist), ptr(self.lin_ctx.nuniq), self.lin_ctx.ulist.numel(),
+                                               ptr(self.lin_ctx.gsum), 4, ptr(self.lin_hp_dev), self.lin_max_unique, 1, self._s()), "sparse_apply")
+            self.launches += 4
+            self._linear_rendezvous()
+
+    def _linear_leaf(self, lo: int, hi: int):
+        """The linear logits of samples [lo, hi) as a leaf of the dense net's graph, and the keyword that hands it to forward_fn."""
+        if not self.linear:
+            return None, {}
+        lin = self.lin_out[lo:hi].detach().requires_grad_(True)
+        return lin, {"linear": lin}
+
+    def _linear_grad(self, lin, lo: int, hi: int) -> None:
+        if lin is None:
+            return
+        if lin.grad is None:                                # forward_fn did not use the linear logits
+            self.lin_dlogit[lo:hi].zero_()
+        else:
+            self.lin_dlogit[lo:hi].copy_(lin.grad)
 
     def _step_body(self) -> None:
         for p in self._plist:
@@ -190,22 +267,26 @@ class FusedRecEngine:
         self._sparse_forward(True)
         if self.micro == 1:
             emb = self.emb_out.detach().requires_grad_(True)
-            logits = self.forward_fn(self.net, self.dense, emb, self.ids)
+            lin, kw = self._linear_leaf(0, self.B)
+            logits = self.forward_fn(self.net, self.dense, emb, self.ids, **kw)
             loss = self.loss_fn(logits, self.labels) / self.world
             self.loss.copy_(loss.detach().reshape(1))
             loss.backward()
             self.demb.copy_(emb.grad.permute(1, 0, 2))      # [B, C, D] -> feature-major bf16 [C, B, D] (what k_sp_segsum reads coalesced)
+            self._linear_grad(lin, 0, self.B)
         else:                                               # auto micro-batch: slices of the gathered activation, gradients accumulate in .grad
             mb = self.B // self.micro
             self.loss.zero_()
             for m in range(self.micro):
                 lo, hi = m * mb, (m + 1) * mb
                 emb = self.emb_out[lo:hi].detach().requires_grad_(True)
-                logits = self.forward_fn(self.net, {k: v[lo:hi] for k, v in self.dense.items()}, emb, self.ids[:, lo:hi])
+                lin, kw = self._linear_leaf(lo, hi)
+                logits = self.forward_fn(self.net, {k: v[lo:hi] for k, v in self.dense.items()}, emb, self.ids[:, lo:hi], **kw)
                 loss = self.loss_fn(logits, self.labels[lo:hi]) / (self.world * self.micro)       # mean over the whole batch = mean of the slice means
                 self.loss.add_(loss.detach().reshape(1))
                 loss.backward()
                 self.demb[:, lo:hi].copy_(emb.grad.permute(1, 0, 2))
+                self._linear_grad(lin, lo, hi)
         self._sparse_backward()
         # (the gather kernel of this step waited for every owner's ROWS flag, so every peer has finished last step's all-reduce reads
         #  of the flat gradient buffer: it may be overwritten now)
@@ -219,6 +300,10 @@ class FusedRecEngine:
         _chk(self.lib.dr_cuda_advance_hyper(ptr(self.hp_dev), self._s()), "advance_hyper")
         self.sp.step_end()
         self.launches += 2
+        if self.linear:
+            _chk(self.lib.dr_cuda_advance_hyper(ptr(self.lin_hp_dev), self._s()), "advance_hyper")
+            self.lin_sp.step_end()
+            self.launches += 2
 
     # ------------------------------------------------------------------------------------------------------------------
     def load_batch(self, ids: torch.Tensor, labels: torch.Tensor, dense: Optional[Dict[str, torch.Tensor]] = None, non_blocking: bool = True) -> None:
@@ -274,12 +359,17 @@ class FusedRecEngine:
         was = self.net.training
         self.net.eval()
         self._sparse_forward(False)
-        out = torch.sigmoid(self.forward_fn(self.net, self.dense, self.emb_out, self.ids).float())
+        kw = {"linear": self.lin_out} if self.linear else {}
+        out = torch.sigmoid(self.forward_fn(self.net, self.dense, self.emb_out, self.ids, **kw).float())
         self.sp.reset()
         if self.world > 1:
             self.sp.signal(3)
             self.comm.wait_dense(self.sp)
         self.sp.step_end()
+        if self.linear:
+            self.lin_sp.reset()
+            self._linear_rendezvous()
+            self.lin_sp.step_end()
         self.net.train(was)
         return out
 
@@ -305,17 +395,21 @@ class FusedRecEngine:
 
 # ---- adapters for the model zoo ------------------------------------------------------------------------------------------------
 def criteo_engine(model, batch_size: int, table_rows: Optional[Sequence[int]] = None, **kw) -> FusedRecEngine:
-    """Any :class:`models.zoo.CriteoModel` (DeepFM, WDL, DCN, DCNv2, MaskNet, DLRM-DCN): 13 dense + 26 id columns, one table each."""
+    """Any :class:`models.zoo.CriteoModel` (DeepFM, WDL, DCN, DCNv2, MaskNet, DLRM-DCN): 13 dense + 26 id columns, one table each.  WDL's wide
+    tables become the engine's linear group (``linear_optimizer`` / ``linear_learning_rate`` in ``kw`` train it with its own optimizer)."""
     T = model.num_sparse
     rows = list(table_rows) if table_rows is not None else [1_000_000] * T
+    wide = hasattr(model, "wide")
     dense_net = _StripTables(model)
 
-    def fwd(net, dense, emb, ids):
+    def fwd(net, dense, emb, ids, linear=None):
         # bf16 activations end to end (wgmma FusedMLP in / out, BatchNorm, FM kernel); fp32 master weights; the loss is taken in fp32
         with torch.autocast(emb.device.type, dtype=torch.bfloat16):
+            if linear is not None:                     # WDL: the wide logit is the engine's fp32 linear sum
+                return net.inner.wide_deep_logits(dense["dense"].to(torch.bfloat16), emb, linear[:, None])
             return net.inner.logits(dense["dense"].to(torch.bfloat16), emb)
     return FusedRecEngine(dense_net, fwd, list(range(T)), rows, batch_size, embedding_dim=model.emb_dim,
-                          dense_inputs={"dense": ((batch_size, model.num_dense), torch.float32)}, **kw)
+                          dense_inputs={"dense": ((batch_size, model.num_dense), torch.float32)}, linear=wide, **kw)
 
 
 def din_engine(model, batch_size: int, max_len: int = 50, table_rows: Sequence[int] = (10_000_000, 100_000_000, 10_000), **kw) -> FusedRecEngine:
@@ -345,9 +439,7 @@ class _StripTables(nn.Module):
 
     def __init__(self, model: nn.Module):
         super().__init__()
-        if hasattr(model, "wide"):
-            raise ValueError("models with a second (wide) embedding group are not supported by FusedRecEngine yet")
-        for name in ("emb", "user", "item", "cat"):
+        for name in ("emb", "wide", "user", "item", "cat"):       # WDL's wide tables: the engine's linear group
             if hasattr(model, name) and isinstance(getattr(model, name), nn.Module):
                 try:
                     delattr(model, name)

@@ -178,7 +178,11 @@ class WDL(CriteoModel):
         return super().forward(dense, ids)
 
     def logits(self, dense, embs):
-        wide = self.wide(self._ids).to(dense.device)[..., 0].sum(1, keepdim=True) + self.wide_dense(dense)     # linear part
+        return self.wide_deep_logits(dense, embs, self.wide(self._ids).to(dense.device)[..., 0].sum(1, keepdim=True))
+
+    def wide_deep_logits(self, dense, embs, linear_sum):
+        """linear_sum [B, 1]: the sum of the wide weights of every sample's ids (FusedRecEngine computes it in its linear group)."""
+        wide = linear_sum + self.wide_dense(dense)     # linear part
         deep = self.out(self.deep(torch.cat([dense, embs.flatten(1)], 1)))
         return (wide + deep).squeeze(-1)
 

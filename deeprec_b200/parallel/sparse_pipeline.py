@@ -63,6 +63,8 @@ def bind(lib):
         "dr_sp_dedup": [P, GP, P, P, P, P, P, P, P, SP, P],
         "dr_sp_segsum": [P, P, GP, P, SP, P],
         "dr_sp_gather": [P, P, GP, P, SP, P],
+        "dr_sp_linear_fwd": [P, P, GP, P, SP, P],
+        "dr_sp_linear_bwd": [P, P, GP, P, SP, P],
         "dr_sp_lookup": [P, P, GP, i64, PP, PP, PP, PP, PP, INT, P, P, P, P, P, i64, SP, P],
         "dr_sp_grad": [P, P, GP, i64, PP, P, P, P, P, SP, P],
         "dr_sp_reset": [GP, i64, P, P, P, P, P],
@@ -212,6 +214,21 @@ class SparsePipeline:
         """Requester side: pre-reduce the per-sample gradient rows (bf16 [C, B, dim]) per distinct key into ugrad; raises GRAD."""
         assert demb.shape == (self.C, self.B, self.dim) and demb.dtype == torch.bfloat16
         _chk(self.lib.dr_sp_segsum(ptr(demb), ptr(self.invT), self.geom_ref(), ptr(self.ugrad), self.sync_ref(), self._s()), "segsum")
+        self.launches += 1
+
+    def linear_fwd(self, out: torch.Tensor) -> None:
+        """Requester side: out[b] = sum over the id columns c of float(urow[inv[b, c], 0]) (fp32 [B], summed in column order); padding adds
+        nothing.  The linear (wide) logit read in place from the unique rows; the kernel waits for every owner's ROWS flag."""
+        assert out.shape == (self.B,) and out.dtype == torch.float32 and out.is_contiguous()
+        _chk(self.lib.dr_sp_linear_fwd(ptr(self.urow), ptr(self.inv), self.geom_ref(), ptr(out), self.sync_ref(), self._s()), "linear_fwd")
+        self.launches += 1
+
+    def linear_bwd(self, dlogit: torch.Tensor) -> None:
+        """Requester side: add the fp32 gradient of every sample's linear logit to element 0 of ugrad[inv[b, c]] for every live id (exact
+        64-bit fixed-point sums, elements 1.. stay zero); raises GRAD.  Takes the place of segsum for a linear group."""
+        assert dlogit.shape == (self.B,) and dlogit.dtype == torch.float32 and dlogit.is_contiguous()
+        assert self.ugrad is not None, "linear_bwd needs a pipeline built with with_grad=True"
+        _chk(self.lib.dr_sp_linear_bwd(ptr(dlogit), ptr(self.invT), self.geom_ref(), ptr(self.ugrad), self.sync_ref(), self._s()), "linear_bwd")
         self.launches += 1
 
     def ugrad_rows(self) -> torch.Tensor:
