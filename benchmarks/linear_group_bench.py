@@ -26,9 +26,9 @@ def main():
     eng = FusedRecEngine(torch.nn.Linear(1, 1), lambda net, dense, emb, ids, linear: linear, list(range(C)), cards, B, linear=True, device=dev)
     _, ids, _ = criteo_batch(B, 13, cards, seed=0)
     eng.ids.copy_(ids.to(dev))
-    sp = eng.lin_sp
+    sp = eng.linear.sp
     sp.dedup(eng.ids)
-    sp.lookup(eng.lin_ctx, eng.lin_tmap, False)
+    sp.lookup(eng.linear.ctx, eng.linear.tmap, False)
     dl = torch.randn(B, device=dev) / B
     out = eng.lin_out
 

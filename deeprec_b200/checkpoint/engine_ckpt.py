@@ -75,17 +75,15 @@ def _dense_state(eng) -> Dict[str, torch.Tensor]:
     if net is not None:
         for k, v in net.named_buffers():
             out["buffer/" + k] = v
-    if getattr(eng, "linear", False):                    # FusedRecEngine's linear group: its own optimizer step / beta powers / decay
-        out["linear/hyper"] = eng.lin_hp_dev
+    for g in eng.groups:                                 # a linear group's own optimizer step / beta powers / decay (the deep group's: dense/hyper)
+        if g.is_linear:
+            out["linear/hyper"] = g.hp_dev
     return out
 
 
 def _groups(eng):
-    """(name, tables, tiers) of every embedding group: the engine's tables, and FusedRecEngine's linear group (single-tier)."""
-    out = [("table", eng.tables, getattr(eng, "tiers", None) or {})]
-    if getattr(eng, "linear", False):
-        out.append(("linear", eng.lin_tables, {}))
-    return out
+    """(name, tables, tiers) of every embedding group of the engine: ``table`` for the deep group, ``linear`` for a linear one."""
+    return [("linear" if g.is_linear else "table", g.tables, g.tiers) for g in eng.groups]
 
 
 def _step_of(eng) -> int:

@@ -25,7 +25,6 @@ Execution design (GPU-first; nothing here is a translation of the TF graph):
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
@@ -33,9 +32,12 @@ from typing import Dict, List, Optional, Sequence
 import torch
 
 from .. import _native
-from .._native import EvConfig, OptHyper, ptr
-from ..ops.device_table import DeviceTable, _chk, _next_pow2, get_context
-from ..optim.optimizers import (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_ADAM, OPT_ADAM_ASYNC, OPT_ADAMW, OPT_FTRL, OPT_SGD)
+from .._native import OptHyper, ptr
+from ..checkpoint.engine_ckpt import restore_engine, save_engine
+from ..ops.device_table import DeviceTable, _chk
+from ..optim.optimizers import OPT_KIND, OPT_SLOTS, slot0_init
+from . import embedding_group as _eg
+from .embedding_group import EmbeddingGroup, stream
 
 # Criteo-Terabyte cardinalities (MLPerf DLRM preprocessing, 40M cap) -- used only to shape the
 # synthetic id distributions and pre-size the tables; EmbeddingVariables are hash tables and grow.
@@ -44,11 +46,6 @@ CRITEO_TB_CARDINALITIES = [39884406, 39043, 17289, 7420, 20263, 3, 7120, 1543, 6
 # Criteo-Kaggle cardinalities used by the modelzoo (modelzoo/dlrm/train.py:33-66)
 CRITEO_KAGGLE_CARDINALITIES = [1460, 583, 10131227, 2202608, 305, 24, 12517, 633, 3, 93145, 5683, 8351593, 3194, 27, 14992,
                                5461306, 10, 5652, 2173, 4, 7046547, 18, 15, 286181, 105, 142572]
-
-_OPT_KIND = {"sgd": OPT_SGD, "gradientdescent": OPT_SGD, "adagrad": OPT_ADAGRAD, "adagraddecay": OPT_ADAGRAD_DECAY,
-             "adam": OPT_ADAM, "adamasync": OPT_ADAM_ASYNC, "adamw": OPT_ADAMW, "ftrl": OPT_FTRL}
-_OPT_SLOTS = {OPT_SGD: 0, OPT_ADAGRAD: 1, OPT_ADAGRAD_DECAY: 1, OPT_ADAM: 2, OPT_ADAM_ASYNC: 2, OPT_ADAMW: 2, OPT_FTRL: 2}
-
 
 @dataclass
 class DLRMConfig:
@@ -99,8 +96,8 @@ class DLRMEngine:
         self.lib.dr_cuda_set_sparse_blocks_per_sm(int(cfg.sparse_blocks_per_sm if cfg.overlap_embedding else 16))
         self.comm = comm                           # parallel.p2p.P2PComm or parallel.nccl_baseline.NcclComm (world_size > 1)
         self.B, self.T, self.D = cfg.batch_size, len(cfg.cardinalities), cfg.embedding_dim
-        self.kind = _OPT_KIND[cfg.optimizer.lower()]
-        self.launches = 0
+        self.kind = OPT_KIND[cfg.optimizer.lower()]
+        self._launches = 0
         self._graph = None
         import os as _os
         self._timing, self._events = _os.environ.get("DEEPREC_STEP_TIMING") == "1", {}
@@ -108,7 +105,6 @@ class DLRMEngine:
         self._build_params()
         self._build_tables()
         self._build_buffers()
-        self._init_hyper()
         self._pack_weights()
         _native.device_sync(self.dev)
 
@@ -159,9 +155,8 @@ class DLRMEngine:
         flat[o:o + n] = (torch.rand(n, generator=g) * 2 - 1) * math.sqrt(6.0 / (self.head_K + 1))
         self.params = flat.to(dev)
         self.grads = torch.zeros(self.P, dtype=torch.float32, device=dev) if self.comm is None else self.comm.alloc_grads(self.P)
-        ns = _OPT_SLOTS[self.kind]
-        self.s0 = torch.full((self.P,), cfg.initial_accumulator_value if self.kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0,
-                             dtype=torch.float32, device=dev) if ns > 0 else None
+        ns = OPT_SLOTS[self.kind]
+        self.s0 = torch.full((self.P,), slot0_init(self.kind, cfg.initial_accumulator_value), dtype=torch.float32, device=dev) if ns > 0 else None
         self.s1 = torch.zeros(self.P, dtype=torch.float32, device=dev) if ns > 1 else None
         # bf16 shadows for the wgmma GEMMs: W [N, Kp] and W^T [Kp, Np]
         for L in self.bot + self.top:
@@ -207,33 +202,13 @@ class DLRMEngine:
         else:
             self.owner_of = [t % W for t in range(self.T)]
             self.local_tables = [t for t in range(self.T) if self.owner_of[t] == self.rank]
-        self.ctx = get_context(self.dev, self.D, owner=id(self) & 0x7FFFFFFF)
-        self.tables: Dict[int, DeviceTable] = {}
-        g = torch.Generator().manual_seed(cfg.seed + 17)
-        ns = _OPT_SLOTS[self.kind]
-        slot_init = [cfg.initial_accumulator_value if self.kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0, 0.0, 0.0, 0.0]
-        for t in self.local_tables:
-            card = int(cfg.cardinalities[t])
-            if self.uf and W > 1:
-                card = card // W + card // (8 * W) + 1024        # this rank's shard (+ hash imbalance slack)
-            c = EvConfig()
-            c.dim, c.num_slots, c.has_scalars = self.D, ns, int(self.kind == OPT_ADAGRAD_DECAY)
-            c.init_capacity = card
-            c.filter_type, c.filter_freq = (1, cfg.filter_freq) if cfg.filter_freq > 0 else (0, 0)
-            c.bloom_counter_bits = 32
-            c.steps_to_live, c.l2_weight_threshold = cfg.steps_to_live, -1.0
-            c.default_value_dim, c.default_value_no_permission = 4096, 0.0
-            c.record_freq = c.record_version = 1
-            c.storage_type = 1
-            for i in range(4):
-                c.slot_init[i] = slot_init[i]
-            g.manual_seed(cfg.seed + 17 + 1000 * t)      # initial values depend on (table, key) only -- never on the sharding
-            dm = torch.empty(4096, self.D).normal_(0.0, 1.0 / math.sqrt(self.D), generator=g)
-            rows = min(card, cfg.max_rows_per_table)
-            rows = max(rows, 1024)
-            cap = _next_pow2(max(2048, 2 * min(card, max(rows, 1))))
-            self.tables[t] = DeviceTable(c, dm, self.dev, capacity=cap, row_capacity=rows, owner=id(self) & 0x7FFFFFFF)
-        self.tmap_local = torch.tensor([self.tables[t].gid for t in self.local_tables], dtype=torch.int32, device=self.dev)
+        self.group = EmbeddingGroup(self.dev, self.D, self.kind, cfg.learning_rate, cfg.initial_accumulator_value, id(self) & 0x7FFFFFFF,
+                                    cfg.seed + 17, self.local_tables, cfg.cardinalities, self.B, col_table=list(range(self.T)) if self.uf else None,
+                                    rank=self.rank, world=W, comm=self.comm, filter_freq=cfg.filter_freq, steps_to_live=cfg.steps_to_live,
+                                    max_rows_per_table=cfg.max_rows_per_table)
+        self.groups = [self.group]
+        self.tables: Dict[int, DeviceTable] = self.group.tables
+        self.sp, self.hp_dev = self.group.sp, self.group.hp_dev
 
     # ------------------------------------------------------------------------------------------------
     # static activations
@@ -244,20 +219,13 @@ class DLRMEngine:
         z = lambda *s, dt=bf: torch.zeros(*s, dtype=dt, device=dev)
         self.dense_in = z(B, self.cfg.num_dense, dt=f32)
         self.labels = z(B, dt=f32)
-        nl = len(self.local_tables)
-        W = self.world
         if self.uf:
-            from ..parallel.sparse_pipeline import SparsePipeline
             self.ids = torch.zeros(T, B, dtype=torch.int64, device=dev)          # feature-major id columns (local: never leave the GPU)
-            self.sp = SparsePipeline(dev, self.rank, W, list(range(T)), T, B, D, comm=self.comm)
             self.emb = self.pos = None
             self.demb = z(T, B, D)                                               # per-sample gradient rows, feature-major (local)
-            self.max_unique = max(1, T * B * min(W, 2))          # distinct keys a step can bring to this rank (overflow is flagged, not UB)
         else:
-            self.sp = None
             self.ids, self.emb, self.demb = self.comm.alloc_exchange(T, B, D)
-            self.pos = torch.zeros(max(1, nl * W * B), dtype=torch.int32, device=dev)   # probe results for owned (table, src, sample)
-            self.max_unique = max(1, nl * W * B)
+            self.pos = torch.zeros(max(1, len(self.local_tables) * self.world * B), dtype=torch.int32, device=dev)   # probe results for owned (table, src, sample)
         self.x0 = z(B, _pad8(self.cfg.num_dense))
         for L in self.bot:
             L.a = z(B, L.N); L.y = z(B, L.N); L.dy = z(B, L.N); L.da = z(B, L.N)
@@ -267,29 +235,14 @@ class DLRMEngine:
         self.prob = z(B, dt=f32)
         self.loss = z(1, dt=f32)
         self.dx = z(B, D)
-        self.ctx.ensure(self.max_unique)
-        self.ctx.claimed_upper = 0
         self._l2_scratch = None
-
-    def _init_hyper(self) -> None:
-        cfg = self.cfg
-        hp = OptHyper()
-        hp.kind, hp.lr = self.kind, cfg.learning_rate
-        hp.beta1, hp.beta2, hp.epsilon = 0.9, 0.999, 1e-8
-        hp.beta1_power, hp.beta2_power = 0.9, 0.999
-        hp.weight_decay, hp.l1, hp.l2, hp.l2_shrinkage, hp.lr_power = 0.0, 0.0, 0.0, 0.0, -0.5
-        hp.decay_rate, hp.decay_baseline, hp.init_accum = 0.9, cfg.initial_accumulator_value, cfg.initial_accumulator_value
-        hp.decay_step, hp.global_step = 100000, 0
-        self.hp = hp
-        self.ctx.set_hyper(hp)
-        self.hp_dev = self.ctx.hp_dev
-        self.step_ptr = C.c_void_p(self.hp_dev.data_ptr() + OptHyper.global_step.offset)
 
     # ------------------------------------------------------------------------------------------------
     # kernel-call helpers (every call is one launch of one of OUR kernels; counted for gpu_launches)
     # ------------------------------------------------------------------------------------------------
-    def _s(self):
-        return None if self.emu else C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+    launches = property(_eg.engine_launches)
+    loss_value = _eg.loss_value
+    save, restore = save_engine, restore_engine      # training-state checkpoints: full / incremental save, restore under any world size
 
     # ---- optional per-phase CUDA-event timing of EAGER steps (DEEPREC_STEP_TIMING=1; never inside a captured graph) ------------
     def _tick(self, name: str) -> None:
@@ -314,9 +267,9 @@ class DLRMEngine:
                     out[nm] = sum(ts) / len(ts)
         return out
 
-    def _call(self, fn, *args, n=1):
-        _chk(fn(*args, self._s()), fn.__name__)
-        self.launches += n
+    def _call(self, fn, *args):
+        _chk(fn(*args, stream(self.dev)), fn.__name__)
+        self._launches += 1
 
     def _gemm(self, A, lda, Bm, ldb, M, N, K, bias, relu, mask, ldm, out, ldc, aux_mode=None, S1=None, S2=None):
         """out[M,N] = A[M,K] Bm[N,K]^T (+bias)(relu); aux ``mask`` with aux_mode 1 = ReLU-backward mask, 2 = S2 partner;
@@ -342,10 +295,7 @@ class DLRMEngine:
             self.comm.lookup_forward(self, train)
             return
         self._tick("e0")
-        self.sp.dedup(self.ids)
-        self._tick("e_dedup")
-        self.sp.lookup(self.ctx, self.tmap_local, train)
-        self.launches += 2
+        self.group.forward(self.ids, train, self._tick)
 
     def _embedding_backward(self) -> None:
         """Owner: pull the sources' pre-reduced gradient rows, then the row-wise optimizer over this step's distinct keys."""
@@ -353,15 +303,7 @@ class DLRMEngine:
             self.comm.sparse_backward(self)
             return
         self._tick("g0")
-        self.sp.segsum(self.demb)        # requester: per-key pre-reduction of my gradient rows (fp32) -> GRAD flags
-        self._tick("g_segsum")
-        self.sp.reset()                  # every owner has read my bucket lists / counts (ROWS flags seen by the interaction kernel)
-        self._tick("g_reset")
-        self.sp.grad(self.ctx, self.tmap_local)
-        self._tick("g_grad")
-        self._call(self.lib.dr_cuda_sparse_apply, ptr(self.ctx.structs()), ptr(self.ctx.ulist), ptr(self.ctx.nuniq), self.ctx.ulist.numel(),
-                   ptr(self.ctx.gsum), self.D, ptr(self.hp_dev), self.max_unique, 1, n=2)
-        self.launches += 3
+        self.group.backward(self.demb, self._tick)
 
     def _bn_fold(self, L, Ln, train: bool) -> None:
         """finalize BatchNorm(L) from the fused epilogue statistics and fold it into the next Linear (Ln)."""
@@ -517,10 +459,7 @@ class DLRMEngine:
             self._call(lib.dr_cuda_dense_apply, ptr(self.params), ptr(self.grads), ptr(self.s0) if self.s0 is not None else None,
                        ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, None)
         self._pack_weights()
-        self._call(lib.dr_cuda_advance_hyper, ptr(self.hp_dev))
-        if self.uf:
-            self.sp.step_end()
-            self.launches += 1
+        self.group.end_step()
         self._tick("u1")
 
     def _step_body(self) -> None:
@@ -562,7 +501,7 @@ class DLRMEngine:
         """One optimizer step on the batch currently in the input buffers (graph replay when captured)."""
         if self._graph is not None:
             self._graph.replay()
-            self.launches += self.launches_per_step
+            self._launches += self.launches_per_step
         else:
             self.train_step_eager()
 
@@ -572,36 +511,12 @@ class DLRMEngine:
         self._forward(False)
         self._head(False)
         if self.uf:
-            self.sp.reset()
-            if self.world > 1:       # rendezvous before any rank overwrites its bucket lists again
-                self.sp.signal(3)
-                self.comm.wait_dense(self.sp)
-            self.sp.step_end()
+            self.group.forward_only_tail()
         return self.prob
-
-    def loss_value(self, global_mean: bool = True) -> float:
-        """Loss of the last step: the mean over the GLOBAL batch (each rank holds its partial sum / (B * world))."""
-        v = self.loss.clone()
-        if global_mean and self.world > 1:
-            if hasattr(self.comm, "host_all_reduce"):          # emulation: ranks are threads (parallel/emu_comm.py)
-                self.comm.host_all_reduce(v)
-            else:
-                import torch.distributed as dist
-                dist.all_reduce(v)
-        return float(v.item())
 
     def global_step(self) -> int:
         raw = bytes(self.hp_dev.cpu().numpy().tobytes())
         return int(OptHyper.from_buffer_copy(raw).global_step)
-
-    # ---- training-state checkpoints (checkpoint/engine_ckpt.py): full / incremental save, restore under any world size ----------
-    def save(self, save_path: str, incremental: bool = False, max_to_keep: int = 5) -> str:
-        from ..checkpoint.engine_ckpt import save_engine
-        return save_engine(self, save_path, incremental=incremental, max_to_keep=max_to_keep)
-
-    def restore(self, save_path: str, step=None, replay_incremental: bool = True) -> int:
-        from ..checkpoint.engine_ckpt import restore_engine
-        return restore_engine(self, save_path, step=step, replay_incremental=replay_incremental)
 
     def l2_flush(self) -> None:
         if self._l2_scratch is None:

@@ -23,22 +23,18 @@ Reference: modelzoo/deepfm/train.py:143-191, modelzoo/din/train.py:143-375 (mode
 """
 from __future__ import annotations
 
-import ctypes as C
-import math
-from typing import Callable, Dict, List, Optional, Sequence
+from typing import Callable, Dict, Optional, Sequence
 
 import torch
 from torch import nn
 
 from .. import _native
-from .._native import EvConfig, OptHyper, ptr
-from ..ops.device_table import DeviceTable, _chk, _next_pow2, get_context
-from ..optim.optimizers import OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_ADAM, OPT_ADAM_ASYNC, OPT_ADAMW, OPT_FTRL, OPT_SGD
-from ..parallel.sparse_pipeline import SparsePipeline
-
-_OPT_KIND = {"sgd": OPT_SGD, "gradientdescent": OPT_SGD, "adagrad": OPT_ADAGRAD, "adagraddecay": OPT_ADAGRAD_DECAY,
-             "adam": OPT_ADAM, "adamasync": OPT_ADAM_ASYNC, "adamw": OPT_ADAMW, "ftrl": OPT_FTRL}
-_OPT_SLOTS = {OPT_SGD: 0, OPT_ADAGRAD: 1, OPT_ADAGRAD_DECAY: 1, OPT_ADAM: 2, OPT_ADAM_ASYNC: 2, OPT_ADAMW: 2, OPT_FTRL: 2}
+from .._native import ptr
+from ..checkpoint.engine_ckpt import restore_engine, save_engine
+from ..ops.device_table import _chk
+from ..optim.optimizers import OPT_KIND, OPT_SLOTS, slot0_init
+from . import embedding_group as _eg
+from .embedding_group import EmbeddingGroup, stream
 
 
 class FusedRecEngine:
@@ -70,44 +66,30 @@ class FusedRecEngine:
         if not self.emu:
             _native.set_device(self.dev.index)
         self.B, self.D, self.C, self.T = batch_size, embedding_dim, len(col_table), len(table_rows)
-        self.kind = _OPT_KIND[optimizer.lower()]
-        self.lr, self.init_acc = learning_rate, initial_accumulator_value
+        self.kind = OPT_KIND[optimizer.lower()]
         self.loss_fn = loss_fn or (lambda logits, labels: nn.functional.binary_cross_entropy_with_logits(logits.float(), labels))
-        self.launches, self._graph = 0, None
+        self._launches, self._graph = 0, None
         self.micro = max(1, int(micro_batch_num))
         if batch_size % self.micro:
             raise ValueError(f"micro_batch_num {self.micro} must divide the batch size {batch_size}")
         dev = self.dev
-        # ---- tables: this rank's hash(key) % world shard of every table
-        self.ctx = get_context(dev, self.D, owner=id(self) & 0x7FFFFFFF)
-        ns = _OPT_SLOTS[self.kind]
-        self.tables = self._make_tables(self.D, self.kind, id(self) & 0x7FFFFFFF, seed + 17, col_table, table_rows, tiered, filter_freq, steps_to_live,
-                                        max_rows_per_table)
-        self.tmap = torch.tensor([self.tables[t].gid for t in range(self.T)], dtype=torch.int32, device=dev)
-        self.tiers = {}
-        if tiered:
-            if world_size > 1 and (comm is None or not hasattr(comm, "symmetric")):
-                raise ValueError("tiered tables with world_size > 1 need a peer-memory communicator (parallel.p2p.P2PComm)")
-            from ..ops.tier_manager import DeviceTierManager
-            for t, o in sorted(tiered.items()):            # sorted: the symmetric allocations inside are collective calls
-                cols = torch.tensor([c for c, ct in enumerate(col_table) if ct == t], dtype=torch.int64, device=dev)
-                n_ids = int(cols.numel()) * batch_size
-                mgr = DeviceTierManager(self.tables[t], int(o["cache_rows"]), strategy=int(o.get("strategy", 0)), pad_key=pad_key,
-                                        max_batch_keys=max(1 << 16, (2 if world_size == 1 else 4) * n_ids),
-                                        comm=comm if world_size > 1 else None, ids_per_prefetch=n_ids)
-                self.tiers[t] = (mgr, cols)
+        # ---- embedding groups: this rank's hash(key) % world shard of every table, each group with its own step context (owner key),
+        #      optimizer and pipeline
+        owner = id(self) & 0x7FFFFFFF
+        group = lambda dim, kind, lr, owner, seed, tiered, is_linear: EmbeddingGroup(
+            dev, dim, kind, lr, initial_accumulator_value, owner, seed, range(self.T), table_rows, batch_size, col_table=col_table, rank=rank,
+            world=world_size, comm=comm, pad_key=pad_key, filter_freq=filter_freq, steps_to_live=steps_to_live,
+            max_rows_per_table=max_rows_per_table, tiered=tiered, is_linear=is_linear)
+        self.deep = group(self.D, self.kind, learning_rate, owner, seed + 17, tiered, False)
+        self.tables, self.tiers, self.sp, self.hp_dev = self.deep.tables, self.deep.tiers, self.deep.sp, self.deep.hp_dev
         self._host_step = 0
-        # ---- sparse pipeline + static buffers
-        self.sp = SparsePipeline(dev, rank, world_size, list(col_table), self.T, batch_size, self.D, comm=comm, pad_key=pad_key)
+        # ---- static buffers
         self.ids = torch.full((self.C, batch_size), pad_key, dtype=torch.int64, device=dev)
         self.labels = torch.zeros(batch_size, dtype=torch.float32, device=dev)
         self.dense: Dict[str, torch.Tensor] = {k: torch.zeros(*shape, dtype=dt, device=dev) for k, (shape, dt) in (dense_inputs or {}).items()}
         self.emb_out = torch.zeros(batch_size, self.C, self.D, dtype=torch.bfloat16, device=dev)
         self.demb = torch.zeros(self.C, batch_size, self.D, dtype=torch.bfloat16, device=dev)
         self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
-        self.max_unique = max(1, self.sp.Btot * min(world_size, 2))
-        self.ctx.ensure(self.max_unique)
-        self.ctx.claimed_upper = 0
         # ---- dense parameters / gradients -> one flat buffer each
         self.net.to(dev)
         plist = [p for p in self.net.parameters() if p.requires_grad]
@@ -134,115 +116,37 @@ class FusedRecEngine:
                 dist.broadcast(self.params, 0)
                 for b in self.net.buffers():
                     dist.broadcast(b, 0)
-        self.s0 = torch.full((self.P,), initial_accumulator_value if self.kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0,
-                             dtype=torch.float32, device=dev) if ns > 0 else None
+        ns = OPT_SLOTS[self.kind]
+        self.s0 = torch.full((self.P,), slot0_init(self.kind, initial_accumulator_value), dtype=torch.float32, device=dev) if ns > 0 else None
         self.s1 = torch.zeros(self.P, dtype=torch.float32, device=dev) if ns > 1 else None
-        self.ctx.set_hyper(self._hyper(self.kind, learning_rate))
-        self.hp_dev = self.ctx.hp_dev
-        # ---- linear group: its own tables, step context (owner key distinct from the deep group's, whatever its dim), optimizer and pipeline
-        self.linear = bool(linear)
-        if self.linear:
-            self.lin_kind = _OPT_KIND[(linear_optimizer or optimizer).lower()]
-            self.lin_lr = learning_rate if linear_learning_rate is None else linear_learning_rate
-            lin_owner = -1 - (id(self) & 0x7FFFFFFF)
-            self.lin_ctx = get_context(dev, 4, owner=lin_owner)
-            self.lin_tables = self._make_tables(4, self.lin_kind, lin_owner, seed + 29, col_table, table_rows, None, filter_freq, steps_to_live,
-                                                max_rows_per_table)
-            self.lin_tmap = torch.tensor([self.lin_tables[t].gid for t in range(self.T)], dtype=torch.int32, device=dev)
-            self.lin_sp = SparsePipeline(dev, rank, world_size, list(col_table), self.T, batch_size, 4, comm=comm, pad_key=pad_key)
+        # ---- linear group: dim-4 tables over the same id columns, owner key distinct from the deep group's (whatever its dim)
+        self.linear = None
+        if linear:
+            self.linear = group(4, OPT_KIND[(linear_optimizer or optimizer).lower()], learning_rate if linear_learning_rate is None else linear_learning_rate,
+                                -1 - owner, seed + 29, None, True)
+            self.lin_tables, self.lin_hp_dev = self.linear.tables, self.linear.hp_dev
             self.lin_out = torch.zeros(batch_size, dtype=torch.float32, device=dev)
             self.lin_dlogit = torch.zeros(batch_size, dtype=torch.float32, device=dev)
-            self.lin_max_unique = max(1, self.lin_sp.Btot * min(world_size, 2))
-            self.lin_ctx.ensure(self.lin_max_unique)
-            self.lin_ctx.claimed_upper = 0
-            self.lin_ctx.set_hyper(self._hyper(self.lin_kind, self.lin_lr))
-            self.lin_hp_dev = self.lin_ctx.hp_dev
+        self.groups = [self.deep] + ([self.linear] if linear else [])
         _native.device_sync(dev)
 
-    def _hyper(self, kind: int, lr: float) -> OptHyper:
-        hp = OptHyper()
-        hp.kind, hp.lr = kind, lr
-        hp.beta1, hp.beta2, hp.epsilon = 0.9, 0.999, 1e-8
-        hp.beta1_power, hp.beta2_power = 0.9, 0.999
-        hp.weight_decay, hp.l1, hp.l2, hp.l2_shrinkage, hp.lr_power = 0.0, 0.0, 0.0, 0.0, -0.5
-        hp.decay_rate, hp.decay_baseline, hp.init_accum = 0.9, self.init_acc, self.init_acc
-        hp.decay_step, hp.global_step = 100000, 0
-        return hp
-
-    def _make_tables(self, dim: int, kind: int, owner: int, seed: int, col_table, table_rows, tiered, filter_freq: int, steps_to_live: int,
-                     max_rows_per_table: int) -> Dict[int, DeviceTable]:
-        """This rank's hash(key) % world shard of every table of one embedding group (default rows: normal(0, 1/sqrt(dim)), seeded per table)."""
-        world_size, batch_size = self.world, self.B
-        ns = _OPT_SLOTS[kind]
-        ia = self.init_acc
-        slot_init = [ia if kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0, 0.0, 0.0, 0.0]
-        tables: Dict[int, DeviceTable] = {}
-        g = torch.Generator()
-        for t, card in enumerate(table_rows):
-            card = int(card)
-            if world_size > 1:
-                card = card // world_size + card // (8 * world_size) + 1024
-            c = EvConfig()
-            c.dim, c.num_slots, c.has_scalars = dim, ns, int(kind == OPT_ADAGRAD_DECAY)
-            c.init_capacity = card
-            c.filter_type, c.filter_freq = (1, filter_freq) if filter_freq > 0 else (0, 0)
-            c.bloom_counter_bits = 32
-            c.steps_to_live, c.l2_weight_threshold = steps_to_live, -1.0
-            c.default_value_dim, c.default_value_no_permission = 4096, 0.0
-            c.record_freq = c.record_version = 1
-            c.storage_type = 1
-            for i in range(4):
-                c.slot_init[i] = slot_init[i]
-            g.manual_seed(seed + 1000 * t)
-            dm = torch.empty(4096, dim).normal_(0.0, 1.0 / math.sqrt(dim), generator=g)
-            rows = max(1024, min(card, max_rows_per_table))
-            if tiered and t in tiered:            # HBM tier = cache: R rows + head-room for the keys two steps can create before an eviction lands
-                ncols_t = sum(1 for ct in col_table if ct == t)
-                # (world > 1: a rank owns ~1/W of the W batches' keys -- the same expectation, plus slack for the imbalance of hash(key) % W)
-                rows = int(tiered[t]["cache_rows"]) + (2 if world_size == 1 else 3) * ncols_t * batch_size + 4096
-                card = rows
-            cap = _next_pow2(max(2048, 2 * min(card, rows)))
-            tables[t] = DeviceTable(c, dm, self.dev, capacity=cap, row_capacity=rows, owner=owner)
-        return tables
+    launches = property(_eg.engine_launches)
+    loss_value = _eg.loss_value
+    save, restore = save_engine, restore_engine      # training-state checkpoints: full / incremental save, restore under any world size
 
     # ------------------------------------------------------------------------------------------------------------------
-    def _s(self):
-        return None if self.emu else C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
-
     def _sparse_forward(self, train: bool) -> None:
-        self.sp.dedup(self.ids)
-        self.sp.lookup(self.ctx, self.tmap, train)
+        self.deep.forward(self.ids, train)
         self.sp.gather(self.emb_out)                  # waits for every owner's ROWS flag in-kernel
-        self.launches += 3
         if self.linear:
-            self.lin_sp.dedup(self.ids)
-            self.lin_sp.lookup(self.lin_ctx, self.lin_tmap, train)
-            self.lin_sp.linear_fwd(self.lin_out)      # waits for every owner's ROWS flag in-kernel
-            self.launches += 3
-
-    def _linear_rendezvous(self) -> None:
-        """world > 1: the linear pipeline's DENSE flags, raised and awaited once per step as the deep pipeline's are -- no rank starts its next
-        linear dedup (which zeroes the ugrad rows the owners pull) before every owner has finished this step's pull."""
-        if self.linear and self.world > 1:
-            self.lin_sp.signal(3)
-            self.comm.wait_dense(self.lin_sp)
-            self.launches += 2
+            self.linear.forward(self.ids, train)
+            self.linear.sp.linear_fwd(self.lin_out)   # waits for every owner's ROWS flag in-kernel
 
     def _sparse_backward(self) -> None:
-        self.sp.segsum(self.demb)
-        self.sp.reset()
-        self.sp.grad(self.ctx, self.tmap)
-        _chk(self.lib.dr_cuda_sparse_apply(ptr(self.ctx.structs()), ptr(self.ctx.ulist), ptr(self.ctx.nuniq), self.ctx.ulist.numel(), ptr(self.ctx.gsum),
-                                           self.D, ptr(self.hp_dev), self.max_unique, 1, self._s()), "sparse_apply")
-        self.launches += 5
+        self.deep.backward(self.demb)
         if self.linear:
-            self.lin_sp.linear_bwd(self.lin_dlogit)
-            self.lin_sp.reset()
-            self.lin_sp.grad(self.lin_ctx, self.lin_tmap)
-            _chk(self.lib.dr_cuda_sparse_apply(ptr(self.lin_ctx.structs()), ptr(self.lin_ctx.ulist), ptr(self.lin_ctx.nuniq), self.lin_ctx.ulist.numel(),
-                                               ptr(self.lin_ctx.gsum), 4, ptr(self.lin_hp_dev), self.lin_max_unique, 1, self._s()), "sparse_apply")
-            self.launches += 4
-            self._linear_rendezvous()
+            self.linear.backward(self.lin_dlogit)
+            self.linear.rendezvous()                  # the deep pipeline's DENSE flags are raised with the dense all-reduce
 
     def _linear_leaf(self, lo: int, hi: int):
         """The linear logits of samples [lo, hi) as a leaf of the dense net's graph, and the keyword that hands it to forward_fn."""
@@ -295,15 +199,11 @@ class FusedRecEngine:
             self.comm.dense_allreduce_update(self)
         else:
             _chk(self.lib.dr_cuda_dense_apply(ptr(self.params), ptr(self.grads), ptr(self.s0) if self.s0 is not None else None,
-                                              ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, None, self._s()), "dense_apply")
-            self.launches += 1
-        _chk(self.lib.dr_cuda_advance_hyper(ptr(self.hp_dev), self._s()), "advance_hyper")
-        self.sp.step_end()
-        self.launches += 2
-        if self.linear:
-            _chk(self.lib.dr_cuda_advance_hyper(ptr(self.lin_hp_dev), self._s()), "advance_hyper")
-            self.lin_sp.step_end()
-            self.launches += 2
+                                              ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, None, stream(self.dev)),
+                 "dense_apply")
+            self._launches += 1
+        for g in self.groups:
+            g.end_step()
 
     # ------------------------------------------------------------------------------------------------------------------
     def load_batch(self, ids: torch.Tensor, labels: torch.Tensor, dense: Optional[Dict[str, torch.Tensor]] = None, non_blocking: bool = True) -> None:
@@ -321,8 +221,9 @@ class FusedRecEngine:
         is captured into one CUDA graph."""
         if self.emu:                                  # kernels run synchronously on the host: the eager step IS the step
             for _ in range(warmup):
+                n0 = self.launches
                 self._step_body()
-            self.launches_per_step = 0
+            self.launches_per_step = self.launches - n0
             return
         cur = torch.cuda.current_stream(self.dev)
         side = torch.cuda.Stream(device=self.dev)
@@ -361,36 +262,10 @@ class FusedRecEngine:
         self._sparse_forward(False)
         kw = {"linear": self.lin_out} if self.linear else {}
         out = torch.sigmoid(self.forward_fn(self.net, self.dense, self.emb_out, self.ids, **kw).float())
-        self.sp.reset()
-        if self.world > 1:
-            self.sp.signal(3)
-            self.comm.wait_dense(self.sp)
-        self.sp.step_end()
-        if self.linear:
-            self.lin_sp.reset()
-            self._linear_rendezvous()
-            self.lin_sp.step_end()
+        for g in self.groups:
+            g.forward_only_tail()
         self.net.train(was)
         return out
-
-    # ---- training-state checkpoints (checkpoint/engine_ckpt.py): full / incremental save, restore under any world size ----------
-    def save(self, save_path: str, incremental: bool = False, max_to_keep: int = 5) -> str:
-        from ..checkpoint.engine_ckpt import save_engine
-        return save_engine(self, save_path, incremental=incremental, max_to_keep=max_to_keep)
-
-    def restore(self, save_path: str, step=None, replay_incremental: bool = True) -> int:
-        from ..checkpoint.engine_ckpt import restore_engine
-        return restore_engine(self, save_path, step=step, replay_incremental=replay_incremental)
-
-    def loss_value(self, global_mean: bool = True) -> float:
-        v = self.loss.clone()
-        if global_mean and self.world > 1:
-            if hasattr(self.comm, "host_all_reduce"):
-                self.comm.host_all_reduce(v)
-            else:
-                import torch.distributed as dist
-                dist.all_reduce(v)
-        return float(v.item())
 
 
 # ---- adapters for the model zoo ------------------------------------------------------------------------------------------------

@@ -22,6 +22,28 @@ from ..embedding_variable import DynamicEmbeddingVariable, EmbeddingVariable, Pa
 
 OPT_SGD, OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_ADAM, OPT_ADAM_ASYNC, OPT_ADAMW, OPT_FTRL, OPT_ADAM_ASYNC_RMSPROP = range(8)
 
+# ---- the fused engines' optimizer table (models/dlrm_engine.py, models/rec_engine.py): one rule for the dense net and the tables -------
+OPT_KIND = {"sgd": OPT_SGD, "gradientdescent": OPT_SGD, "adagrad": OPT_ADAGRAD, "adagraddecay": OPT_ADAGRAD_DECAY,
+            "adam": OPT_ADAM, "adamasync": OPT_ADAM_ASYNC, "adamw": OPT_ADAMW, "ftrl": OPT_FTRL}
+OPT_SLOTS = {OPT_SGD: 0, OPT_ADAGRAD: 1, OPT_ADAGRAD_DECAY: 1, OPT_ADAM: 2, OPT_ADAM_ASYNC: 2, OPT_ADAMW: 2, OPT_FTRL: 2}
+
+
+def slot0_init(kind: int, initial_accumulator_value: float) -> float:
+    """The value slot 0 starts at: the accumulator of Adagrad / AdagradDecay / FTRL, the first moment (0) otherwise."""
+    return initial_accumulator_value if kind in (OPT_ADAGRAD, OPT_ADAGRAD_DECAY, OPT_FTRL) else 0.0
+
+
+def engine_hyper(kind: int, lr: float, initial_accumulator_value: float) -> OptHyper:
+    """The fused engines' hyper-parameters: the reference optimizers' defaults at learning rate ``lr``, global step 0."""
+    hp = OptHyper()
+    hp.kind, hp.lr = kind, lr
+    hp.beta1, hp.beta2, hp.epsilon = 0.9, 0.999, 1e-8
+    hp.beta1_power, hp.beta2_power = 0.9, 0.999
+    hp.weight_decay, hp.l1, hp.l2, hp.l2_shrinkage, hp.lr_power = 0.0, 0.0, 0.0, 0.0, -0.5
+    hp.decay_rate, hp.decay_baseline, hp.init_accum = 0.9, initial_accumulator_value, initial_accumulator_value
+    hp.decay_step, hp.global_step = 100000, 0
+    return hp
+
 
 class GlobalStep:
     """``tf.train.get_or_create_global_step`` analogue."""

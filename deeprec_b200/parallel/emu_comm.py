@@ -58,6 +58,7 @@ class EmuComm:
         self.dev = torch.device("cpu")
         self._n = 0
         self._buffers = []
+        self.launches = 0            # kernels of the step's all-reduce / rendezvous calls (the pipeline counts its own DENSE signal)
 
     def symmetric(self, nbytes: int) -> _EmuSymmetricBuffer:
         """Collective: every rank thread calls it in the same order."""
@@ -84,13 +85,14 @@ class EmuComm:
                                                          ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), None)
         if rc != 0:
             raise RuntimeError(f"allreduce_apply failed ({rc})")
-        eng.launches += 2
+        self.launches += 1
 
     def wait_dense(self, sp) -> None:
         from .. import _native
         rc = _native.cuda().dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, None, None, None, 0, None, None, sp.sync_ref(), None)
         if rc != 0:
             raise RuntimeError(f"wait_dense failed ({rc})")
+        self.launches += 1
 
     def host_broadcast(self, tensors, src: int = 0) -> None:
         """Rank ``src``'s values into every rank's tensors (engine construction)."""

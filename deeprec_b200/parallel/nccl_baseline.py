@@ -13,13 +13,14 @@ swaps the dense net for cuBLAS (torch.nn + autocast bf16) to give the full "NCCL
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Tuple
 
 import torch
 import torch.distributed as dist
 
 from .. import _native
-from .._native import ptr
+from .._native import OptHyper, ptr
 
 
 def _chk(rc, what):
@@ -35,11 +36,13 @@ class NcclComm:
             out.copy_(inp)
         else:
             dist.all_to_all_single(out, inp, recv_counts, send_counts, group=self.group)
+        self.launches += 1
 
     def __init__(self, rank: int, world: int, dev: torch.device, group=None):
         self.rank, self.world, self.dev, self.group = rank, world, dev, group
         self.lib = _native.cuda()
         _native.set_device(dev.index)
+        self.launches = 0            # kernels and collectives this communicator launches (the engine's embedding group counts its apply)
 
     def alloc_grads(self, P: int) -> torch.Tensor:
         return torch.zeros(P, dtype=torch.float32, device=self.dev)
@@ -70,7 +73,9 @@ class NcclComm:
         nb.grad_recv = torch.empty(max(1, W * nl * B), D, dtype=torch.bfloat16, device=self.dev)
         nb.perm = torch.cat(nb.idx) if eng.T else torch.empty(0, dtype=torch.int64, device=self.dev)   # table order grouped by owner
         # offsets for table-index search inside the kernels: segment = (src rank, local table) of size B
-        nb.tmap = eng.tmap_local.repeat(W).contiguous() if nl else eng.tmap_local                       # [W * nl]
+        g = eng.group
+        nb.tmap = g.tmap.repeat(W).contiguous() if nl else g.tmap                                     # [W * nl]
+        nb.step_ptr = C.c_void_p(g.hp_dev.data_ptr() + OptHyper.global_step.offset)
         eng._nb = nb
 
     def lookup_forward(self, eng, train: bool) -> None:
@@ -80,42 +85,46 @@ class NcclComm:
         s = torch.cuda.current_stream(self.dev).cuda_stream
         # 1. pack ids by owner, NCCL all-to-all (C2)
         nb.keys_send.copy_(eng.ids.index_select(0, nb.perm).view(-1))
+        self.launches += 1
         self._a2a(nb.keys_recv[: W * nl * B], nb.keys_send, nb.recv_counts_ids, nb.send_counts_ids)
         # 2. probe + gather as separate kernels (K1/K3)
         n = W * nl * B
         if n:
-            st = eng.ctx.structs()
-            _chk(lib.dr_cuda_table_lookup(ptr(st), ptr(nb.tmap), W * nl, ptr(nb.keys_recv), None, B, n, int(train), eng.step_ptr, ptr(eng.pos),
-                                          ptr(eng.ctx.ulist) if train else None, ptr(eng.ctx.nuniq) if train else None,
-                                          eng.ctx.ulist.numel() if train else 0, s), "lookup")
+            ctx = eng.group.ctx
+            st = ctx.structs()
+            _chk(lib.dr_cuda_table_lookup(ptr(st), ptr(nb.tmap), W * nl, ptr(nb.keys_recv), None, B, n, int(train), nb.step_ptr, ptr(eng.pos),
+                                          ptr(ctx.ulist) if train else None, ptr(ctx.nuniq) if train else None,
+                                          ctx.ulist.numel() if train else 0, s), "lookup")
             _chk(lib.dr_cuda_table_gather(ptr(st), ptr(nb.tmap), W * nl, D, ptr(nb.keys_recv), ptr(eng.pos), None, B, n, ptr(nb.rows_send), 1, 0, 0, 1, s), "gather")
+            self.launches += 2
         # 3. NCCL all-to-all of the vectors (C3) + un-permute into feature-major order (S2 reorderKernel)
         self._a2a(nb.rows_recv, nb.rows_send[: W * nl * B], [c for c in nb.send_counts_ids], [c for c in nb.recv_counts_ids])
         eng.emb.index_copy_(0, nb.perm, nb.rows_recv.view(eng.T, B, D))
-        eng.launches += 6
+        self.launches += 1
 
     def sparse_backward(self, eng) -> None:
         nb, W, B, D, lib = eng._nb, self.world, eng.B, eng.D, self.lib
         nl = len(nb.owned[self.rank])
         s = torch.cuda.current_stream(self.dev).cuda_stream
         nb.grad_send.copy_(eng.demb.index_select(0, nb.perm).view(-1, D))
+        self.launches += 1
         self._a2a(nb.grad_recv[: W * nl * B], nb.grad_send, nb.recv_counts_ids, nb.send_counts_ids)     # C4
         n = W * nl * B
         if n:
-            st = eng.ctx.structs()
-            _chk(lib.dr_cuda_sparse_accumulate(ptr(st), ptr(nb.tmap), W * nl, D, ptr(eng.pos), None, B, n, ptr(nb.grad_recv), 1, 0, 0, 1, None, None,
-                                               ptr(eng.ctx.gsum), s), "accumulate")
-        _chk(lib.dr_cuda_sparse_apply(ptr(eng.ctx.structs()), ptr(eng.ctx.ulist), ptr(eng.ctx.nuniq), eng.ctx.ulist.numel(), ptr(eng.ctx.gsum), D,
-                                      ptr(eng.hp_dev), eng.max_unique, 1, s), "sparse_apply")
-        eng.launches += 5
+            ctx = eng.group.ctx
+            _chk(lib.dr_cuda_sparse_accumulate(ptr(ctx.structs()), ptr(nb.tmap), W * nl, D, ptr(eng.pos), None, B, n, ptr(nb.grad_recv), 1, 0, 0, 1,
+                                               None, None, ptr(ctx.gsum), s), "accumulate")
+            self.launches += 1
+        eng.group.apply()
 
     def dense_allreduce_update(self, eng) -> None:
         if self.world > 1:
             dist.all_reduce(eng.grads, group=self.group)                                                                              # C1
+            self.launches += 1
         s = torch.cuda.current_stream(self.dev).cuda_stream
         _chk(self.lib.dr_cuda_dense_apply(ptr(eng.params), ptr(eng.grads), ptr(eng.s0) if eng.s0 is not None else None,
                                           ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), 1.0, None, s), "dense_apply")
-        eng.launches += 2
+        self.launches += 1
 
 
 class BaselineDLRM:

@@ -119,6 +119,7 @@ class P2PComm:
         self.signals = SymmetricBuffer(self, 16 * 16 * 4)
         self.epochs = torch.zeros(16, dtype=torch.int32, device=dev)
         self._buffers: List[SymmetricBuffer] = [self.signals]
+        self.launches = 0            # kernels of the step's all-reduce / rendezvous calls (the pipeline counts its own DENSE signal)
         dist.barrier(group=group)
 
     def _s(self):
@@ -217,25 +218,27 @@ class P2PComm:
             _chk(self.lib.dr_nvls_allreduce_2phase(vp(self.nvls["mc"]), vp(self.nvls["local"]), self.rank, self.world, ptr(eng.params),
                                                    ptr(eng.s0) if eng.s0 is not None else None, ptr(eng.s1) if eng.s1 is not None else None, eng.P,
                                                    ptr(eng.hp_dev), sp.sync_ref(), self._s()), "nvls_allreduce_2phase")
-            eng.launches += 3
+            self.launches += 2
             return
         if getattr(self, "nvls", None) is not None:     # in-switch reduction: one multimem.ld_reduce per 16 B instead of W peer loads
             _chk(self.lib.dr_nvls_allreduce_apply(vp(self.nvls["mc"]), ptr(eng.params), ptr(eng.s0) if eng.s0 is not None else None,
                                                   ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), self._s()),
                  "nvls_allreduce_apply")
-            eng.launches += 2
+            self.launches += 1
             return
         _chk(self.lib.dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, ptr(eng.params), ptr(eng.s0) if eng.s0 is not None else None,
                                                    ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), self._s()),
              "allreduce_apply")
-        eng.launches += 2
+        self.launches += 1
 
     def wait_dense(self, sp) -> None:
         """In-kernel rendezvous on the DENSE flags without any reduction (forward-only passes)."""
         if getattr(self, "nvls", None) is not None:
             _chk(self.lib.dr_nvls_allreduce_apply(vp(self.nvls["mc"]), None, None, None, 0, None, None, sp.sync_ref(), self._s()), "wait_dense")
-            return
-        _chk(self.lib.dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, None, None, None, 0, None, None, sp.sync_ref(), self._s()), "wait_dense")
+        else:
+            _chk(self.lib.dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, None, None, None, 0, None, None, sp.sync_ref(), self._s()),
+                 "wait_dense")
+        self.launches += 1
 
     def allreduce(self, out: torch.Tensor, two_phase: bool = False) -> None:
         """All-reduce of the symmetric grads buffer into ``out`` (tests / metrics).  ``two_phase`` (NVLS only) reduces IN PLACE: the
