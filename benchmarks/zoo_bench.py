@@ -30,9 +30,10 @@ from deeprec_b200.models.zoo import CRITEO_MODELS, build_model  # noqa: E402
 
 
 def engine_main(a):
-    """BASELINE configs #3 (DeepFM) and #4 (DIN, 1B-id behaviour table with admission) on the fused engine, 1-8 GPUs."""
+    """BASELINE configs #3 (DeepFM) and #4 (DIN, 1B-id behaviour table with admission) on the fused engine, 1-8 GPUs; DSSM and the
+    multi-task models (ESMM, MMoE, DBMTL, PLE, SimpleMultiTask) over pooled history bags."""
     import torch.distributed as dist
-    from deeprec_b200.models.rec_engine import criteo_engine, din_engine, din_ids
+    from deeprec_b200.models.rec_engine import POOLED_SEQ_MODELS, criteo_engine, din_engine, din_ids, pooled_seq_engine, taobao_engine_batch
     world, rank, lr = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0")), int(os.environ.get("LOCAL_RANK", "0"))
     from deeprec_b200.utils.affinity import bind_to_gpu_numa
     bound = bind_to_gpu_numa(lr)                                    # host threads (pinned buffers, OpenMP pool) next to the GPU
@@ -57,6 +58,15 @@ def engine_main(a):
             d, ids, y = criteo_batch(a.batch, 13, cards, seed=s * world + rank)
             host.append((ids.pin_memory(), y.pin_memory(), {"dense": d.pin_memory()}))
         extra = {}
+    elif name in POOLED_SEQ_MODELS:             # DSSM / multi-task: the behaviour history pooled into bags (sum) inside the sparse pipeline
+        eng = pooled_seq_engine(model, a.batch, 50, table_rows=(10_000_000, min(a.id_space, 200_000_000), 10_000), optimizer=a.optimizer,
+                                device=dev, rank=rank, world_size=world, comm=comm)
+        host = []
+        for s in range(n):
+            b = taobao_batch(a.batch, 50, 10_000_000, a.id_space, 10_000, seed=s * world + rank)
+            ids, y, _ = taobao_engine_batch(b) if eng.labels.dim() == 2 else (din_ids(b), b["labels"], None)
+            host.append((ids.pin_memory(), y.pin_memory(), None))
+        extra = {"item_id_space": a.id_space, "bags": "sum"}
     else:
         eng = din_engine(model, a.batch, 50, table_rows=(10_000_000, min(a.id_space, 200_000_000), 10_000), optimizer=a.optimizer,
                          filter_freq=a.filter_freq, steps_to_live=100000, device=dev, rank=rank, world_size=world, comm=comm,

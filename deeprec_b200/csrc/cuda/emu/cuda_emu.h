@@ -309,6 +309,8 @@ inline float __expf(float x) { return expf(x); }
 inline float __logf(float x) { return logf(x); }
 inline float __fdividef(float a, float b) { return a / b; }
 inline float __frcp_rn(float a) { return 1.f / a; }
+inline float __fsqrt_rn(float a) { return sqrtf(a); }
+inline float __fmul_rn(float a, float b) { return a * b; }
 inline float rsqrtf(float x) { return 1.f / sqrtf(x); }
 inline float __fmaf_rn(float a, float b, float c) { return fmaf(a, b, c); }
 inline float __saturatef(float x) { return x < 0.f ? 0.f : x > 1.f ? 1.f : x; }

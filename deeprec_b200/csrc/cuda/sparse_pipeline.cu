@@ -22,6 +22,9 @@
 //   k_sp_reset   (requester)  clears the touched scratch slots through the bucket lists (no 50 MB memset per step).
 //   k_sp_linear_fwd / k_sp_linear_bwd (requester)  a linear (wide) embedding group: the per-sample sum of element 0 of the unique rows,
 //                             and its fp32 gradient scattered into element 0 of ugrad -- in place of gather / segsum.
+//   k_sp_pool / k_sp_pool_segsum (requester)  multi-hot bags: runs of consecutive id columns pooled (sum / mean / sqrtn) into one [B, F, dim]
+//                             activation slot each, and the pooled gradient scaled back onto every column of its bag -- in place of gather /
+//                             segsum.
 //
 // With the bench's id distribution only ~15 % of the ids of a batch are distinct: NVLink traffic, owner-side probes and
 // owner-side atomics all shrink by that factor, and what is left on the requester is perfectly balanced across ranks.
@@ -60,6 +63,13 @@ struct DrSpGeom {
   int64_t B;
   int32_t dim, ldinv;
   int64_t pad_key;            // ids equal to this (or the reserved empty/tombstone keys) are padding: inv = -1
+};
+// Multi-hot bags: bag f pools the id columns [off[f], off[f+1]) into activation slot f; together the F bags cover the C columns in order.
+struct DrSpBags {
+  const int32_t* off;         // [F + 1]
+  const int32_t* comb;        // [F] 0 = sum, 1 = mean, 2 = sqrtn
+  const int32_t* col_bag;     // [C] bag of id column c
+  int32_t F;
 };
 }
 
@@ -388,6 +398,107 @@ __global__ void __launch_bounds__(256) k_sp_gather(const __nv_bfloat16* __restri
 }
 
 // -----------------------------------------------------------------------------------------------------------------
+// k_sp_pool (requester): out[b][f][:] = w * (sum over the live columns c of bag f of urow[inv[b][c]]), added in column order in fp32 and rounded
+// once to bf16.  n = the live ids of the bag: padding (inv < 0) neither adds nor counts, a key a CounterFilter has not admitted counts with its
+// no_permission row.  w = 1, 1/n or 1/sqrt(n) for sum / mean / sqrtn (correctly rounded), 0 for an empty bag; it is stored to w_out[f][b]
+// for the backward, which cannot cheaply recount n per column.  One LPR-lane group per (b, f), so the result does not depend on the grid.
+// Waits in-kernel for every owner's ROWS flag, like k_sp_gather.
+// -----------------------------------------------------------------------------------------------------------------
+template <int LPR>
+__global__ void __launch_bounds__(256) k_sp_pool(const __nv_bfloat16* __restrict__ urow, const int32_t* __restrict__ inv, int ldinv, int64_t B,
+                                                 DrSpBags bags, __nv_bfloat16* __restrict__ out, float* __restrict__ w_out, DrSpSync sync) {
+  pdl_sync();
+  sp_wait_all(sync, SP_CH_ROWS);
+  constexpr int dim = 4 * LPR;
+  const int lane = threadIdx.x % LPR;
+  const int F = bags.F;
+  const int64_t n = B * F;
+  for (int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / LPR; i < n; i += (int64_t)gridDim.x * blockDim.x / LPR) {
+    const int64_t b = i / F; const int f = (int)(i % F);
+    const int32_t* ib = inv + b * ldinv;
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    int live = 0;
+    for (int c = bags.off[f], ce = bags.off[f + 1]; c < ce; ++c) {
+      const int32_t gs = ib[c];
+      if (gs < 0) continue;
+      uint2 v;
+      DR_LD_V2_VOLATILE_U32(v, urow + (int64_t)gs * dim + 4 * lane);       // peer-written row: bypass L1, as k_sp_gather does
+      const float2 x = unpack_bf16x2(v.x), y = unpack_bf16x2(v.y);
+      a0 += x.x; a1 += x.y; a2 += y.x; a3 += y.y;
+      ++live;
+    }
+    const int comb = bags.comb[f];
+    const float w = live == 0 ? 0.f : comb == 0 ? 1.f : comb == 1 ? __frcp_rn((float)live) : __frcp_rn(__fsqrt_rn((float)live));
+    *reinterpret_cast<uint2*>(out + i * dim + 4 * lane) = make_uint2(pack_bf16x2(a0 * w, a1 * w), pack_bf16x2(a2 * w, a3 * w));
+    if (lane == 0) w_out[(int64_t)f * B + b] = w;
+  }
+}
+
+// -----------------------------------------------------------------------------------------------------------------
+// k_sp_pool_segsum (requester): k_sp_segsum for pooled bags.  Column c of sample b contributes its bag's gradient row dpool[bag(c)][b] times
+// w[bag(c)][b] (each element rounded once to fp32, no fused multiply-add), so with sum bags (w = 1) a key's sum equals k_sp_segsum's on the bag
+// gradient repeated per column, bit for bit.  Same unit of work (one warp = 32 consecutive samples of one column), match.any leader sums,
+// 64-bit fixed-point atomics; the last block raises GRAD.
+// -----------------------------------------------------------------------------------------------------------------
+template <int LPR /* dim / 4 */>
+__global__ void __launch_bounds__(256) k_sp_pool_segsum(const __nv_bfloat16* __restrict__ dpool /* [F][B][dim] */, const float* __restrict__ wbag /* [F][B] */,
+                                                        const int32_t* __restrict__ invT /* [C][B] */, DrSpGeom g, DrSpBags bags,
+                                                        unsigned long long* __restrict__ ugrad, DrSpSync sync) {
+  pdl_sync();
+  constexpr int dim = 4 * LPR;
+  constexpr int V = dim / 8;                                   // int4 (8 bf16) chunks per row
+  __shared__ __align__(16) int4 s_row[8][32][V];
+  __shared__ float s_w[8][32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t tiles = (g.B + 31) / 32;
+  const int64_t units = tiles * g.C;
+  for (int64_t u = (int64_t)blockIdx.x * 8 + warp; u < units; u += (int64_t)gridDim.x * 8) {
+    const int c = (int)(u / tiles);
+    const int64_t b = (u % tiles) * 32 + lane;
+    int32_t gs = -1;
+    if (b < g.B) gs = invT[(int64_t)c * g.B + b];
+    const bool live = gs >= 0;
+    const unsigned lm = __ballot_sync(0xffffffffu, live);
+    if (live) {
+      const int64_t r = (int64_t)bags.col_bag[c] * g.B + b;
+      const int4* src = reinterpret_cast<const int4*>(dpool + r * dim);
+#pragma unroll
+      for (int v = 0; v < V; ++v) s_row[warp][lane][v] = ld_nc_v4(src + v);
+      s_w[warp][lane] = wbag[r];
+    }
+    __syncwarp();
+    if (live) {
+      const unsigned same = __match_any_sync(lm, gs);
+      if (lane == __ffs(same) - 1) {                            // leader of this key inside the tile
+        float acc[dim];
+#pragma unroll
+        for (int d = 0; d < dim; ++d) acc[d] = 0.f;
+        for (unsigned m = same; m; m &= m - 1) {
+          const int src_lane = __ffs(m) - 1;
+          const float w = s_w[warp][src_lane];
+#pragma unroll
+          for (int v = 0; v < V; ++v) {
+            const int4 raw = s_row[warp][src_lane][v];
+            const uint32_t q[4] = {(uint32_t)raw.x, (uint32_t)raw.y, (uint32_t)raw.z, (uint32_t)raw.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float2 f = unpack_bf16x2(q[e]);
+              acc[8 * v + 2 * e] += __fmul_rn(f.x, w);
+              acc[8 * v + 2 * e + 1] += __fmul_rn(f.y, w);
+            }
+          }
+        }
+        unsigned long long* dst = ugrad + (int64_t)gs * dim;
+#pragma unroll
+        for (int d = 0; d < dim; ++d) atomicAdd(dst + d, ugrad_fix(acc[d]));
+      }
+    }
+    __syncwarp();
+  }
+  sp_signal_last_block(sync, SP_CH_GRAD);
+}
+
+// -----------------------------------------------------------------------------------------------------------------
 // k_sp_linear_fwd (requester): out[b] = sum_c float(urow[inv[b][c]][0])  -- the linear (wide) logit of a sample, read in place from the
 // unique rows instead of gathering a [B, C, dim] activation.  One thread per sample adds its columns in order in fp32, so the result is
 // the sequential float sum whatever the launch geometry.  Padding (inv < 0) adds nothing.  Waits in-kernel for every owner's ROWS flag.
@@ -625,6 +736,39 @@ int dr_sp_gather(const void* urow, const int32_t* inv, const DrSpGeom* g, void* 
     default: return -3;
   }
 #undef SPGA
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// out: bf16 [B][F][dim] pooled bags, w_out: fp32 [F][B] the factor each bag was scaled by; waits for every owner's ROWS flag
+int dr_sp_pool(const void* urow, const int32_t* inv, const DrSpGeom* g, const DrSpBags* bags, void* out, float* w_out, const DrSpSync* sync,
+               cudaStream_t s) {
+  if (bags->F <= 0 || bags->F > g->C || g->ldinv < g->C) return -2;
+  const int lpr = g->dim / 4;
+  const int64_t n = g->B * bags->F;
+  const int grid = sp_grid((n * lpr + 255) / 256);
+#define SPP(L) DR_PDL_LAUNCH((k_sp_pool<L>), grid, 256, 0, s, (const __nv_bfloat16*)urow, inv, g->ldinv, g->B, *bags, (__nv_bfloat16*)out, w_out, *sync)
+  switch (g->dim % 4 ? 0 : lpr) {
+    case 2: SPP(2); break; case 4: SPP(4); break; case 8: SPP(8); break; case 16: SPP(16); break; case 32: SPP(32); break;
+    default: return -3;
+  }
+#undef SPP
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// dpool: bf16 [F][B][dim] gradient of the pooled bags, w: fp32 [F][B] as dr_sp_pool stored it; accumulates into ugrad and raises the GRAD flags
+int dr_sp_pool_segsum(const void* dpool, const float* w, const int32_t* invT, const DrSpGeom* g, const DrSpBags* bags, void* ugrad,
+                      const DrSpSync* sync, cudaStream_t s) {
+  if (bags->F <= 0 || bags->F > g->C) return -2;
+  const int64_t units = ((g->B + 31) / 32) * g->C;
+  const int grid = sp_grid((units + 7) / 8);
+#define SPPS(L) DR_PDL_LAUNCH((k_sp_pool_segsum<L>), grid, 256, 0, s, (const __nv_bfloat16*)dpool, w, invT, *g, *bags, (unsigned long long*)ugrad, *sync)
+  switch (g->dim % 4 ? 0 : g->dim / 4) {
+    case 2: SPPS(2); break; case 4: SPPS(4); break; case 8: SPPS(8); break; case 16: SPPS(16); break;
+    default: return -3;
+  }
+#undef SPPS
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -15,7 +15,7 @@ from .. import _native
 from .._native import EvConfig, ptr
 from ..ops.device_table import DeviceTable, _chk, _next_pow2, get_context
 from ..optim.optimizers import OPT_ADAGRAD_DECAY, OPT_SLOTS, engine_hyper, slot0_init
-from ..parallel.sparse_pipeline import CH_DENSE, SparsePipeline
+from ..parallel.sparse_pipeline import CH_DENSE, Bags, SparsePipeline
 
 
 def stream(dev: torch.device):
@@ -30,10 +30,12 @@ class EmbeddingGroup:
     def __init__(self, dev: torch.device, dim: int, kind: int, learning_rate: float, initial_accumulator_value: float, owner: int, seed: int,
                  tables: Sequence[int], table_rows: Sequence[int], batch_size: int, col_table: Optional[Sequence[int]] = None, rank: int = 0,
                  world: int = 1, comm=None, pad_key: int = -1, filter_freq: int = 0, steps_to_live: int = 0, max_rows_per_table: int = 1 << 25,
-                 tiered: Optional[Dict[int, dict]] = None, is_linear: bool = False):
+                 tiered: Optional[Dict[int, dict]] = None, is_linear: bool = False, bags: Optional[Sequence[tuple]] = None):
         """tables: the tables this rank holds; table_rows[t]: expected distinct keys of table t (pre-sizing hint, tables grow).  col_table[c]:
         table of id column c -- unique-first: a pipeline over the id columns, the hash(key) % world shard of every table; None: table-wise
-        placement, whole tables, no pipeline.  owner: key of the step context (one per group).  tiered: as FusedRecEngine's."""
+        placement, whole tables, no pipeline.  owner: key of the step context (one per group).  tiered: as FusedRecEngine's.
+        bags: ``(n_cols, combiner)`` multi-hot bags over the id columns (``parallel.sparse_pipeline.Bags``): the group's activation is pooled
+        per bag (``pool``) and its backward takes the pooled gradient [F, B, dim] (``pool_segsum``)."""
         self.dev, self.dim, self.is_linear, self.world, self.comm = dev, dim, is_linear, world, comm
         self.lib = _native.cuda()
         self._launches = 0
@@ -59,6 +61,12 @@ class EmbeddingGroup:
         else:
             self.sp = None
             self.max_unique = max(1, len(tables) * world * batch_size)
+        self.bags = self.pool_w = None
+        if bags is not None:
+            if is_linear or self.sp is None:
+                raise ValueError("bags need a deep group over a unique-first pipeline")
+            self.bags = Bags(dev, bags, self.sp.C)
+            self.pool_w = torch.zeros(self.bags.F, batch_size, dtype=torch.float32, device=dev)    # per-(bag, sample) factor of the pooling
         self.ctx.ensure(self.max_unique)
         self.ctx.claimed_upper = 0
         self.ctx.set_hyper(engine_hyper(kind, learning_rate, initial_accumulator_value))
@@ -111,10 +119,13 @@ class EmbeddingGroup:
         self.sp.lookup(self.ctx, self.tmap, train)
 
     def backward(self, grad: torch.Tensor, tick: Callable[[str], None] = _no_tick) -> None:
-        """grad: the per-sample gradient rows (bf16 [C, B, dim]), or for a linear group the gradient of every sample's linear logit (fp32 [B]).
-        Requester: pre-reduce it per distinct key.  Owner: pull the sources' per-key gradients, then the row-wise optimizer."""
+        """grad: the per-sample gradient rows (bf16 [C, B, dim]; with bags the pooled rows [F, B, dim]), or for a linear group the gradient of
+        every sample's linear logit (fp32 [B]).  Requester: pre-reduce it per distinct key.  Owner: pull the sources' per-key gradients, then the
+        row-wise optimizer."""
         if self.is_linear:
             self.sp.linear_bwd(grad)
+        elif self.bags is not None:
+            self.sp.pool_segsum(grad, self.pool_w, self.bags)
         else:
             self.sp.segsum(grad)
         tick("g_segsum")

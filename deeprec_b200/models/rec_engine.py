@@ -43,7 +43,7 @@ class FusedRecEngine:
                  initial_accumulator_value: float = 0.1, filter_freq: int = 0, steps_to_live: int = 0, pad_key: int = -1, seed: int = 1234,
                  max_rows_per_table: int = 1 << 25, device=None, rank: int = 0, world_size: int = 1, comm=None, loss_fn: Optional[Callable] = None,
                  tiered: Optional[Dict[int, dict]] = None, micro_batch_num: int = 1, linear: bool = False, linear_optimizer: Optional[str] = None,
-                 linear_learning_rate: Optional[float] = None):
+                 linear_learning_rate: Optional[float] = None, bags: Optional[Sequence[tuple]] = None, label_dim: int = 1):
         """net: dense module (its parameters are trained); forward_fn(net, dense: dict of static tensors, emb [B, C, D] bf16, ids [C, B]) -> logits [B].
         col_table[c]: table of id column c; table_rows[t]: expected distinct keys of table t (pre-sizing hint, tables grow).
         tiered: {table: {"cache_rows": R, "strategy": 0 (LFU) | 1 (LRU)}} -- those tables keep at most ~R rows PER RANK in HBM over a host DRAM tier
@@ -57,7 +57,15 @@ class FusedRecEngine:
         of which element 0 is the weight of an id.  Every step computes the per-sample sum of those weights in fp32 (``linear_fwd``, read in place from
         the unique rows) and hands it to ``forward_fn`` as the keyword ``linear=`` (fp32 [B], a leaf whose gradient trains the group); without the
         group forward_fn is called without it.  The group has its own optimizer: ``linear_optimizer`` / ``linear_learning_rate`` (None: the same as
-        the deep tables), e.g. FTRL at 0.2 as the reference trains Wide & Deep's linear part.  Linear tables are single-tier."""
+        the deep tables), e.g. FTRL at 0.2 as the reference trains Wide & Deep's linear part.  Linear tables are single-tier.
+        bags: multi-hot id bags, a list of ``(n_cols, combiner)`` over the id columns in order (the counts sum to C; combiner ``sum | mean |
+        sqrtn``, padding neither adds nor counts).  Bag f pools its columns into slot f of the activation, which is then [B, F, D]: forward_fn
+        receives that, and its gradient goes back to every column of the bag (``k_sp_pool`` / ``k_sp_pool_segsum``, in place of gather / segsum).
+        Not combined with ``linear``.
+        label_dim: labels are [B] (1) or [B, label_dim]; forward_fn may return a dict of logits, which ``loss_fn`` then receives and of which
+        ``predict()`` returns the sigmoids."""
+        if linear and bags is not None:
+            raise ValueError("FusedRecEngine: bags with linear=True (a wide part over pooled bags) is not supported")
         self.net, self.forward_fn = net, forward_fn
         self.rank, self.world, self.comm = rank, world_size, comm
         self.emu = _native.emu_active()              # CPU CI: the same step on the CUDA-on-CPU emulation of the kernels (eager, no CUDA graph)
@@ -76,19 +84,20 @@ class FusedRecEngine:
         # ---- embedding groups: this rank's hash(key) % world shard of every table, each group with its own step context (owner key),
         #      optimizer and pipeline
         owner = id(self) & 0x7FFFFFFF
-        group = lambda dim, kind, lr, owner, seed, tiered, is_linear: EmbeddingGroup(
+        group = lambda dim, kind, lr, owner, seed, tiered, is_linear, bags=None: EmbeddingGroup(
             dev, dim, kind, lr, initial_accumulator_value, owner, seed, range(self.T), table_rows, batch_size, col_table=col_table, rank=rank,
             world=world_size, comm=comm, pad_key=pad_key, filter_freq=filter_freq, steps_to_live=steps_to_live,
-            max_rows_per_table=max_rows_per_table, tiered=tiered, is_linear=is_linear)
-        self.deep = group(self.D, self.kind, learning_rate, owner, seed + 17, tiered, False)
+            max_rows_per_table=max_rows_per_table, tiered=tiered, is_linear=is_linear, bags=bags)
+        self.deep = group(self.D, self.kind, learning_rate, owner, seed + 17, tiered, False, bags)
         self.tables, self.tiers, self.sp, self.hp_dev = self.deep.tables, self.deep.tiers, self.deep.sp, self.deep.hp_dev
         self._host_step = 0
         # ---- static buffers
         self.ids = torch.full((self.C, batch_size), pad_key, dtype=torch.int64, device=dev)
-        self.labels = torch.zeros(batch_size, dtype=torch.float32, device=dev)
+        self.labels = torch.zeros((batch_size,) if label_dim == 1 else (batch_size, label_dim), dtype=torch.float32, device=dev)
         self.dense: Dict[str, torch.Tensor] = {k: torch.zeros(*shape, dtype=dt, device=dev) for k, (shape, dt) in (dense_inputs or {}).items()}
-        self.emb_out = torch.zeros(batch_size, self.C, self.D, dtype=torch.bfloat16, device=dev)
-        self.demb = torch.zeros(self.C, batch_size, self.D, dtype=torch.bfloat16, device=dev)
+        slots = self.C if self.deep.bags is None else self.deep.bags.F      # activation rows per sample: id columns, or pooled bags
+        self.emb_out = torch.zeros(batch_size, slots, self.D, dtype=torch.bfloat16, device=dev)
+        self.demb = torch.zeros(slots, batch_size, self.D, dtype=torch.bfloat16, device=dev)
         self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
         # ---- dense parameters / gradients -> one flat buffer each
         self.net.to(dev)
@@ -137,7 +146,10 @@ class FusedRecEngine:
     # ------------------------------------------------------------------------------------------------------------------
     def _sparse_forward(self, train: bool) -> None:
         self.deep.forward(self.ids, train)
-        self.sp.gather(self.emb_out)                  # waits for every owner's ROWS flag in-kernel
+        if self.deep.bags is not None:                # both wait for every owner's ROWS flag in-kernel
+            self.sp.pool(self.emb_out, self.deep.pool_w, self.deep.bags)
+        else:
+            self.sp.gather(self.emb_out)
         if self.linear:
             self.linear.forward(self.ids, train)
             self.linear.sp.linear_fwd(self.lin_out)   # waits for every owner's ROWS flag in-kernel
@@ -255,13 +267,14 @@ class FusedRecEngine:
             self.train_step_eager()
 
     @torch.no_grad()
-    def predict(self) -> torch.Tensor:
-        """Forward only (tables read-only; BatchNorm in eval mode)."""
+    def predict(self):
+        """Forward only (tables read-only; BatchNorm in eval mode): the sigmoid of the logits, a dict of them for a multi-output forward_fn."""
         was = self.net.training
         self.net.eval()
         self._sparse_forward(False)
         kw = {"linear": self.lin_out} if self.linear else {}
-        out = torch.sigmoid(self.forward_fn(self.net, self.dense, self.emb_out, self.ids, **kw).float())
+        logits = self.forward_fn(self.net, self.dense, self.emb_out, self.ids, **kw)
+        out = {k: torch.sigmoid(v.float()) for k, v in logits.items()} if isinstance(logits, dict) else torch.sigmoid(logits.float())
         for g in self.groups:
             g.forward_only_tail()
         self.net.train(was)
@@ -307,6 +320,46 @@ def din_engine(model, batch_size: int, max_len: int = 50, table_rows: Sequence[i
 def din_ids(batch: Dict[str, torch.Tensor]) -> torch.Tensor:
     """Taobao-shaped batch dict -> the [3 + 2 L, B] id-column block :func:`din_engine` expects (run it in the input pipeline)."""
     return torch.cat([batch["user"][None], batch["item"][None], batch["cat"][None], batch["hist_item"].t(), batch["hist_cat"].t()], 0).contiguous()
+
+
+POOLED_SEQ_MODELS = ("dssm", "esmm", "mmoe", "dbmtl", "ple", "simple_multitask")
+
+
+def pooled_seq_engine(model, batch_size: int, max_len: int = 50, combiner: str = "sum",
+                      table_rows: Sequence[int] = (10_000_000, 100_000_000, 10_000), **kw) -> FusedRecEngine:
+    """:class:`models.zoo.DSSM` and the multi-task models (ESMM, MMoE, DBMTL, PLE, SimpleMultiTask), which only consume the pooled behaviour
+    history: the id columns of :func:`din_ids` ([user | item | cat | hist_item x L | hist_cat x L]) pooled into five bags
+    [user | item | cat | hist_item | hist_cat] with ``combiner`` (``sum`` is what the framework path's ``_embed_pooled`` computes; the reference
+    pools these columns with ``mean``), so the dense net sees a [B, 5, D] activation.  Multi-task models train on labels [B, 2] (click, conversion:
+    :func:`taobao_engine_batch`) with the model's own ``multitask_loss``."""
+    from .zoo import DSSM, _MultiTask
+    L = max_len
+    col_table = [0, 1, 2] + [1] * L + [2] * L
+    bags = [(1, combiner), (1, combiner), (1, combiner), (L, combiner), (L, combiner)]
+    multitask = isinstance(model, _MultiTask)
+    if not multitask and not isinstance(model, DSSM):
+        raise ValueError(f"pooled_seq_engine: {type(model).__name__} is neither DSSM nor a multi-task model")
+    dense_net = _StripTables(model)
+
+    def fwd(net, dense, emb, ids):
+        u = emb[:, 0]
+        q = torch.cat([emb[:, 1], emb[:, 2]], -1)
+        pooled = torch.cat([emb[:, 3], emb[:, 4]], -1)
+        with torch.autocast(emb.device.type, dtype=torch.bfloat16):
+            if multitask:
+                return net.inner.tower_logits(torch.cat([u, q, pooled], -1))
+            return net.inner.head(u, q, pooled)
+    if multitask:
+        kw.setdefault("loss_fn", lambda out, y: dense_net.inner.multitask_loss({k: v.float() for k, v in out.items()}, y[:, 0], y[:, 1]))
+    return FusedRecEngine(dense_net, fwd, col_table, list(table_rows), batch_size, embedding_dim=model.emb_dim, bags=bags,
+                          label_dim=2 if multitask else 1, **kw)
+
+
+def taobao_engine_batch(batch: Dict[str, torch.Tensor]):
+    """Taobao-shaped batch dict -> ``(ids, labels [B, 2], None)`` for a multi-task :func:`pooled_seq_engine`: the click label and the conversion
+    label built as :meth:`models.zoo._MultiTask.loss` builds it."""
+    y = batch["labels"].float()
+    return din_ids(batch), torch.stack([y, y * (batch["item"] % 2 == 0).to(y.dtype)], 1), None
 
 
 class _StripTables(nn.Module):

@@ -51,7 +51,7 @@ def get_arg_parser():
                         "roles with `python -m deeprec_b200.parallel.ps_train`")
     p.add_argument("--timeline", type=int, default=0)
     p.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
-    p.add_argument("--engine", action="store_true", help="fused sm_90a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / DIN through FusedRecEngine (models/rec_engine.py)")
+    p.add_argument("--engine", action="store_true", help="fused sm_90a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / DIN, and DSSM / ESMM / MMoE / DBMTL / PLE / SimpleMultiTask over pooled history bags, through FusedRecEngine (models/rec_engine.py)")
     p.add_argument("--log_every", type=int, default=20)
     p.add_argument("--watchdog", type=float, default=0, help="seconds without a finished step before the job dumps stacks and exits 86")
     return p
@@ -85,9 +85,10 @@ def main(argv=None) -> int:
         # every other Criteo-style model (and DIN) through FusedRecEngine: the same unique-first sparse pipeline + one CUDA graph per step
         # under the model's own dense net (models/rec_engine.py; 1..8 GPUs when launched with torchrun / parallel.launch)
         from deeprec_b200.models import zoo
-        from deeprec_b200.models.rec_engine import criteo_engine, din_engine, din_ids
-        if name not in zoo.CRITEO_MODELS and name != "din":
-            raise SystemExit(f"--engine: no fused-engine adapter for {name} (dlrm, {', '.join(sorted(zoo.CRITEO_MODELS))}, din)")
+        from deeprec_b200.models.rec_engine import POOLED_SEQ_MODELS, criteo_engine, din_engine, din_ids, pooled_seq_engine, taobao_engine_batch
+        if name not in zoo.CRITEO_MODELS and name != "din" and name not in POOLED_SEQ_MODELS:
+            raise SystemExit(f"--engine: no fused-engine adapter for {name} "
+                             f"(dlrm, {', '.join(sorted(zoo.CRITEO_MODELS))}, din, {', '.join(POOLED_SEQ_MODELS)})")
         import torch.distributed as dist
         world, rank, lrank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0")), int(os.environ.get("LOCAL_RANK", "0"))
         torch.cuda.set_device(lrank)
@@ -109,6 +110,13 @@ def main(argv=None) -> int:
             def batch(s):
                 b = taobao_batch(a.batch_size, L, 100000, 200000, 1000, seed=s * world + rank)
                 return din_ids(b), b["labels"], None
+        elif name in POOLED_SEQ_MODELS:
+            L = 20
+            eng = pooled_seq_engine(model, a.batch_size, L, table_rows=(100000, 200000, 1000), **kw)
+
+            def batch(s):
+                b = taobao_batch(a.batch_size, L, 100000, 200000, 1000, seed=s * world + rank)
+                return taobao_engine_batch(b) if eng.labels.dim() == 2 else (din_ids(b), b["labels"], None)
         else:
             cards = [1000] * 26
             eng = criteo_engine(model, a.batch_size, table_rows=cards, **kw)

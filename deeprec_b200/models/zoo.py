@@ -392,11 +392,15 @@ class DSSM(_SeqBase):
         self.item_tower = mlp(dnn_hidden_units, D2, last_act=False, device=dev)
         self.scale = nn.Parameter(torch.tensor(5.0, device=dev))
 
-    def forward(self, b):
-        u, q, pooled = self._embed_pooled(b)
+    def head(self, u, q, pooled):
+        """Dense part on already-looked-up embeddings (user [B, D], target [B, 2D], pooled history [B, 2D]) -- what
+        :func:`models.rec_engine.pooled_seq_engine` runs on top of the unique-first sparse pipeline."""
         ue = self.user_tower(torch.cat([u, pooled], -1))
         ie = self.item_tower(q)
         return F.cosine_similarity(ue, ie, dim=-1) * self.scale
+
+    def forward(self, b):
+        return self.head(*self._embed_pooled(b))
 
 
 class _MultiTask(_SeqBase):
@@ -410,11 +414,24 @@ class _MultiTask(_SeqBase):
     def feat_dim(self):
         return self.emb_dim + 4 * self.emb_dim
 
+    def tower_logits(self, f):
+        """Dense part on the feature vector [user | target | pooled history] ([B, 5D]): a dict of per-task logits -- what
+        :func:`models.rec_engine.pooled_seq_engine` runs on top of the unique-first sparse pipeline."""
+        raise NotImplementedError
+
+    def forward(self, b):
+        return self.tower_logits(self._features(b))
+
+    @staticmethod
+    def multitask_loss(out, y, y2):
+        """Click loss on ``ctr`` plus conversion loss on ``ctcvr`` (ESMM) or ``cvr``."""
+        return F.binary_cross_entropy_with_logits(out["ctr"], y) + F.binary_cross_entropy_with_logits(out.get("ctcvr", out["cvr"]), y2)
+
     def loss(self, b):
         out = self.forward(b)
         y = b["labels"].to(next(iter(out.values())).device)
         y2 = y * (b["item"].to(y.device) % 2 == 0).to(y.dtype)          # synthetic conversion label nested in clicks
-        return F.binary_cross_entropy_with_logits(out["ctr"], y) + F.binary_cross_entropy_with_logits(out.get("ctcvr", out["cvr"]), y2)
+        return self.multitask_loss(out, y, y2)
 
 
 class ESMM(_MultiTask):
@@ -426,8 +443,7 @@ class ESMM(_MultiTask):
         self.ctr = nn.Sequential(mlp(ctr_mlp, self.feat_dim, device=dev), nn.Linear(ctr_mlp[-1], 1, device=dev))
         self.cvr = nn.Sequential(mlp(cvr_mlp, self.feat_dim, device=dev), nn.Linear(cvr_mlp[-1], 1, device=dev))
 
-    def forward(self, b):
-        f = self._features(b)
+    def tower_logits(self, f):
         ctr, cvr = self.ctr(f).squeeze(-1), self.cvr(f).squeeze(-1)
         p = (torch.sigmoid(ctr) * torch.sigmoid(cvr)).clamp(1e-7, 1 - 1e-7)
         return {"ctr": ctr, "cvr": cvr, "ctcvr": torch.log(p) - torch.log1p(-p)}
@@ -441,8 +457,7 @@ class MMoE(_MultiTask):
         self.gates = nn.ModuleDict({t: nn.Linear(self.feat_dim, num_experts, device=dev) for t in self.tasks})
         self.towers = nn.ModuleDict({t: nn.Sequential(mlp(tower, expert_hidden_units[-1], device=dev), nn.Linear(tower[-1], 1, device=dev)) for t in self.tasks})
 
-    def forward(self, b):
-        f = self._features(b)
+    def tower_logits(self, f):
         e = torch.stack([x(f) for x in self.experts], 1)
         return {t: self.towers[t]((torch.softmax(self.gates[t](f), -1).unsqueeze(-1) * e).sum(1)).squeeze(-1) for t in self.tasks}
 
@@ -459,8 +474,8 @@ class DBMTL(_MultiTask):
         self.rel = mlp((32,), 2 * tower[-1], device=dev)
         self.o_ctr, self.o_cvr = nn.Linear(tower[-1], 1, device=dev), nn.Linear(32, 1, device=dev)
 
-    def forward(self, b):
-        s = self.bottom(self._features(b))
+    def tower_logits(self, f):
+        s = self.bottom(f)
         a, c = self.t_ctr(s), self.t_cvr(s)
         return {"ctr": self.o_ctr(a).squeeze(-1), "cvr": self.o_cvr(self.rel(torch.cat([a, c], -1))).squeeze(-1)}
 
@@ -483,8 +498,7 @@ class PLE(_MultiTask):
             d = expert_units[-1]
         self.towers = nn.ModuleDict({t: nn.Sequential(mlp(tower, d, device=dev), nn.Linear(tower[-1], 1, device=dev)) for t in self.tasks})
 
-    def forward(self, b):
-        f = self._features(b)
+    def tower_logits(self, f):
         xs = {t: f for t in self.tasks}
         xs["shared"] = f
         for L in self.layers:
@@ -508,8 +522,7 @@ class SimpleMultiTask(_MultiTask):
         dev = self.device
         self.towers = nn.ModuleDict({t: nn.Sequential(mlp(hidden, self.feat_dim, device=dev), nn.Linear(hidden[-1], 1, device=dev)) for t in self.tasks})
 
-    def forward(self, b):
-        f = self._features(b)
+    def tower_logits(self, f):
         return {t: self.towers[t](f).squeeze(-1) for t in self.tasks}
 
 

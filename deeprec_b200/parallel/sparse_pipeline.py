@@ -41,6 +41,44 @@ class SpGeom(C.Structure):
                 ("dim", i32), ("ldinv", i32), ("pad_key", i64)]
 
 
+class SpBags(C.Structure):
+    """Mirror of DrSpBags."""
+    _fields_ = [("off", vp), ("comb", vp), ("col_bag", vp), ("F", i32)]
+
+
+COMBINERS = {"sum": 0, "mean": 1, "sqrtn": 2}
+
+
+class Bags:
+    """Multi-hot bags over the id columns: ``bags`` lists ``(n_cols, combiner)`` in column order, bag f pools the next ``n_cols`` columns into
+    activation slot f with ``sum | mean | sqrtn`` (padding neither adds nor counts).  The geometry lives in device tensors, built once."""
+
+    def __init__(self, dev: torch.device, bags: Sequence[tuple], num_cols: int):
+        bags = [(int(n), str(c)) for n, c in bags]
+        if not bags:
+            raise ValueError("bags: at least one bag")
+        for n, c in bags:
+            if n < 1:
+                raise ValueError(f"bags: a bag needs at least one id column, got {n}")
+            if c not in COMBINERS:
+                raise ValueError(f"bags: combiner must be one of {'|'.join(COMBINERS)}, got {c!r}")
+        if sum(n for n, _ in bags) != num_cols:
+            raise ValueError(f"bags: the column counts sum to {sum(n for n, _ in bags)}, the engine has {num_cols} id columns")
+        off = [0]
+        for n, _ in bags:
+            off.append(off[-1] + n)
+        self.F, self.spec = len(bags), bags
+        self.off = torch.tensor(off, dtype=torch.int32, device=dev)
+        self.comb = torch.tensor([COMBINERS[c] for _, c in bags], dtype=torch.int32, device=dev)
+        self.col_bag = torch.tensor([f for f, (n, _) in enumerate(bags) for _ in range(n)], dtype=torch.int32, device=dev)
+        s = SpBags()
+        s.off, s.comb, s.col_bag, s.F = self.off.data_ptr(), self.comb.data_ptr(), self.col_bag.data_ptr(), self.F
+        self.struct = s
+
+    def ref(self):
+        return C.byref(self.struct)
+
+
 def _next_pow2(n: int) -> int:
     p = 1
     while p < n:
@@ -57,12 +95,14 @@ def bind(lib):
     if getattr(lib, "_sp_bound", False):
         return lib
     INT, P = C.c_int, vp
-    GP, SP, PP = C.POINTER(SpGeom), C.POINTER(SpSync), C.POINTER(Peers)
+    GP, SP, PP, BP = C.POINTER(SpGeom), C.POINTER(SpSync), C.POINTER(Peers), C.POINTER(SpBags)
     sigs = {
         "dr_sp_init_scratch": [P, i64, P],
         "dr_sp_dedup": [P, GP, P, P, P, P, P, P, P, SP, P],
         "dr_sp_segsum": [P, P, GP, P, SP, P],
         "dr_sp_gather": [P, P, GP, P, SP, P],
+        "dr_sp_pool": [P, P, GP, BP, P, P, SP, P],
+        "dr_sp_pool_segsum": [P, P, P, GP, BP, P, SP, P],
         "dr_sp_linear_fwd": [P, P, GP, P, SP, P],
         "dr_sp_linear_bwd": [P, P, GP, P, SP, P],
         "dr_sp_lookup": [P, P, GP, i64, PP, PP, PP, PP, PP, INT, P, P, P, P, P, i64, SP, P],
@@ -214,6 +254,25 @@ class SparsePipeline:
         """Requester side: pre-reduce the per-sample gradient rows (bf16 [C, B, dim]) per distinct key into ugrad; raises GRAD."""
         assert demb.shape == (self.C, self.B, self.dim) and demb.dtype == torch.bfloat16
         _chk(self.lib.dr_sp_segsum(ptr(demb), ptr(self.invT), self.geom_ref(), ptr(self.ugrad), self.sync_ref(), self._s()), "segsum")
+        self.launches += 1
+
+    def pool(self, out: torch.Tensor, w: torch.Tensor, bags: Bags) -> None:
+        """Requester side: out[b, f, :] = w[f, b] * sum of the live rows urow[inv[b, c]] of bag f (bf16 [B, F, dim], fp32 sum in column order);
+        w (fp32 [F, B]) = 1, 1/n or 1/sqrt(n) over the bag's n live ids, 0 for an empty bag.  Takes the place of gather; waits for ROWS."""
+        assert out.shape == (self.B, bags.F, self.dim) and out.dtype == torch.bfloat16 and out.is_contiguous()
+        assert w.shape == (bags.F, self.B) and w.dtype == torch.float32 and w.is_contiguous()
+        assert bags.col_bag.numel() == self.C
+        _chk(self.lib.dr_sp_pool(ptr(self.urow), ptr(self.inv), self.geom_ref(), bags.ref(), ptr(out), ptr(w), self.sync_ref(), self._s()), "pool")
+        self.launches += 1
+
+    def pool_segsum(self, dpool: torch.Tensor, w: torch.Tensor, bags: Bags) -> None:
+        """Requester side: segsum of the pooled bags' gradient (bf16 [F, B, dim]): every live column c of sample b adds dpool[bag(c), b] *
+        w[bag(c), b] to the per-key sums in ugrad; raises GRAD.  Takes the place of segsum."""
+        assert dpool.shape == (bags.F, self.B, self.dim) and dpool.dtype == torch.bfloat16 and dpool.is_contiguous()
+        assert w.shape == (bags.F, self.B) and w.dtype == torch.float32 and w.is_contiguous()
+        assert bags.col_bag.numel() == self.C and self.ugrad is not None
+        _chk(self.lib.dr_sp_pool_segsum(ptr(dpool), ptr(w), ptr(self.invT), self.geom_ref(), bags.ref(), ptr(self.ugrad), self.sync_ref(), self._s()),
+             "pool_segsum")
         self.launches += 1
 
     def linear_fwd(self, out: torch.Tensor) -> None:
