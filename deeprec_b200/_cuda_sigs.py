@@ -93,6 +93,8 @@ def _bind(lib):
     _sig(lib, "dr_cuda_dot_interaction_bwd", [P, i64, P, i64, P, i64, i64, INT, INT, i64, P, i64, P, i64, i64, S])
     _sig(lib, "dr_cuda_fm_fwd", [P, i64, i64, INT, INT, i64, P, i64, P, S])
     _sig(lib, "dr_cuda_fm_bwd", [P, i64, P, i64, i64, P, INT, INT, i64, P, i64, i64, INT, S])
+    _sig(lib, "dr_cuda_gru_fwd", [P, P, P, P, INT, INT, INT, P, S])
+    _sig(lib, "dr_cuda_gru_bwd", [P, P, P, P, P, P, INT, INT, INT, P, P, P, P, P, S])
     # comm (optional symbols: present once comm_kernels.cu is built)
     for name, args in _COMM_SIGS.items():
         if hasattr(lib, name):

@@ -39,6 +39,7 @@ CUDA_SOURCES = [
     "cuda/fused_ops.cu",
     "cuda/allocator.cu",
     "cuda/attention_kernels.cu",
+    "cuda/rnn_kernels.cu",              # tensor-core GRU recurrence (mma.sync): hardware only, not in EMU_SOURCES
 ]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

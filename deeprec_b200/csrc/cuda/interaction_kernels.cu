@@ -7,6 +7,7 @@
 // against 1.6 kB of traffic -- so it is HBM-bound by two orders of magnitude; it reads the embedding rows
 // exactly once, straight from the (peer-written) feature-major receive buffer, and emits the padded bf16
 // activation the wgmma top-MLP GEMM consumes through TMA.
+#include "mma_sync.cuh"
 #include "sp_sync.cuh"
 
 using namespace drc;
@@ -189,13 +190,8 @@ __global__ void __launch_bounds__(256) k_fm_bwd(const __nv_bfloat16* __restrict_
 //              the strict lower-triangle elements of its accumulator fragments into the sample's Z row.
 //   backward:  dF = S F [32 x 16 x 32] with S the symmetric 32 x 32 gradient matrix of the sample (eight mma.sync.m16n8k16);
 //              lane i then owns dF_i.
-// The SIMT kernels above remain as the general-shape fallback.
+// The SIMT kernels above remain as the general-shape fallback.  mma_bf16_16816: mma_sync.cuh.
 // =================================================================================================
-__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 // INDIRECT: `emb` is the requester-side unique-row buffer urow[gs][16] (written by the owners over NVLink) and feature t of sample b
 // is row inv[b][t] of it (-1 = padding -> zeros); the kernel first waits for every owner's ROWS flag (sp_sync.cuh).

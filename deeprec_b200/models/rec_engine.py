@@ -301,11 +301,16 @@ def criteo_engine(model, batch_size: int, table_rows: Optional[Sequence[int]] = 
 
 
 def din_engine(model, batch_size: int, max_len: int = 50, table_rows: Sequence[int] = (10_000_000, 100_000_000, 10_000), **kw) -> FusedRecEngine:
-    """:class:`models.zoo.DIN`: id columns = [user | item | cat | hist_item x L | hist_cat x L] over the three tables (user, item, cat);
-    the history positions are columns of the item / category tables, padding (-1) gives zero rows and the attention mask."""
+    """:class:`models.zoo.DIN` and :class:`models.zoo.DIEN`: id columns = [user | item | cat | hist_item x L | hist_cat x L] over the three
+    tables (user, item, cat); the history positions are columns of the item / category tables, padding (-1) gives zero rows and the attention
+    mask.  DIEN's two GRUs run on :func:`nn.fused_gru`, which stops each sample after ``mask.sum(1)`` steps: its padding must be a tail (every
+    id after the first -1 of a history is -1 too), as :func:`din_ids` of the project's Taobao-shaped batches gives."""
+    from ..nn import fused_gru
+    from .zoo import DIEN
     L = max_len
     col_table = [0, 1, 2] + [1] * L + [2] * L
     dense_net = _StripTables(model)
+    kw_head = {"gru": fused_gru} if isinstance(model, DIEN) else {}
 
     def fwd(net, dense, emb, ids):
         u = emb[:, 0]
@@ -313,7 +318,7 @@ def din_engine(model, batch_size: int, max_len: int = 50, table_rows: Sequence[i
         k = torch.cat([emb[:, 3:3 + L], emb[:, 3 + L:3 + 2 * L]], -1)             # [B, L, 2D] bf16 (padding rows are already zero)
         mask = (ids[3:3 + L] >= 0).t()
         with torch.autocast(emb.device.type, dtype=torch.bfloat16):
-            return net.inner.head(u, q, k, mask)
+            return net.inner.head(u, q, k, mask, **kw_head)
     return FusedRecEngine(dense_net, fwd, col_table, list(table_rows), batch_size, embedding_dim=model.emb_dim, **kw)
 
 

@@ -348,16 +348,25 @@ class DIEN(_SeqBase):
         self.top = nn.Sequential(nn.Linear(self.emb_dim + D2 + hidden + D2, 200, device=dev), nn.PReLU(device=dev), nn.Linear(200, 80, device=dev), nn.PReLU(device=dev),
                                  nn.Linear(80, 1, device=dev))
 
-    def forward(self, b):
-        u, q, k, mask = self._embed(b)
-        h1, _ = self.gru1(k)
+    def head(self, u, q, k, mask, gru=None):
+        """Dense part on already-looked-up embeddings (user [B, D], target [B, 2D], history [B, L, 2D] zero-padded at the tail, mask [B, L]).
+        ``gru=None`` runs both layers through ``nn.GRU``; otherwise ``gru(x, module, lengths)`` (:func:`nn.fused_gru`, what
+        :func:`models.rec_engine.din_engine` passes) runs each layer only over the first ``lengths = max(mask.sum(1), 1)`` steps of a sample."""
+        lens = mask.sum(1).clamp_min(1)
+        run = (lambda x, m: m(x)[0]) if gru is None else (lambda x, m: gru(x, m, lens))
+        # Both paths give the same logits.  A GRU is causal, so h1 and h2 agree on the first lens steps, the only steps the masked softmax
+        # weighs and ``final`` reads.  An empty history (mask all False) counts as length 1: the all-masked softmax gives every position
+        # 1 / L, and final = h2[0] depends on step 0 alone, which the length-1 run computes too.
+        h1 = run(k, self.gru1)
         qh = self.qproj(q).unsqueeze(1).expand_as(h1)
         s = self.att(torch.cat([qh, h1, qh - h1, qh * h1], -1)).squeeze(-1).masked_fill(~mask, -2 ** 31)
         w = torch.softmax(s, -1).unsqueeze(-1)
-        h2, _ = self.gru2(h1 * w)
-        lens = mask.sum(1).clamp_min(1) - 1
-        final = h2[torch.arange(h2.shape[0], device=h2.device), lens]
+        h2 = run(h1 * w, self.gru2)
+        final = h2[torch.arange(h2.shape[0], device=h2.device), lens - 1]
         return self.top(torch.cat([u, q, final, k.sum(1)], -1)).squeeze(-1)
+
+    def forward(self, b):
+        return self.head(*self._embed(b))
 
 
 class BST(_SeqBase):

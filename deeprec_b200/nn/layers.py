@@ -7,6 +7,8 @@
     are re-packed every forward by one small kernel per layer.
   * ``dot_interaction`` (DLRM) and ``fm_interaction`` (DeepFM second order) autograd functions on
     csrc/cuda/interaction_kernels.cu.
+  * ``fused_gru``: a single-layer GRU over tail-padded sequences for training -- the input projection on the wgmma GEMM, the recurrence
+    forward and backward through time on csrc/cuda/rnn_kernels.cu.
 
 The reference runs these through cuBLAS (stream_executor/cuda/cuda_blas.cc) and ~10 TF ops per interaction
 (modelzoo/dlrm/train.py:163-236, modelzoo/deepfm/train.py:178-187).  CPU tensors fall back to the equivalent torch expression.
@@ -264,3 +266,56 @@ def fm_interaction(emb: torch.Tensor) -> torch.Tensor:
     if emb.is_cuda and emb.shape[2] in (8, 16, 32, 64):
         return _FMInteraction.apply(emb)
     return 0.5 * (emb.sum(1) ** 2 - (emb ** 2).sum(1))
+
+
+# ---- GRU ---------------------------------------------------------------------------------------------------------------------
+GRU_HIDDEN = (16, 32, 48, 64)         # hidden sizes csrc/cuda/rnn_kernels.cu is compiled for
+
+
+class _GRURecurrenceFn(torch.autograd.Function):
+    """gi [B L, 3H] bf16 (x W_ih^T + b_ih) -> y [B, L, H] fp32: the recurrence of a GRU with W_hh, b_hh, sample b running lengths[b] steps."""
+
+    @staticmethod
+    def forward(ctx, gi, w_hh, b_hh, lengths, B: int, L: int):
+        H = w_hh.shape[1]
+        w, b = w_hh.detach().float().contiguous(), b_hh.detach().float().contiguous()
+        y = torch.empty(B, L, H, dtype=torch.float32, device=gi.device)
+        _chk(_native.cuda().dr_cuda_gru_fwd(ptr(gi), ptr(w), ptr(b), ptr(lengths), B, L, H, ptr(y), stream_ptr()), "gru_fwd")
+        ctx.save_for_backward(gi, w, b, lengths, y)
+        ctx.shape = (B, L, H)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        gi, w, b, lengths, y = ctx.saved_tensors
+        B, L, H = ctx.shape
+        dev = gi.device
+        dgi = torch.empty(B * L, 3 * H, dtype=torch.bfloat16, device=dev)
+        dgh = torch.empty(B * L, 3 * H, dtype=torch.bfloat16, device=dev)
+        hprev = torch.empty(B * L, H, dtype=torch.bfloat16, device=dev)
+        dw = torch.zeros(3 * H, H, dtype=torch.float32, device=dev)
+        db = torch.zeros(3 * H, dtype=torch.float32, device=dev)
+        dy = dy.float().contiguous()
+        _chk(_native.cuda().dr_cuda_gru_bwd(ptr(gi), ptr(w), ptr(b), ptr(lengths), ptr(y), ptr(dy), B, L, H, ptr(dgi), ptr(dgh), ptr(hprev),
+                                            ptr(dw), ptr(db), stream_ptr()), "gru_bwd")
+        return dgi, dw, db, None, None, None
+
+
+def fused_gru(x: torch.Tensor, gru: nn.GRU, lengths: torch.Tensor) -> torch.Tensor:
+    """Single-layer, batch-first, unidirectional ``gru`` over ``x`` [B, L, I] whose sample b is ``lengths[b]`` (0..L) steps long, the rest
+    being tail padding: y [B, L, H] is h_t for t < lengths[b] and 0 past it (``tf.nn.dynamic_rnn(..., sequence_length=)``), h_0 = 0.
+    Trains the module's own parameters, so checkpoints keep its tensor names.  CUDA: the input projection on the wgmma GEMM (bf16), the
+    recurrence forward and backward on mma.sync kernels (bf16 operands, fp32 state), fp32 weight gradients; H must be one of
+    ``GRU_HIDDEN``.  CPU: the module itself, its outputs past the length zeroed."""
+    if gru.num_layers != 1 or not gru.batch_first or gru.bidirectional or not gru.bias or getattr(gru, "proj_size", 0):
+        raise ValueError("fused_gru: needs a single-layer, batch-first, unidirectional nn.GRU with biases")
+    B, L, I = x.shape
+    H = gru.hidden_size
+    if not x.is_cuda:
+        y, _ = gru(x.to(gru.weight_ih_l0.dtype))
+        valid = torch.arange(L, device=x.device)[None] < lengths.to(x.device)[:, None]
+        return y * valid.unsqueeze(-1).to(y.dtype)
+    if H not in GRU_HIDDEN:
+        raise ValueError(f"fused_gru: hidden size {H} is not supported on CUDA (one of {GRU_HIDDEN})")
+    gi = _FusedMLPFn.apply(x.reshape(B * L, I).to(torch.bfloat16), False, gru.weight_ih_l0, gru.bias_ih_l0)
+    return _GRURecurrenceFn.apply(gi.contiguous(), gru.weight_hh_l0, gru.bias_hh_l0, lengths.to(device=x.device, dtype=torch.int32).contiguous(), B, L)
