@@ -163,7 +163,8 @@ class cuda_emulation:
         global _EMU, _EMU_DEPTH
         with _LOCK:
             if _EMU is None or getattr(_EMU, "_sanitize", None) != self.sanitize:
-                lib = C.CDLL(_build.build_cuda_emu(self.sanitize))
+                from . import _cuda_sigs
+                lib = _cuda_sigs.bind(C.CDLL(_build.build_cuda_emu(self.sanitize)), skip_missing=True)
                 lib._sanitize = self.sanitize
                 _EMU = lib
             _EMU_DEPTH += 1
@@ -189,10 +190,6 @@ def cuda():
     """The sm_90a kernel library.  Raises if it is missing (never falls back silently)."""
     global _CUDA
     if _EMU_DEPTH > 0:
-        if not getattr(_EMU, "_sigs_bound", False):
-            from . import _cuda_sigs
-            _cuda_sigs.bind(_EMU, missing_ok=True)          # entry points of the wgmma / NVLS translation units do not exist in the emulation
-            _EMU._sigs_bound = True
         return _EMU
     if _CUDA is None:
         with _LOCK:
@@ -202,8 +199,6 @@ def cuda():
                     path = _build.build_cuda()
                 from . import _cuda_sigs
                 lib = _cuda_sigs.bind(C.CDLL(path))
-                lib.dr_cuda_set_device.argtypes, lib.dr_cuda_set_device.restype = [C.c_int], C.c_int
-                lib.dr_cuda_set_sparse_blocks_per_sm.argtypes, lib.dr_cuda_set_sparse_blocks_per_sm.restype = [C.c_int], C.c_int
                 if torch.cuda.is_available():
                     lib.dr_cuda_set_device(torch.cuda.current_device())
                 _CUDA = lib
@@ -228,9 +223,13 @@ def set_device(index: int) -> None:
     """The kernel library links its own static cudart: its current device must follow torch's."""
     if _EMU_DEPTH > 0:
         return
-    rc = cuda().dr_cuda_set_device(int(index))
+    check(cuda().dr_cuda_set_device(int(index)), f"set_device({index})")
+
+
+def check(rc: int, what: str) -> None:
+    """Raise if a kernel-library call returned an error code."""
     if rc != 0:
-        raise RuntimeError(f"dr_cuda_set_device({index}) failed: {rc}")
+        raise RuntimeError(f"deeprec_cuda: {what} failed with code {rc}")
 
 
 def ptr(t: torch.Tensor | None):
@@ -241,7 +240,9 @@ def ptr(t: torch.Tensor | None):
     return C.c_void_p(t.data_ptr())
 
 
-def stream_ptr():
+def stream_ptr(device=None):
+    """The stream argument of a kernel call: the current stream of ``device`` (default: the current device), or None while the kernel
+    emulation is active (emulated launches are synchronous)."""
     if _EMU_DEPTH > 0:
         return None
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)

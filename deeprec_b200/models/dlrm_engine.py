@@ -32,12 +32,12 @@ from typing import Dict, List, Optional, Sequence
 import torch
 
 from .. import _native
-from .._native import OptHyper, ptr
+from .._native import OptHyper, check, ptr, stream_ptr
 from ..checkpoint.engine_ckpt import restore_engine, save_engine
-from ..ops.device_table import DeviceTable, _chk
+from ..ops.device_table import DeviceTable
 from ..optim.optimizers import OPT_KIND, OPT_SLOTS, slot0_init
 from . import embedding_group as _eg
-from .embedding_group import EmbeddingGroup, stream
+from .embedding_group import EmbeddingGroup
 
 # Criteo-Terabyte cardinalities (MLPerf DLRM preprocessing, 40M cap) -- used only to shape the
 # synthetic id distributions and pre-size the tables; EmbeddingVariables are hash tables and grow.
@@ -268,7 +268,7 @@ class DLRMEngine:
         return out
 
     def _call(self, fn, *args):
-        _chk(fn(*args, stream(self.dev)), fn.__name__)
+        check(fn(*args, stream_ptr(self.dev)), fn.__name__)
         self._launches += 1
 
     def _gemm(self, A, lda, Bm, ldb, M, N, K, bias, relu, mask, ldm, out, ldc, aux_mode=None, S1=None, S2=None):

@@ -5,22 +5,16 @@ optimizer, i.e. this rank's shard of every table, their step context, device-res
 Also here: the helpers both engines share."""
 from __future__ import annotations
 
-import ctypes as C
 import math
 from typing import Callable, Dict, Optional, Sequence
 
 import torch
 
 from .. import _native
-from .._native import EvConfig, ptr
-from ..ops.device_table import DeviceTable, _chk, _next_pow2, get_context
+from .._native import EvConfig, check, ptr, stream_ptr
+from ..ops.device_table import DeviceTable, _next_pow2, get_context
 from ..optim.optimizers import OPT_ADAGRAD_DECAY, OPT_SLOTS, engine_hyper, slot0_init
 from ..parallel.sparse_pipeline import CH_DENSE, Bags, SparsePipeline
-
-
-def stream(dev: torch.device):
-    """The stream argument of a kernel call: the current stream of ``dev`` (None on the CUDA-on-CPU emulation, whose launches are synchronous)."""
-    return None if _native.emu_active() else C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 _no_tick = lambda name: None          # noqa: E731  (phase markers: DLRMEngine._tick)
@@ -138,13 +132,13 @@ class EmbeddingGroup:
     def apply(self) -> None:
         """Row-wise optimizer over this step's distinct keys (k_apply), then the distinct-key counter restarts (k_reset_counter)."""
         c = self.ctx
-        _chk(self.lib.dr_cuda_sparse_apply(ptr(c.structs()), ptr(c.ulist), ptr(c.nuniq), c.ulist.numel(), ptr(c.gsum), self.dim, ptr(self.hp_dev),
-                                           self.max_unique, 1, stream(self.dev)), "sparse_apply")
+        check(self.lib.dr_cuda_sparse_apply(ptr(c.structs()), ptr(c.ulist), ptr(c.nuniq), c.ulist.numel(), ptr(c.gsum), self.dim, ptr(self.hp_dev),
+                                            self.max_unique, 1, stream_ptr(self.dev)), "sparse_apply")
         self._launches += 2
 
     def end_step(self) -> None:
         """Global step / beta powers / decay of the hyper-parameters in device memory, then the pipeline's step boundary."""
-        _chk(self.lib.dr_cuda_advance_hyper(ptr(self.hp_dev), stream(self.dev)), "advance_hyper")
+        check(self.lib.dr_cuda_advance_hyper(ptr(self.hp_dev), stream_ptr(self.dev)), "advance_hyper")
         self._launches += 1
         if self.sp is not None:
             self.sp.step_end()

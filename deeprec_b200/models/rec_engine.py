@@ -29,12 +29,11 @@ import torch
 from torch import nn
 
 from .. import _native
-from .._native import ptr
+from .._native import check, ptr, stream_ptr
 from ..checkpoint.engine_ckpt import restore_engine, save_engine
-from ..ops.device_table import _chk
 from ..optim.optimizers import OPT_KIND, OPT_SLOTS, slot0_init
 from . import embedding_group as _eg
-from .embedding_group import EmbeddingGroup, stream
+from .embedding_group import EmbeddingGroup
 
 
 class FusedRecEngine:
@@ -210,9 +209,9 @@ class FusedRecEngine:
         if self.comm is not None:
             self.comm.dense_allreduce_update(self)
         else:
-            _chk(self.lib.dr_cuda_dense_apply(ptr(self.params), ptr(self.grads), ptr(self.s0) if self.s0 is not None else None,
-                                              ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, None, stream(self.dev)),
-                 "dense_apply")
+            check(self.lib.dr_cuda_dense_apply(ptr(self.params), ptr(self.grads), ptr(self.s0) if self.s0 is not None else None,
+                                               ptr(self.s1) if self.s1 is not None else None, self.P, ptr(self.hp_dev), 1.0, None, stream_ptr(self.dev)),
+                  "dense_apply")
             self._launches += 1
         for g in self.groups:
             g.end_step()

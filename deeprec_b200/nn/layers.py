@@ -22,16 +22,11 @@ from torch import nn
 from torch.nn import functional as F
 
 from .. import _native
-from .._native import ptr, stream_ptr
+from .._native import check, ptr, stream_ptr
 
 
 def _pad8(n: int) -> int:
     return (n + 7) // 8 * 8
-
-
-def _chk(rc: int, what: str) -> None:
-    if rc != 0:
-        raise RuntimeError(f"deeprec_cuda: {what} failed with code {rc}")
 
 
 _CONST = {}
@@ -51,7 +46,7 @@ def _to_bf16_padded(x: torch.Tensor, Kp: int) -> torch.Tensor:
     M, K = x.shape
     if x.dtype == torch.float32 and x.is_contiguous():
         y = torch.empty(M, Kp, dtype=torch.bfloat16, device=x.device)
-        _chk(_native.cuda().dr_cuda_cast_pad(ptr(x), M, K, ptr(y), Kp, stream_ptr()), "cast_pad")
+        check(_native.cuda().dr_cuda_cast_pad(ptr(x), M, K, ptr(y), Kp, stream_ptr()), "cast_pad")
         return y
     y = x.to(torch.bfloat16)
     if Kp != K:
@@ -84,14 +79,14 @@ class _FusedMLPFn(torch.autograd.Function):
             Wp = Wp.contiguous()
             wb = torch.empty(Np, Kp, dtype=torch.bfloat16, device=dev)
             wt = torch.empty(Kp, Np, dtype=torch.bfloat16, device=dev)
-            _chk(lib.dr_cuda_pack_weights(ptr(Wp), Np, Kp, ptr(wb), ptr(wt), Np, s), "pack_weights")
+            check(lib.dr_cuda_pack_weights(ptr(Wp), Np, Kp, ptr(wb), ptr(wt), Np, s), "pack_weights")
             bias = b.detach().float() if b is not None else None
             if bias is not None and Np != N:
                 bias = F.pad(bias, (0, Np - N))
             relu = int(i + 1 < nl or last_act)
             out = torch.empty(M, Np, dtype=torch.bfloat16, device=dev)
-            _chk(lib.dr_cuda_gemm_tn_ex(ptr(acts[-1]), Kp, ptr(wb), Kp, M, Np, Kp, ptr(bias) if bias is not None else None, relu, None, 0, 0,
-                                        ptr(out), Np, None, None, None, 0, 0, s), "gemm_tn")
+            check(lib.dr_cuda_gemm_tn_ex(ptr(acts[-1]), Kp, ptr(wb), Kp, M, Np, Kp, ptr(bias) if bias is not None else None, relu, None, 0, 0,
+                                         ptr(out), Np, None, None, None, 0, 0, s), "gemm_tn")
             acts.append(out); wts.append(wt); dims.append((N, K, Np, Kp, b is not None))
         ctx.save_for_backward(*acts, *wts)
         ctx.meta = (nl, last_act, dims, x.dtype, x.requires_grad, K0)
@@ -116,15 +111,15 @@ class _FusedMLPFn(torch.autograd.Function):
         if last_act:
             one, zero = _const_vec(dev, Np, 1.0), _const_vec(dev, Np, 0.0)
             da = torch.empty(M, Np, dtype=torch.bfloat16, device=dev)
-            _chk(lib.dr_cuda_bn_bwd_apply_v2(ptr(g), ptr(acts[-1]), M, Np, Np, ptr(one), ptr(zero), ptr(zero), ptr(zero), ptr(zero), ptr(da), 1, ptr(db), s),
-                 "relu_bwd")
+            check(lib.dr_cuda_bn_bwd_apply_v2(ptr(g), ptr(acts[-1]), M, Np, Np, ptr(one), ptr(zero), ptr(zero), ptr(zero), ptr(zero), ptr(da), 1, ptr(db), s),
+                  "relu_bwd")
         else:
             da = g
-            _chk(lib.dr_cuda_colstats(ptr(da), None, M, Np, Np, Np, ptr(db), None, s), "colstats")
+            check(lib.dr_cuda_colstats(ptr(da), None, M, Np, Np, Np, ptr(db), None, s), "colstats")
         for i in range(nl - 1, -1, -1):
             N, K, Np, Kp, has_bias = dims[i]
             dW = torch.zeros(Np, Kp, dtype=torch.float32, device=dev)
-            _chk(lib.dr_cuda_gemm_dw(ptr(da), Np, ptr(acts[i]), Kp, M, Np, Kp, ptr(dW), Kp, 0, s), "gemm_dw")
+            check(lib.dr_cuda_gemm_dw(ptr(da), Np, ptr(acts[i]), Kp, M, Np, Kp, ptr(dW), Kp, 0, s), "gemm_dw")
             grads[2 * i] = dW[:N, :K] if (Np, Kp) != (N, K) else dW
             if has_bias:
                 grads[2 * i + 1] = db[:N] if Np != N else db
@@ -135,12 +130,12 @@ class _FusedMLPFn(torch.autograd.Function):
                 # dX epilogue: * relu'(a_{i-1}); the bias gradient of layer i-1 (column sums) is fused for wide layers
                 db = torch.zeros(Kp, dtype=torch.float32, device=dev)
                 fused = Kp > 32
-                _chk(lib.dr_cuda_gemm_tn_ex(ptr(da), Np, ptr(wts[i]), Np, M, Kp, Np, None, 0, ptr(acts[i]), Kp, 1, ptr(prev), Kp, None,
-                                            ptr(db) if fused else None, None, 0, 0, s), "gemm_dx")
+                check(lib.dr_cuda_gemm_tn_ex(ptr(da), Np, ptr(wts[i]), Np, M, Kp, Np, None, 0, ptr(acts[i]), Kp, 1, ptr(prev), Kp, None,
+                                             ptr(db) if fused else None, None, 0, 0, s), "gemm_dx")
                 if not fused:
-                    _chk(lib.dr_cuda_colstats(ptr(prev), None, M, Kp, Kp, Kp, ptr(db), None, s), "colstats")
+                    check(lib.dr_cuda_colstats(ptr(prev), None, M, Kp, Kp, Kp, ptr(db), None, s), "colstats")
             else:
-                _chk(lib.dr_cuda_gemm_tn_ex(ptr(da), Np, ptr(wts[i]), Np, M, Kp, Np, None, 0, None, 0, 0, ptr(prev), Kp, None, None, None, 0, 0, s), "gemm_dx")
+                check(lib.dr_cuda_gemm_tn_ex(ptr(da), Np, ptr(wts[i]), Np, M, Kp, Np, None, 0, None, 0, 0, ptr(prev), Kp, None, None, None, 0, 0, s), "gemm_dx")
             da = prev
         dx = None
         if need_dx:
@@ -207,7 +202,7 @@ class _DotInteraction(torch.autograd.Function):
         nz = D + (T + 1) * T // 2
         Zp = _pad8(nz)
         Z = torch.zeros(B, Zp, dtype=torch.bfloat16, device=x.device)
-        _chk(lib.dr_cuda_dot_interaction_fwd(ptr(xb), D, ptr(eb), D, T * D, T, D, B, ptr(Z), Zp, stream_ptr()), "dot_interaction_fwd")
+        check(lib.dr_cuda_dot_interaction_fwd(ptr(xb), D, ptr(eb), D, T * D, T, D, B, ptr(Z), Zp, stream_ptr()), "dot_interaction_fwd")
         ctx.save_for_backward(xb, eb)
         ctx.meta = (nz, Zp, x.dtype, emb.dtype)
         return Z[:, :nz].to(x.dtype)
@@ -221,8 +216,8 @@ class _DotInteraction(torch.autograd.Function):
         g = _to_bf16_padded(gz.contiguous() if gz.dtype == torch.float32 else gz, Zp)
         dx = torch.empty(B, D, dtype=torch.bfloat16, device=gz.device)
         de = torch.empty(B, T, D, dtype=torch.bfloat16, device=gz.device)
-        _chk(lib.dr_cuda_dot_interaction_bwd(ptr(g), Zp, ptr(xb), D, ptr(eb), D, T * D, T, D, B, ptr(dx), D, ptr(de), D, T * D, stream_ptr()),
-             "dot_interaction_bwd")
+        check(lib.dr_cuda_dot_interaction_bwd(ptr(g), Zp, ptr(xb), D, ptr(eb), D, T * D, T, D, B, ptr(dx), D, ptr(de), D, T * D, stream_ptr()),
+              "dot_interaction_bwd")
         return dx.to(xdt), de.to(edt)
 
 
@@ -245,7 +240,7 @@ class _FMInteraction(torch.autograd.Function):
         eb = emb.to(torch.bfloat16).contiguous()
         out = torch.empty(B, D, dtype=torch.bfloat16, device=emb.device)
         ssum = torch.empty(B, D, dtype=torch.float32, device=emb.device)
-        _chk(lib.dr_cuda_fm_fwd(ptr(eb), D, T * D, T, D, B, ptr(out), D, ptr(ssum), stream_ptr()), "fm_fwd")
+        check(lib.dr_cuda_fm_fwd(ptr(eb), D, T * D, T, D, B, ptr(out), D, ptr(ssum), stream_ptr()), "fm_fwd")
         ctx.save_for_backward(eb, ssum)
         ctx.dt = emb.dtype
         return out.to(emb.dtype)
@@ -257,7 +252,7 @@ class _FMInteraction(torch.autograd.Function):
         B, T, D = eb.shape
         gb = g.to(torch.bfloat16).contiguous()
         de = torch.empty(B, T, D, dtype=torch.bfloat16, device=g.device)
-        _chk(lib.dr_cuda_fm_bwd(ptr(gb), D, ptr(eb), D, T * D, ptr(ssum), T, D, B, ptr(de), D, T * D, 0, stream_ptr()), "fm_bwd")
+        check(lib.dr_cuda_fm_bwd(ptr(gb), D, ptr(eb), D, T * D, ptr(ssum), T, D, B, ptr(de), D, T * D, 0, stream_ptr()), "fm_bwd")
         return de.to(ctx.dt)
 
 
@@ -280,7 +275,7 @@ class _GRURecurrenceFn(torch.autograd.Function):
         H = w_hh.shape[1]
         w, b = w_hh.detach().float().contiguous(), b_hh.detach().float().contiguous()
         y = torch.empty(B, L, H, dtype=torch.float32, device=gi.device)
-        _chk(_native.cuda().dr_cuda_gru_fwd(ptr(gi), ptr(w), ptr(b), ptr(lengths), B, L, H, ptr(y), stream_ptr()), "gru_fwd")
+        check(_native.cuda().dr_cuda_gru_fwd(ptr(gi), ptr(w), ptr(b), ptr(lengths), B, L, H, ptr(y), stream_ptr()), "gru_fwd")
         ctx.save_for_backward(gi, w, b, lengths, y)
         ctx.shape = (B, L, H)
         return y
@@ -296,8 +291,8 @@ class _GRURecurrenceFn(torch.autograd.Function):
         dw = torch.zeros(3 * H, H, dtype=torch.float32, device=dev)
         db = torch.zeros(3 * H, dtype=torch.float32, device=dev)
         dy = dy.float().contiguous()
-        _chk(_native.cuda().dr_cuda_gru_bwd(ptr(gi), ptr(w), ptr(b), ptr(lengths), ptr(y), ptr(dy), B, L, H, ptr(dgi), ptr(dgh), ptr(hprev),
-                                            ptr(dw), ptr(db), stream_ptr()), "gru_bwd")
+        check(_native.cuda().dr_cuda_gru_bwd(ptr(gi), ptr(w), ptr(b), ptr(lengths), ptr(y), ptr(dy), B, L, H, ptr(dgi), ptr(dgh), ptr(hprev),
+                                             ptr(dw), ptr(db), stream_ptr()), "gru_bwd")
         return dgi, dw, db, None, None, None
 
 

@@ -8,25 +8,13 @@ softmax over the behaviour history, weighted sum of the keys.
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 
 import torch
 import torch.nn as nn
 
 from .. import _native
-from .._native import ptr, stream_ptr
-
-def _lib():
-    L = _native.cuda()
-    if not getattr(L, "_din_bound", False):
-        P, i64, INT = C.c_void_p, C.c_int64, C.c_int
-        L.dr_cuda_din_attention_fwd.restype = INT
-        L.dr_cuda_din_attention_fwd.argtypes = [P, P, P, i64, INT, INT, P, P, INT, P, P, INT, P, C.c_float, P, P]
-        L.dr_cuda_din_attention_bwd.restype = INT
-        L.dr_cuda_din_attention_bwd.argtypes = [P, P, P, P, i64, INT, INT, P, P, INT, P, P, INT, P, C.c_float, P, P, P, P, P, P, P, P, P]
-        L._din_bound = True
-    return L
+from .._native import check, ptr, stream_ptr
 
 
 def din_attention_reference(q: torch.Tensor, k: torch.Tensor, mask: torch.Tensor, att: nn.Module) -> torch.Tensor:
@@ -79,10 +67,8 @@ class _DinAttentionFused(torch.autograd.Function):
         ws = [t.detach().float().contiguous() for t in (W1, b1, W2, b2, W3.reshape(-1))]
         b3f = float(b3.detach().float().item())
         out = torch.empty(B, D, device=q.device, dtype=torch.float32)
-        rc = _lib().dr_cuda_din_attention_fwd(ptr(qf), ptr(kf), ptr(mk), B, L, D, ptr(ws[0]), ptr(ws[1]), W1.shape[0], ptr(ws[2]), ptr(ws[3]), W2.shape[0],
-                                              ptr(ws[4]), b3f, ptr(out), stream_ptr())
-        if rc != 0:
-            raise RuntimeError(f"dr_cuda_din_attention_fwd failed: {rc}")
+        check(_native.cuda().dr_cuda_din_attention_fwd(ptr(qf), ptr(kf), ptr(mk), B, L, D, ptr(ws[0]), ptr(ws[1]), W1.shape[0], ptr(ws[2]), ptr(ws[3]),
+                                                       W2.shape[0], ptr(ws[4]), b3f, ptr(out), stream_ptr()), "din_attention_fwd")
         ctx.save_for_backward(qf, kf, mk, *ws)
         ctx.b3, ctx.dtypes = b3f, (q.dtype, k.dtype, W1.dtype, b1.dtype, W2.dtype, b2.dtype, W3.dtype, b3.dtype)
         ctx.w3_shape = W3.shape
@@ -98,10 +84,9 @@ class _DinAttentionFused(torch.autograd.Function):
         dq, dk = torch.empty_like(qf), torch.empty_like(kf)
         dW1, db1, dW2, db2 = torch.zeros_like(W1), torch.zeros_like(b1), torch.zeros_like(W2), torch.zeros_like(b2)
         dw3, db3 = torch.zeros_like(w3), torch.zeros(1, device=dev)
-        rc = _lib().dr_cuda_din_attention_bwd(ptr(qf), ptr(kf), ptr(mk), ptr(gf), B, L, D, ptr(W1), ptr(b1), H1, ptr(W2), ptr(b2), H2, ptr(w3), ctx.b3,
-                                              ptr(dq), ptr(dk), ptr(dW1), ptr(db1), ptr(dW2), ptr(db2), ptr(dw3), ptr(db3), stream_ptr())
-        if rc != 0:
-            raise RuntimeError(f"dr_cuda_din_attention_bwd failed: {rc}")
+        check(_native.cuda().dr_cuda_din_attention_bwd(ptr(qf), ptr(kf), ptr(mk), ptr(gf), B, L, D, ptr(W1), ptr(b1), H1, ptr(W2), ptr(b2), H2, ptr(w3),
+                                                       ctx.b3, ptr(dq), ptr(dk), ptr(dW1), ptr(db1), ptr(dW2), ptr(db2), ptr(dw3), ptr(db3), stream_ptr()),
+              "din_attention_bwd")
         t = ctx.dtypes
         return (dq.to(t[0]), dk.to(t[1]), None, dW1.to(t[2]), db1.to(t[3]), dW2.to(t[4]), db2.to(t[5]), dw3.view(ctx.w3_shape).to(t[6]), db3.to(t[7]))
 
@@ -127,15 +112,14 @@ def din_attention(q: torch.Tensor, k: torch.Tensor, mask: torch.Tensor, att: nn.
     qf, kf = q.detach().float().contiguous(), k.detach().float().contiguous()
     mk = mask.to(torch.bool).contiguous()
     out = torch.empty(B, D, device=q.device, dtype=torch.float32)
-    rc = _lib().dr_cuda_din_attention_fwd(ptr(qf), ptr(kf), ptr(mk), B, L, D, ptr(l1.weight.detach().float().contiguous()),
-                                          ptr(l1.bias.detach().float().contiguous()), l1.out_features,
-                                          ptr(l2.weight.detach().float().contiguous()), ptr(l2.bias.detach().float().contiguous()), l2.out_features,
-                                          ptr(l3.weight.detach().float().contiguous().view(-1)), _b3(l3),
-                                          ptr(out), stream_ptr())
+    rc = _native.cuda().dr_cuda_din_attention_fwd(ptr(qf), ptr(kf), ptr(mk), B, L, D, ptr(l1.weight.detach().float().contiguous()),
+                                                  ptr(l1.bias.detach().float().contiguous()), l1.out_features,
+                                                  ptr(l2.weight.detach().float().contiguous()), ptr(l2.bias.detach().float().contiguous()), l2.out_features,
+                                                  ptr(l3.weight.detach().float().contiguous().view(-1)), _b3(l3),
+                                                  ptr(out), stream_ptr())
     if rc == -1:                                   # shape does not fit the kernel's shared-memory budget
         return din_attention_reference(q, k, mask, att)
-    if rc != 0:
-        raise RuntimeError(f"dr_cuda_din_attention_fwd failed: {rc}")
+    check(rc, "din_attention_fwd")
     return out.to(q.dtype)
 
 

@@ -21,7 +21,7 @@ import torch
 
 from .. import _native
 from .._cuda_sigs import DeviceTableStruct
-from .._native import EvConfig, OptHyper, ptr, stream_ptr
+from .._native import EvConfig, OptHyper, check, ptr, stream_ptr
 
 EMPTY_KEY = -(1 << 63)
 _COMB = {"sum": 0, "mean": 1, "sqrtn": 2}
@@ -32,11 +32,6 @@ def _next_pow2(n: int) -> int:
     while p < n:
         p <<= 1
     return p
-
-
-def _chk(rc: int, what: str) -> None:
-    if rc != 0:
-        raise RuntimeError(f"deeprec_cuda: {what} failed with code {rc}")
 
 
 class StepContext:
@@ -105,8 +100,8 @@ class StepContext:
         if not self.pending:
             return
         self.set_hyper(hp)
-        _chk(self.lib.dr_cuda_sparse_apply(ptr(self.structs()), ptr(self.ulist), ptr(self.nuniq), self.ulist.numel(), ptr(self.gsum),
-                                           self.dim, ptr(self.hp_dev), self.claimed_upper, 1, stream_ptr()), "sparse_apply")
+        check(self.lib.dr_cuda_sparse_apply(ptr(self.structs()), ptr(self.ulist), ptr(self.nuniq), self.ulist.numel(), ptr(self.gsum),
+                                            self.dim, ptr(self.hp_dev), self.claimed_upper, 1, stream_ptr()), "sparse_apply")
         self.pending = False
         self.claimed_upper = 0
 
@@ -169,7 +164,7 @@ class DeviceTable:
         # array-of-structs: one 32-byte DrSlot {key, freq, version, row_of, tag, dirty, pad} per position (csrc/cuda/table.cuh);
         # the per-field tensors below are strided VIEWS of it (multi-tier victim selection, tests, debugging)
         self.slots = torch.empty(capacity * 4, dtype=torch.int64, device=d)
-        _chk(self.lib.dr_cuda_table_init_slots(ptr(self.slots), capacity, stream_ptr()), "init_slots")
+        check(self.lib.dr_cuda_table_init_slots(ptr(self.slots), capacity, stream_ptr()), "init_slots")
         s32 = self.slots.view(torch.int32).view(capacity, 8)
         self.keys = self.slots.view(capacity, 4)[:, 0]
         self.freq, self.version, self.row_of, self.tag, self.dirty = s32[:, 2], s32[:, 3], s32[:, 4], s32[:, 5], s32[:, 6]
@@ -230,7 +225,7 @@ class DeviceTable:
             self._alloc_keys(new_cap)
         self._refresh_struct()
         if rehash:
-            _chk(self.lib.dr_cuda_table_rehash(C.byref(old_struct), C.byref(self.struct), stream_ptr()), "rehash")
+            check(self.lib.dr_cuda_table_rehash(C.byref(old_struct), C.byref(self.struct), stream_ptr()), "rehash")
         _native.stream_sync()
         del keep
 
@@ -256,9 +251,9 @@ class DeviceTable:
         if n == 0:
             return out
         s, st = stream_ptr(), self.ctx.structs()
-        _chk(self.lib.dr_cuda_table_lookup(ptr(st), ptr(self._map), 1, ptr(k), None, n, n, 0, None, ptr(pos), None, None, 0, s), "lookup")
-        _chk(self.lib.dr_cuda_table_gather(ptr(st), ptr(self._map), 1, self.dim, ptr(k), ptr(pos), None, n, n, ptr(out),
-                                           int(out_dtype == torch.bfloat16), 0, 0, 1, s), "gather")
+        check(self.lib.dr_cuda_table_lookup(ptr(st), ptr(self._map), 1, ptr(k), None, n, n, 0, None, ptr(pos), None, None, 0, s), "lookup")
+        check(self.lib.dr_cuda_table_gather(ptr(st), ptr(self._map), 1, self.dim, ptr(k), ptr(pos), None, n, n, ptr(out),
+                                            int(out_dtype == torch.bfloat16), 0, 0, 1, s), "gather")
         return out
 
     def lookup_train(self, keys: torch.Tensor, step: int, out_dtype: torch.dtype = torch.float32):
@@ -274,10 +269,10 @@ class DeviceTable:
             return out, pos
         s, st = stream_ptr(), ctx.structs()
         ctx.set_step(step)
-        _chk(self.lib.dr_cuda_table_lookup(ptr(st), ptr(self._map), 1, ptr(k), None, n, n, 1, ptr(ctx.step_dev), ptr(pos), ptr(ctx.ulist),
-                                           ptr(ctx.nuniq), ctx.ulist.numel(), s), "lookup_train")
-        _chk(self.lib.dr_cuda_table_gather(ptr(st), ptr(self._map), 1, self.dim, ptr(k), ptr(pos), None, n, n, ptr(out),
-                                           int(out_dtype == torch.bfloat16), 0, 0, 1, s), "gather")
+        check(self.lib.dr_cuda_table_lookup(ptr(st), ptr(self._map), 1, ptr(k), None, n, n, 1, ptr(ctx.step_dev), ptr(pos), ptr(ctx.ulist),
+                                            ptr(ctx.nuniq), ctx.ulist.numel(), s), "lookup_train")
+        check(self.lib.dr_cuda_table_gather(ptr(st), ptr(self._map), 1, self.dim, ptr(k), ptr(pos), None, n, n, ptr(out),
+                                            int(out_dtype == torch.bfloat16), 0, 0, 1, s), "gather")
         ctx.pending = True
         return out, pos
 
@@ -289,9 +284,9 @@ class DeviceTable:
         g = grads.contiguous().view(n, self.dim)
         if g.dtype not in (torch.float32, torch.bfloat16):
             g = g.float()
-        _chk(self.lib.dr_cuda_sparse_accumulate(ptr(self.ctx.structs()), ptr(self._map), 1, self.dim, ptr(pos), None, n, n, ptr(g),
-                                                int(g.dtype == torch.bfloat16), 0, 0, 1, None, None, ptr(self.ctx.gsum), stream_ptr()),
-             "sparse_accumulate")
+        check(self.lib.dr_cuda_sparse_accumulate(ptr(self.ctx.structs()), ptr(self._map), 1, self.dim, ptr(pos), None, n, n, ptr(g),
+                                                 int(g.dtype == torch.bfloat16), 0, 0, 1, None, None, ptr(self.ctx.gsum), stream_ptr()),
+              "sparse_accumulate")
 
     def apply_step(self, hp: OptHyper) -> None:
         self.ctx.apply_step(hp)
@@ -317,25 +312,25 @@ class DeviceTable:
     def get_freq(self, keys: torch.Tensor) -> torch.Tensor:
         k = self._keys(keys)
         out = torch.empty(k.numel(), dtype=torch.int64, device=self.device)
-        _chk(self.lib.dr_cuda_table_get_meta(C.byref(self.struct), ptr(k), k.numel(), ptr(out), None, None, stream_ptr()), "get_meta")
+        check(self.lib.dr_cuda_table_get_meta(C.byref(self.struct), ptr(k), k.numel(), ptr(out), None, None, stream_ptr()), "get_meta")
         return out.cpu()
 
     def get_version(self, keys: torch.Tensor) -> torch.Tensor:
         k = self._keys(keys)
         out = torch.empty(k.numel(), dtype=torch.int64, device=self.device)
-        _chk(self.lib.dr_cuda_table_get_meta(C.byref(self.struct), ptr(k), k.numel(), None, ptr(out), None, stream_ptr()), "get_meta")
+        check(self.lib.dr_cuda_table_get_meta(C.byref(self.struct), ptr(k), k.numel(), None, ptr(out), None, stream_ptr()), "get_meta")
         return out.cpu()
 
     def lookup_slot(self, keys: torch.Tensor, slot: int) -> torch.Tensor:
         k = self._keys(keys)
         out = torch.empty(k.numel(), self.dim, dtype=torch.float32, device=self.device)
-        _chk(self.lib.dr_cuda_table_gather_slot(C.byref(self.struct), ptr(k), k.numel(), int(slot), ptr(out), stream_ptr()), "gather_slot")
+        check(self.lib.dr_cuda_table_gather_slot(C.byref(self.struct), ptr(k), k.numel(), int(slot), ptr(out), stream_ptr()), "gather_slot")
         return out.cpu()
 
     # ---- lifecycle -------------------------------------------------------------------------------------
     def shrink(self, step: int) -> int:
         n = torch.zeros(1, dtype=torch.int32, device=self.device)
-        _chk(self.lib.dr_cuda_table_shrink(C.byref(self.struct), int(step), ptr(n), stream_ptr()), "shrink")
+        check(self.lib.dr_cuda_table_shrink(C.byref(self.struct), int(step), ptr(n), stream_ptr()), "shrink")
         removed = int(n.item())
         if removed:
             self._purge_tombstones()
@@ -346,14 +341,14 @@ class DeviceTable:
         keep = (self.slots,)
         self._alloc_keys(self.capacity)
         self._refresh_struct()
-        _chk(self.lib.dr_cuda_table_rehash(C.byref(old_struct), C.byref(self.struct), stream_ptr()), "rehash")
+        check(self.lib.dr_cuda_table_rehash(C.byref(old_struct), C.byref(self.struct), stream_ptr()), "rehash")
         _native.stream_sync()
         del keep
 
     def remove(self, keys: torch.Tensor) -> int:
         k = self._keys(keys)
         n = torch.zeros(1, dtype=torch.int32, device=self.device)
-        _chk(self.lib.dr_cuda_table_remove(C.byref(self.struct), ptr(k), k.numel(), ptr(n), stream_ptr()), "remove")
+        check(self.lib.dr_cuda_table_remove(C.byref(self.struct), ptr(k), k.numel(), ptr(n), stream_ptr()), "remove")
         removed = int(n.item())
         self._tombstones = getattr(self, "_tombstones", 0) + removed
         if self._tombstones * 4 > self.capacity:      # probes skip tombstones; rebuild only when they pile up
@@ -362,21 +357,21 @@ class DeviceTable:
         return removed
 
     def clear_dirty(self) -> None:
-        _chk(self.lib.dr_cuda_table_clear_dirty(C.byref(self.struct), stream_ptr()), "clear_dirty")
+        check(self.lib.dr_cuda_table_clear_dirty(C.byref(self.struct), stream_ptr()), "clear_dirty")
 
     def snapshot(self, dirty_only: bool = False, part_id: int = 0, part_num: int = 1) -> Dict[str, torch.Tensor]:
         d, s = self.device, stream_ptr()
         counts = torch.zeros(2, dtype=torch.int32, device=d)
-        _chk(self.lib.dr_cuda_table_snapshot(C.byref(self.struct), int(dirty_only), part_id, part_num, ptr(counts),
-                                             None, None, None, None, None, None, None, s), "snapshot(count)")
+        check(self.lib.dr_cuda_table_snapshot(C.byref(self.struct), int(dirty_only), part_id, part_num, ptr(counts),
+                                              None, None, None, None, None, None, None, s), "snapshot(count)")
         na, nf = [int(x) for x in counts.cpu()]
         keys = torch.empty(na, dtype=torch.int64, device=d); rows = torch.empty(na, self.stride, dtype=torch.float32, device=d)
         freqs = torch.empty(na, dtype=torch.int64, device=d); vers = torch.empty(na, dtype=torch.int64, device=d)
         fkeys = torch.empty(nf, dtype=torch.int64, device=d); ffreqs = torch.empty(nf, dtype=torch.int64, device=d)
         fvers = torch.empty(nf, dtype=torch.int64, device=d)
         counts.zero_()
-        _chk(self.lib.dr_cuda_table_snapshot(C.byref(self.struct), int(dirty_only), part_id, part_num, ptr(counts), ptr(keys), ptr(rows),
-                                             ptr(freqs), ptr(vers), ptr(fkeys), ptr(ffreqs), ptr(fvers), s), "snapshot(fill)")
+        check(self.lib.dr_cuda_table_snapshot(C.byref(self.struct), int(dirty_only), part_id, part_num, ptr(counts), ptr(keys), ptr(rows),
+                                              ptr(freqs), ptr(vers), ptr(fkeys), ptr(ffreqs), ptr(fvers), s), "snapshot(fill)")
 
         def order(k):
             if k.numel() == 0:
@@ -403,8 +398,8 @@ class DeviceTable:
         f = freqs.to(self.device, torch.int64).contiguous() if freqs is not None else None
         v = versions.to(self.device, torch.int64).contiguous() if versions is not None else None
         kept = torch.zeros(1, dtype=torch.int32, device=self.device)
-        _chk(self.lib.dr_cuda_table_import(C.byref(self.struct), ptr(k), ptr(r), r.shape[1] if r is not None else 0, ptr(f), ptr(v), n,
-                                           part_id, part_num, int(reset_version), ptr(kept), stream_ptr()), "import")
+        check(self.lib.dr_cuda_table_import(C.byref(self.struct), ptr(k), ptr(r), r.shape[1] if r is not None else 0, ptr(f), ptr(v), n,
+                                            part_id, part_num, int(reset_version), ptr(kept), stream_ptr()), "import")
         return int(kept.item())
 
     def bloom_state(self):
@@ -433,14 +428,14 @@ class _GroupLookupFn(torch.autograd.Function):
             sc.ensure(nnz)
         st = sc.structs()
         sc.set_step(step)
-        _chk(lib.dr_cuda_table_lookup(ptr(st), ptr(tmap), T, ptr(keys), ptr(offs), 0, nnz, int(train), ptr(sc.step_dev), ptr(pos),
-                                      ptr(sc.ulist) if train else None, ptr(sc.nuniq) if train else None,
-                                      sc.ulist.numel() if train else 0, s), "group lookup")
+        check(lib.dr_cuda_table_lookup(ptr(st), ptr(tmap), T, ptr(keys), ptr(offs), 0, nnz, int(train), ptr(sc.step_dev), ptr(pos),
+                                       ptr(sc.ulist) if train else None, ptr(sc.nuniq) if train else None,
+                                       sc.ulist.numel() if train else 0, s), "group lookup")
         out = torch.empty(B, T, dim, dtype=torch.float32, device=dev)
         nnz_scale = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
         nnz_row = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
-        _chk(lib.dr_cuda_combine_fwd(ptr(st), ptr(tmap), T, B, dim, ptr(keys), ptr(pos), ptr(bag_offsets), ptr(weights), ptr(combiners),
-                                     ptr(out), 0, T * dim, dim, ptr(nnz_scale), ptr(nnz_row), s), "combine_fwd")
+        check(lib.dr_cuda_combine_fwd(ptr(st), ptr(tmap), T, B, dim, ptr(keys), ptr(pos), ptr(bag_offsets), ptr(weights), ptr(combiners),
+                                      ptr(out), 0, T * dim, dim, ptr(nnz_scale), ptr(nnz_row), s), "combine_fwd")
         if train:
             sc.pending = True
         ctx.sc, ctx.meta = sc, (B, T, dim, nnz)
@@ -453,8 +448,8 @@ class _GroupLookupFn(torch.autograd.Function):
         B, T, dim, nnz = ctx.meta
         sc = ctx.sc
         g = grad_out.contiguous().float()
-        _chk(sc.lib.dr_cuda_sparse_accumulate(ptr(sc.structs()), ptr(tmap), T, dim, ptr(pos), ptr(offs), 0, nnz, ptr(g), 0, T * dim, dim, 0,
-                                              ptr(nnz_row), ptr(nnz_scale), ptr(sc.gsum), stream_ptr()), "group accumulate")
+        check(sc.lib.dr_cuda_sparse_accumulate(ptr(sc.structs()), ptr(tmap), T, dim, ptr(pos), ptr(offs), 0, nnz, ptr(g), 0, T * dim, dim, 0,
+                                               ptr(nnz_row), ptr(nnz_scale), ptr(sc.gsum), stream_ptr()), "group accumulate")
         return (None,) * 9
 
 

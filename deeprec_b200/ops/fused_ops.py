@@ -2,29 +2,10 @@
 CUDA tensors run the sm_90a kernels (csrc/cuda/fused_ops.cu); CPU tensors use the equivalent torch expression."""
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 
 from .. import _native
 from .._native import ptr, stream_ptr
-
-_BOUND = False
-
-
-def _lib():
-    global _BOUND
-    lib = _native.cuda()
-    if not _BOUND:
-        i64, INT, f32, P = C.c_int64, C.c_int, C.c_float, C.c_void_p
-        for name, args in {"dr_cuda_layer_norm_fwd": [P, i64, INT, P, P, f32, P, P, P, P], "dr_cuda_layer_norm_bwd": [P, P, i64, INT, P, P, P, P, P, P, P],
-                           "dr_cuda_l2_normalize_fwd": [P, i64, INT, f32, P, P, P], "dr_cuda_l2_normalize_bwd": [P, P, P, i64, INT, P, P],
-                           "dr_cuda_gelu_fwd": [P, i64, INT, P, P], "dr_cuda_gelu_bwd": [P, P, i64, INT, P, P],
-                           "dr_cuda_dice_fwd": [P, i64, INT, P, P, P, P, P]}.items():
-            fn = getattr(lib, name); fn.argtypes, fn.restype = args, INT
-        _BOUND = True
-    return lib
-
 
 class _LayerNorm(torch.autograd.Function):
     @staticmethod
@@ -32,7 +13,7 @@ class _LayerNorm(torch.autograd.Function):
         x2 = x.contiguous().float().view(-1, x.shape[-1])
         rows, cols = x2.shape
         y = torch.empty_like(x2); mean = torch.empty(rows, device=x.device); rstd = torch.empty(rows, device=x.device)
-        _lib().dr_cuda_layer_norm_fwd(ptr(x2), rows, cols, ptr(gamma), ptr(beta), float(eps), ptr(y), ptr(mean), ptr(rstd), stream_ptr())
+        _native.cuda().dr_cuda_layer_norm_fwd(ptr(x2), rows, cols, ptr(gamma), ptr(beta), float(eps), ptr(y), ptr(mean), ptr(rstd), stream_ptr())
         ctx.save_for_backward(x2, gamma, mean, rstd); ctx.shape = x.shape
         return y.view(x.shape)
 
@@ -42,7 +23,7 @@ class _LayerNorm(torch.autograd.Function):
         rows, cols = x2.shape
         g2 = g.contiguous().float().view(rows, cols)
         dx = torch.empty_like(x2); dg = torch.zeros(cols, device=g.device); db = torch.zeros(cols, device=g.device)
-        _lib().dr_cuda_layer_norm_bwd(ptr(g2), ptr(x2), rows, cols, ptr(gamma), ptr(mean), ptr(rstd), ptr(dx), ptr(dg), ptr(db), stream_ptr())
+        _native.cuda().dr_cuda_layer_norm_bwd(ptr(g2), ptr(x2), rows, cols, ptr(gamma), ptr(mean), ptr(rstd), ptr(dx), ptr(dg), ptr(db), stream_ptr())
         return dx.view(ctx.shape), dg, db, None
 
 
@@ -58,7 +39,7 @@ class _L2Norm(torch.autograd.Function):
         x2 = x.contiguous().float().view(-1, x.shape[-1])
         rows, cols = x2.shape
         y = torch.empty_like(x2); rn = torch.empty(rows, device=x.device)
-        _lib().dr_cuda_l2_normalize_fwd(ptr(x2), rows, cols, float(eps), ptr(y), ptr(rn), stream_ptr())
+        _native.cuda().dr_cuda_l2_normalize_fwd(ptr(x2), rows, cols, float(eps), ptr(y), ptr(rn), stream_ptr())
         ctx.save_for_backward(y, rn); ctx.shape = x.shape
         return y.view(x.shape)
 
@@ -68,7 +49,7 @@ class _L2Norm(torch.autograd.Function):
         rows, cols = y.shape
         g2 = g.contiguous().float().view(rows, cols)
         dx = torch.empty_like(y)
-        _lib().dr_cuda_l2_normalize_bwd(ptr(g2), ptr(y), ptr(rn), rows, cols, ptr(dx), stream_ptr())
+        _native.cuda().dr_cuda_l2_normalize_bwd(ptr(g2), ptr(y), ptr(rn), rows, cols, ptr(dx), stream_ptr())
         return dx.view(ctx.shape), None
 
 
@@ -84,7 +65,7 @@ class _Gelu(torch.autograd.Function):
     def forward(ctx, x, approximate):
         x2 = x.contiguous().float()
         y = torch.empty_like(x2)
-        _lib().dr_cuda_gelu_fwd(ptr(x2), x2.numel(), int(approximate), ptr(y), stream_ptr())
+        _native.cuda().dr_cuda_gelu_fwd(ptr(x2), x2.numel(), int(approximate), ptr(y), stream_ptr())
         ctx.save_for_backward(x2); ctx.approx = approximate
         return y
 
@@ -92,7 +73,7 @@ class _Gelu(torch.autograd.Function):
     def backward(ctx, g):
         (x2,) = ctx.saved_tensors
         dx = torch.empty_like(x2)
-        _lib().dr_cuda_gelu_bwd(ptr(g.contiguous().float()), ptr(x2), x2.numel(), int(ctx.approx), ptr(dx), stream_ptr())
+        _native.cuda().dr_cuda_gelu_bwd(ptr(g.contiguous().float()), ptr(x2), x2.numel(), int(ctx.approx), ptr(dx), stream_ptr())
         return dx, None
 
 
@@ -108,8 +89,8 @@ def dice(x, alpha, mean, var, eps: float = 1e-9):
     if x.is_cuda and not x.requires_grad:
         x2 = x.contiguous().float().view(-1, x.shape[-1])
         y = torch.empty_like(x2)
-        _lib().dr_cuda_dice_fwd(ptr(x2), x2.shape[0], x2.shape[1], ptr(mean.contiguous().float()), ptr(rstd.contiguous().float()),
-                                ptr(alpha.contiguous().float()), ptr(y), stream_ptr())
+        _native.cuda().dr_cuda_dice_fwd(ptr(x2), x2.shape[0], x2.shape[1], ptr(mean.contiguous().float()), ptr(rstd.contiguous().float()),
+                                        ptr(alpha.contiguous().float()), ptr(y), stream_ptr())
         return y.view(x.shape)
     p = torch.sigmoid((x - mean) * rstd)
     return p * x + (1 - p) * alpha * x

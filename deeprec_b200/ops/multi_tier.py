@@ -19,9 +19,9 @@ from typing import Dict, Optional
 
 import torch
 
-from .._native import EvConfig, OptHyper, ptr, stream_ptr
+from .._native import EvConfig, OptHyper, check, ptr, stream_ptr
 from ..embedding_variable import HostTable
-from .device_table import DeviceTable, _chk
+from .device_table import DeviceTable
 
 
 class MultiTierTable:
@@ -74,8 +74,8 @@ class MultiTierTable:
         if protect is not None and protect.numel():
             # pinned / in-flight keys must stay: find their positions and lift their score
             pos = torch.empty(protect.numel(), dtype=torch.int32, device=self.device)
-            _chk(self.lib.dr_cuda_table_lookup(ptr(t.ctx.structs()), ptr(t._map), 1, ptr(protect), None, protect.numel(), protect.numel(), 0, None,
-                                               ptr(pos), None, None, 0, stream_ptr()), "lookup(protect)")
+            check(self.lib.dr_cuda_table_lookup(ptr(t.ctx.structs()), ptr(t._map), 1, ptr(protect), None, protect.numel(), protect.numel(), 0, None,
+                                                ptr(pos), None, None, 0, stream_ptr()), "lookup(protect)")
             ok = pos >= 0
             score[pos[ok].long()] = float("inf")
         n_evict = min(n_evict, int(torch.isfinite(score).sum()))
@@ -87,7 +87,7 @@ class MultiTierTable:
         rows = torch.empty(n_evict, self.stride, dtype=torch.float32, device=self.device)
         freqs = torch.empty(n_evict, dtype=torch.int64, device=self.device); vers = torch.empty(n_evict, dtype=torch.int64, device=self.device)
         found = torch.empty(n_evict, dtype=torch.uint8, device=self.device)
-        _chk(self.lib.dr_cuda_table_export_keys(C.byref(t.struct), ptr(vkeys), n_evict, ptr(rows), ptr(freqs), ptr(vers), ptr(found), stream_ptr()), "export_keys")
+        check(self.lib.dr_cuda_table_export_keys(C.byref(t.struct), ptr(vkeys), n_evict, ptr(rows), ptr(freqs), ptr(vers), ptr(found), stream_ptr()), "export_keys")
         self.dram.import_(vkeys.cpu(), rows.cpu(), freqs.cpu(), vers.cpu())     # BatchCommit into the host tier
         t.remove(vkeys)
 
@@ -96,8 +96,8 @@ class MultiTierTable:
         uniq = torch.unique(k)
         pos = torch.empty(uniq.numel(), dtype=torch.int32, device=self.device)
         t = self.hbm
-        _chk(self.lib.dr_cuda_table_lookup(ptr(t.ctx.structs()), ptr(t._map), 1, ptr(uniq), None, uniq.numel(), uniq.numel(), 0, None, ptr(pos),
-                                           None, None, 0, stream_ptr()), "lookup(presence)")
+        check(self.lib.dr_cuda_table_lookup(ptr(t.ctx.structs()), ptr(t._map), 1, ptr(uniq), None, uniq.numel(), uniq.numel(), 0, None, ptr(pos),
+                                            None, None, 0, stream_ptr()), "lookup(presence)")
         miss = uniq[pos < 0]
         self.hits += int(uniq.numel() - miss.numel()); self.misses += int(miss.numel())
         protect = uniq if self._pinned is None else torch.unique(torch.cat([uniq, self._pinned]))
@@ -165,7 +165,7 @@ class MultiTierTable:
         """0 = HBM, 1 = DRAM only, -1 = absent (KvResourceLookupTier)."""
         k = keys.to(self.device, torch.int64).reshape(-1)
         row = torch.empty(k.numel(), dtype=torch.int32, device=self.device)
-        _chk(self.lib.dr_cuda_table_get_meta(C.byref(self.hbm.struct), ptr(k), k.numel(), None, None, ptr(row), stream_ptr()), "get_meta")
+        check(self.lib.dr_cuda_table_get_meta(C.byref(self.hbm.struct), ptr(k), k.numel(), None, None, ptr(row), stream_ptr()), "get_meta")
         in_hbm = (row >= 0).cpu()
         n = k.numel()
         kc = k.cpu().contiguous()

@@ -17,6 +17,9 @@ import ctypes as C
 
 import torch
 
+from .. import _native
+from .._native import check, stream_ptr
+
 E4M3_MAX = 448.0
 
 
@@ -72,15 +75,6 @@ def dequantize_mxfp8(q: torch.Tensor, sf: torch.Tensor) -> torch.Tensor:
     return (q.view(torch.float8_e4m3fn).float().reshape(R, Kp // 32, 32) * scale.unsqueeze(2)).reshape(R, Kp)
 
 
-def _lib():
-    from .. import _native
-    return _native.cuda()
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def quantize_mxfp8(x: torch.Tensor):
     """CUDA quantiser (k_quantize_mxfp8): x [R, C] fp32 / bf16 on the device -> (q uint8 [R, Kp], sf int32 [sf_words])."""
     assert x.is_cuda and x.dim() == 2 and x.stride(1) == 1 and x.dtype in (torch.float32, torch.bfloat16)
@@ -88,10 +82,8 @@ def quantize_mxfp8(x: torch.Tensor):
     Kp = padded_k(Cc)
     q = torch.empty(R, Kp, dtype=torch.uint8, device=x.device)
     sf = torch.zeros(sf_words(R, Kp), dtype=torch.int32, device=x.device)
-    rc = _lib().dr_cuda_quantize_mxfp8(C.c_void_p(x.data_ptr()), int(x.dtype == torch.bfloat16), R, Cc, x.stride(0), C.c_void_p(q.data_ptr()), Kp,
-                                       C.c_void_p(sf.data_ptr()), _stream())
-    if rc != 0:
-        raise RuntimeError(f"dr_cuda_quantize_mxfp8 failed: {rc}")
+    check(_native.cuda().dr_cuda_quantize_mxfp8(C.c_void_p(x.data_ptr()), int(x.dtype == torch.bfloat16), R, Cc, x.stride(0), C.c_void_p(q.data_ptr()),
+                                                Kp, C.c_void_p(sf.data_ptr()), stream_ptr()), "quantize_mxfp8")
     return q, sf
 
 
@@ -100,11 +92,9 @@ def mxfp8_gemm(aq, sfa, bq, sfb, n: int, bias=None, relu: bool = False, max_ctas
     M, Kp = aq.shape
     assert bq.shape[1] == Kp and bq.shape[0] >= n and n % 8 == 0
     out = torch.empty(M, n, dtype=torch.bfloat16, device=aq.device)
-    rc = _lib().dr_cuda_gemm_mxfp8_tn(C.c_void_p(aq.data_ptr()), C.c_void_p(sfa.data_ptr()), C.c_void_p(bq.data_ptr()), C.c_void_p(sfb.data_ptr()), M, n, Kp,
-                                      C.c_void_p(bias.data_ptr()) if bias is not None else None, int(relu), C.c_void_p(out.data_ptr()), n, max_ctas,
-                                      _stream())
-    if rc != 0:
-        raise RuntimeError(f"dr_cuda_gemm_mxfp8_tn failed: {rc}")
+    check(_native.cuda().dr_cuda_gemm_mxfp8_tn(C.c_void_p(aq.data_ptr()), C.c_void_p(sfa.data_ptr()), C.c_void_p(bq.data_ptr()), C.c_void_p(sfb.data_ptr()),
+                                               M, n, Kp, C.c_void_p(bias.data_ptr()) if bias is not None else None, int(relu), C.c_void_p(out.data_ptr()), n,
+                                               max_ctas, stream_ptr()), "gemm_mxfp8_tn")
     return out
 
 

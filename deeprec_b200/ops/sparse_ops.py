@@ -8,40 +8,19 @@ CUDA tensors run ``csrc/cuda/sparse_utils.cu`` (every data-dependent size stays 
 count per call); CPU tensors use the equivalent torch expressions below, which are also the oracle of the GPU tests."""
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional, Sequence, Tuple
 
 import torch
 
 from .. import _native
-from .._native import ptr, stream_ptr
+from .._native import check, ptr, stream_ptr
 from .embedding_ops import SparseIds
 
 _MODES = {"sum": 0, "mean": 1, "sqrtn": 2}
 
 
-def _lib():
-    lib = _native.cuda()
-    if not getattr(lib, "_spu_bound", False):
-        i64, INT, P = C.c_int64, C.c_int, C.c_void_p
-        lib.dr_cuda_sparse_utils_workspace.argtypes, lib.dr_cuda_sparse_utils_workspace.restype = [i64, i64], i64
-        for name, args in {"dr_cuda_sparse_prune_fill": [P, P, P, i64, i64, INT, INT, i64, P, P, P, P, P, P, P],
-                           "dr_cuda_sparse_slice": [P, P, INT, i64, INT, P, P, P, P, P, P, P],
-                           "dr_cuda_sparse_reshape": [P, i64, INT, P, INT, P, P, P],
-                           "dr_cuda_sparse_segment_fwd": [P, i64, INT, P, P, i64, i64, INT, P, P],
-                           "dr_cuda_sparse_segment_bwd": [P, i64, INT, P, P, i64, i64, INT, P, P]}.items():
-            fn = getattr(lib, name); fn.argtypes, fn.restype = args, INT
-        lib._spu_bound = True
-    return lib
-
-
-def _chk(rc: int, what: str) -> None:
-    if rc != 0:
-        raise RuntimeError(f"{what} failed (rc {rc})")
-
-
 def _workspace(nnz: int, rows: int, dev) -> torch.Tensor:
-    return torch.empty(int(_lib().dr_cuda_sparse_utils_workspace(nnz, rows)), dtype=torch.uint8, device=dev)
+    return torch.empty(int(_native.cuda().dr_cuda_sparse_utils_workspace(nnz, rows)), dtype=torch.uint8, device=dev)
 
 
 # ------------------------------------------------------------------------------------------------------------ prune + fill-empty-rows
@@ -79,8 +58,8 @@ def sparse_prune_fill(sp: SparseIds, default_id: Optional[int] = None, prune: bo
     empty = torch.empty(B, dtype=torch.int32, device=dev)
     count = torch.zeros(1, dtype=torch.int64, device=dev)
     ws = _workspace(nnz, B, dev)
-    _chk(_lib().dr_cuda_sparse_prune_fill(ptr(v), ptr(r), ptr(wf), nnz, B, int(prune), int(fill), int(default_id or 0), ptr(ov), ptr(orow), ptr(ow), ptr(empty),
-                                          ptr(count), ptr(ws), stream_ptr()), "sparse_prune_fill")
+    check(_native.cuda().dr_cuda_sparse_prune_fill(ptr(v), ptr(r), ptr(wf), nnz, B, int(prune), int(fill), int(default_id or 0), ptr(ov), ptr(orow), ptr(ow), ptr(empty),
+                                                   ptr(count), ptr(ws), stream_ptr()), "sparse_prune_fill")
     n = int(count.item())                                   # the one host read of this op
     return SparseIds(ov[:n], orow[:n], B, ow[:n].to(w.dtype) if ow is not None else None), empty.bool()
 
@@ -109,8 +88,8 @@ def sparse_slice(indices: torch.Tensor, values: torch.Tensor, shape: Sequence[in
     oi, ov = torch.empty_like(idx), torch.empty_like(val)
     count = torch.zeros(1, dtype=torch.int64, device=dev)
     ws = _workspace(nnz, 1, dev)
-    _chk(_lib().dr_cuda_sparse_slice(ptr(idx), ptr(val), val.element_size(), nnz, R, ptr(st), ptr(sz), ptr(oi), ptr(ov), ptr(count), ptr(ws), stream_ptr()),
-         "sparse_slice")
+    check(_native.cuda().dr_cuda_sparse_slice(ptr(idx), ptr(val), val.element_size(), nnz, R, ptr(st), ptr(sz), ptr(oi), ptr(ov), ptr(count), ptr(ws), stream_ptr()),
+          "sparse_slice")
     n = int(count.item())
     return oi[:n], ov[:n], out_shape
 
@@ -150,7 +129,7 @@ def sparse_reshape(indices: torch.Tensor, shape: Sequence[int], new_shape: Seque
     idx = indices.contiguous()
     s0 = torch.tensor([int(d) for d in shape], dtype=torch.int64, device=dev); s1 = torch.tensor(new_shape, dtype=torch.int64, device=dev)
     out = torch.empty(idx.shape[0], R1, dtype=torch.int64, device=dev)
-    _chk(_lib().dr_cuda_sparse_reshape(ptr(idx), idx.shape[0], R0, ptr(s0), R1, ptr(s1), ptr(out), stream_ptr()), "sparse_reshape")
+    check(_native.cuda().dr_cuda_sparse_reshape(ptr(idx), idx.shape[0], R0, ptr(s0), R1, ptr(s1), ptr(out), stream_ptr()), "sparse_reshape")
     return out, new_shape
 
 
@@ -171,8 +150,8 @@ class _SparseSegment(torch.autograd.Function):
         d = data.contiguous().float()
         N, D = d.shape
         out = torch.empty(num_segments, D, dtype=torch.float32, device=d.device)
-        _chk(_lib().dr_cuda_sparse_segment_fwd(ptr(d), N, D, ptr(indices), ptr(segment_ids), indices.numel(), num_segments, mode, ptr(out), stream_ptr()),
-             "sparse_segment_fwd")
+        check(_native.cuda().dr_cuda_sparse_segment_fwd(ptr(d), N, D, ptr(indices), ptr(segment_ids), indices.numel(), num_segments, mode, ptr(out), stream_ptr()),
+              "sparse_segment_fwd")
         ctx.save_for_backward(indices, segment_ids); ctx.N, ctx.mode, ctx.dtype = N, mode, data.dtype
         return out.to(data.dtype)
 
@@ -182,8 +161,8 @@ class _SparseSegment(torch.autograd.Function):
         g2 = g.contiguous().float()
         S, D = g2.shape
         dd = torch.zeros(ctx.N, D, dtype=torch.float32, device=g.device)
-        _chk(_lib().dr_cuda_sparse_segment_bwd(ptr(g2), S, D, ptr(indices), ptr(segment_ids), indices.numel(), ctx.N, ctx.mode, ptr(dd), stream_ptr()),
-             "sparse_segment_bwd")
+        check(_native.cuda().dr_cuda_sparse_segment_bwd(ptr(g2), S, D, ptr(indices), ptr(segment_ids), indices.numel(), ctx.N, ctx.mode, ptr(dd), stream_ptr()),
+              "sparse_segment_bwd")
         return dd.to(ctx.dtype), None, None, None, None
 
 

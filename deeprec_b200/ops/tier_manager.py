@@ -14,26 +14,11 @@ from typing import Dict, Optional
 import torch
 
 from .. import _native
-from .._native import EvConfig, ptr
+from .._native import EvConfig, check, ptr, stream_ptr
 from ..embedding_variable import HostTable
 from .device_table import DeviceTable
 
-vp, i64, i32 = C.c_void_p, C.c_int64, C.c_int32
-
-
-def _bind(lib):
-    if getattr(lib, "_tier_bound", False):
-        return lib
-    lib.dr_tier_create.argtypes, lib.dr_tier_create.restype = [vp, vp, vp, C.c_int, i64, i64, C.c_int], vp
-    lib.dr_tier_destroy.argtypes, lib.dr_tier_destroy.restype = [vp], None
-    lib.dr_tier_prefetch.argtypes, lib.dr_tier_prefetch.restype = [vp, vp, vp, i64, i64, C.c_uint32, vp], C.c_int
-    lib.dr_tier_prefetch_mp.argtypes, lib.dr_tier_prefetch_mp.restype = [vp, vp, vp, i64, i64, C.c_uint32, vp, vp, C.c_int, C.c_int, vp], C.c_int
-    lib.dr_tier_commit.argtypes, lib.dr_tier_commit.restype = [vp, vp, C.c_uint32, vp], i64
-    lib.dr_tier_evict.argtypes, lib.dr_tier_evict.restype = [vp, vp, i32, C.c_uint32, i64, C.c_int, vp], C.c_int
-    lib.dr_tier_drain.argtypes, lib.dr_tier_drain.restype = [vp], None
-    lib.dr_tier_stats.argtypes, lib.dr_tier_stats.restype = [vp, vp], None
-    lib._tier_bound = True
-    return lib
+vp, i64 = C.c_void_p, C.c_int64
 
 
 class DeviceTierManager:
@@ -59,7 +44,7 @@ class DeviceTierManager:
         if host.stride != table.stride:
             raise ValueError(f"tier row layouts differ: host stride {host.stride}, device stride {table.stride}")
         self.host = host
-        self.lib = _bind(_native.cuda())
+        self.lib = _native.cuda()
         hl = _native.host()
         fexp = C.cast(hl.dr_host_ev_export_keys, vp)
         fimp = C.cast(hl.dr_host_ev_import, vp)
@@ -123,7 +108,7 @@ class DeviceTierManager:
     def commit(self, step: int) -> int:
         """Step boundary (before the step that consumes the prefetched batch is launched): promoted rows are imported on the current
         stream; cold rows are demoted when the slab passed its high watermark.  Returns the number of promoted rows."""
-        s = None if self.emu else vp(torch.cuda.current_stream(self.dev).cuda_stream)
+        s = stream_ptr(self.dev)
         self._epoch += 1
         n = int(self.lib.dr_tier_commit(self.h, C.byref(self.table.struct), self._epoch, s))
         if n < 0:
@@ -149,9 +134,7 @@ class DeviceTierManager:
         self.drain()
         k = keys.to(self.dev, torch.int64).reshape(-1)
         row = torch.empty(k.numel(), dtype=torch.int32, device=self.dev)
-        from .device_table import _chk
-        from .._native import stream_ptr
-        _chk(self.lib.dr_cuda_table_get_meta(C.byref(self.table.struct), ptr(k), k.numel(), None, None, ptr(row), stream_ptr()), "get_meta")
+        check(self.lib.dr_cuda_table_get_meta(C.byref(self.table.struct), ptr(k), k.numel(), None, None, ptr(row), stream_ptr()), "get_meta")
         out = self.table.lookup(k)
         in_hbm = (row >= 0)
         kc = k.cpu()

@@ -23,40 +23,11 @@ from typing import Optional
 import torch
 
 from .. import _native
-from .._native import ptr
-from .sparse_pipeline import Peers, SpSync, _LocalBuffer, bind as _bind_sp
+from .._cuda_sigs import AgGeom, AgPeers, SpSync
+from .._native import check, ptr, stream_ptr
+from .sparse_pipeline import _LocalBuffer
 
-vp, i32, i64 = C.c_void_p, C.c_int32, C.c_int64
 CH_IDS, CH_ROWS, CH_GRAD, CH_DONE = 0, 1, 2, 4
-
-
-class AgGeom(C.Structure):
-    """Mirror of DrAgGeom."""
-    _fields_ = [("W", i32), ("rank", i32), ("dim", i32), ("table_index", i32), ("B", i64), ("nnz_cap", i64)]
-
-
-class AgPeers(C.Structure):
-    """Mirror of DrAgPeers."""
-    _fields_ = [("keys", Peers), ("rows", Peers), ("meta", Peers), ("partial", Peers), ("grad", Peers)]
-
-
-def _bind(lib):
-    if getattr(lib, "_ag_bound", False):
-        return lib
-    INT, P = C.c_int, vp
-    GP, PP, SP = C.POINTER(AgGeom), C.POINTER(AgPeers), C.POINTER(SpSync)
-    lib.dr_ag_lookup.argtypes, lib.dr_ag_lookup.restype = [P, GP, PP, INT, P, P, P, P, P, i64, SP, P], INT
-    lib.dr_ag_reduce.argtypes, lib.dr_ag_reduce.restype = [GP, PP, P, P, SP, P], INT
-    lib.dr_ag_grad.argtypes, lib.dr_ag_grad.restype = [P, GP, PP, P, P, P, P, i64, SP, P], INT
-    lib.dr_ag_sizeof_geom.argtypes, lib.dr_ag_sizeof_geom.restype = [], INT
-    assert lib.dr_ag_sizeof_geom() == C.sizeof(AgGeom)
-    lib._ag_bound = True
-    return lib
-
-
-def _chk(rc, what):
-    if rc != 0:
-        raise RuntimeError(f"deeprec_cuda all-gather embedding: {what} failed with code {rc}")
 
 
 class AllGatherEmbedding:
@@ -68,7 +39,7 @@ class AllGatherEmbedding:
         if world > 16:
             raise ValueError("one peer-memory domain: at most 16 ranks")
         self.dev, self.rank, self.W, self.table, self.B, self.D, self.nnz_cap = dev, rank, world, table, int(batch), int(table.dim), int(nnz_cap)
-        self.lib = _bind(_bind_sp(_native.cuda()))
+        self.lib = _native.cuda()
         sym = (lambda nb: comm.symmetric(nb)) if world > 1 else (lambda nb: _LocalBuffer(dev, nb))
         self.keys_buf, self.rows_buf, self.meta_buf = sym(self.nnz_cap * 8), sym(self.nnz_cap * 4), sym(64)
         self.partial_buf, self.grad_buf, self.flags_buf = sym(world * self.B * self.D * 4), sym(self.B * self.D * 4), sym(8 * 16 * 4)
@@ -93,11 +64,8 @@ class AllGatherEmbedding:
         if world > 1:
             comm.host_barrier()
 
-    def _s(self):
-        return None if _native.emu_active() else vp(torch.cuda.current_stream(self.dev).cuda_stream)
-
     def _signal(self, ch: int) -> None:
-        _chk(self.lib.dr_sp_signal(C.byref(self.sync), ch, self._s()), "signal")
+        check(self.lib.dr_sp_signal(C.byref(self.sync), ch, stream_ptr(self.dev)), "signal")
 
     # ---- requester side -------------------------------------------------------------------------------------------------------------------
     def load_ids(self, values: torch.Tensor, row_ids: torch.Tensor) -> None:
@@ -117,7 +85,7 @@ class AllGatherEmbedding:
             cnt = torch.bincount(self._rows_now.to(torch.int64), minlength=self.B).clamp(min=1).to(torch.float32)
             self._scale = (1.0 / cnt if combiner == "mean" else cnt.rsqrt()).to(self.dev).contiguous()
         out = torch.empty(self.B, self.D, dtype=torch.float32, device=self.dev)
-        _chk(self.lib.dr_ag_reduce(C.byref(self.geom), C.byref(self.peers), ptr(self._scale), ptr(out), C.byref(self.sync), self._s()), "reduce")
+        check(self.lib.dr_ag_reduce(C.byref(self.geom), C.byref(self.peers), ptr(self._scale), ptr(out), C.byref(self.sync), stream_ptr(self.dev)), "reduce")
         return out
 
     def stage_grad(self, dout: torch.Tensor) -> None:
@@ -132,13 +100,13 @@ class AllGatherEmbedding:
     def lookup(self, ctx, train: bool) -> None:
         if train:
             ctx.ensure(self.W * self.nnz_cap)
-        _chk(self.lib.dr_ag_lookup(ptr(ctx.structs()), C.byref(self.geom), C.byref(self.peers), int(train), ptr(self.own_pos), ptr(self.own_row), ptr(self.own_cnt),
-                                   ptr(ctx.ulist) if train else None, ptr(ctx.nuniq) if train else None, ctx.ulist.numel() if train else 0, C.byref(self.sync), self._s()),
-             "lookup")
+        check(self.lib.dr_ag_lookup(ptr(ctx.structs()), C.byref(self.geom), C.byref(self.peers), int(train), ptr(self.own_pos), ptr(self.own_row), ptr(self.own_cnt),
+                                    ptr(ctx.ulist) if train else None, ptr(ctx.nuniq) if train else None, ctx.ulist.numel() if train else 0, C.byref(self.sync), stream_ptr(self.dev)),
+              "lookup")
 
     def grad(self, ctx) -> None:
-        _chk(self.lib.dr_ag_grad(ptr(ctx.structs()), C.byref(self.geom), C.byref(self.peers), ptr(self.own_pos), ptr(self.own_row), ptr(self.own_cnt), ptr(ctx.gsum),
-                                 ctx.ulist.numel(), C.byref(self.sync), self._s()), "grad")
+        check(self.lib.dr_ag_grad(ptr(ctx.structs()), C.byref(self.geom), C.byref(self.peers), ptr(self.own_pos), ptr(self.own_row), ptr(self.own_cnt), ptr(ctx.gsum),
+                                  ctx.ulist.numel(), C.byref(self.sync), stream_ptr(self.dev)), "grad")
 
     def step_end(self) -> None:
-        _chk(self.lib.dr_sp_step_end(ptr(self.state), self._s()), "step_end")
+        check(self.lib.dr_sp_step_end(ptr(self.state), stream_ptr(self.dev)), "step_end")

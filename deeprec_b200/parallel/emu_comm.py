@@ -10,7 +10,9 @@ from typing import Dict, List
 
 import torch
 
-from .sparse_pipeline import Peers
+from .. import _native
+from .._cuda_sigs import Peers
+from .._native import check, ptr
 
 
 class EmuWorld:
@@ -77,21 +79,16 @@ class EmuComm:
 
     def dense_allreduce_update(self, eng) -> None:
         """DENSE flag + the one-shot peer-pull all-reduce fused with the optimizer (comm_kernels.cu: k_allreduce_apply polls the flags itself)."""
-        from .. import _native
-        from .._native import ptr
         sp = eng.sp
         sp.signal(3)
-        rc = _native.cuda().dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, ptr(eng.params), ptr(eng.s0) if eng.s0 is not None else None,
-                                                         ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), None)
-        if rc != 0:
-            raise RuntimeError(f"allreduce_apply failed ({rc})")
+        check(_native.cuda().dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, ptr(eng.params), ptr(eng.s0) if eng.s0 is not None else None,
+                                                          ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), None),
+              "allreduce_apply")
         self.launches += 1
 
     def wait_dense(self, sp) -> None:
-        from .. import _native
-        rc = _native.cuda().dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, None, None, None, 0, None, None, sp.sync_ref(), None)
-        if rc != 0:
-            raise RuntimeError(f"wait_dense failed ({rc})")
+        check(_native.cuda().dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, None, None, None, 0, None, None, sp.sync_ref(), None),
+              "wait_dense")
         self.launches += 1
 
     def host_broadcast(self, tensors, src: int = 0) -> None:

@@ -20,12 +20,7 @@ import torch
 import torch.distributed as dist
 
 from .. import _native
-from .._native import OptHyper, ptr
-
-
-def _chk(rc, what):
-    if rc != 0:
-        raise RuntimeError(f"deeprec_cuda: {what} failed with code {rc}")
+from .._native import OptHyper, check, ptr, stream_ptr
 
 
 class NcclComm:
@@ -82,7 +77,7 @@ class NcclComm:
         self._setup(eng)
         nb, W, B, D, lib = eng._nb, self.world, eng.B, eng.D, self.lib
         nl = len(nb.owned[self.rank])
-        s = torch.cuda.current_stream(self.dev).cuda_stream
+        s = stream_ptr(self.dev)
         # 1. pack ids by owner, NCCL all-to-all (C2)
         nb.keys_send.copy_(eng.ids.index_select(0, nb.perm).view(-1))
         self.launches += 1
@@ -92,10 +87,10 @@ class NcclComm:
         if n:
             ctx = eng.group.ctx
             st = ctx.structs()
-            _chk(lib.dr_cuda_table_lookup(ptr(st), ptr(nb.tmap), W * nl, ptr(nb.keys_recv), None, B, n, int(train), nb.step_ptr, ptr(eng.pos),
-                                          ptr(ctx.ulist) if train else None, ptr(ctx.nuniq) if train else None,
-                                          ctx.ulist.numel() if train else 0, s), "lookup")
-            _chk(lib.dr_cuda_table_gather(ptr(st), ptr(nb.tmap), W * nl, D, ptr(nb.keys_recv), ptr(eng.pos), None, B, n, ptr(nb.rows_send), 1, 0, 0, 1, s), "gather")
+            check(lib.dr_cuda_table_lookup(ptr(st), ptr(nb.tmap), W * nl, ptr(nb.keys_recv), None, B, n, int(train), nb.step_ptr, ptr(eng.pos),
+                                           ptr(ctx.ulist) if train else None, ptr(ctx.nuniq) if train else None,
+                                           ctx.ulist.numel() if train else 0, s), "lookup")
+            check(lib.dr_cuda_table_gather(ptr(st), ptr(nb.tmap), W * nl, D, ptr(nb.keys_recv), ptr(eng.pos), None, B, n, ptr(nb.rows_send), 1, 0, 0, 1, s), "gather")
             self.launches += 2
         # 3. NCCL all-to-all of the vectors (C3) + un-permute into feature-major order (S2 reorderKernel)
         self._a2a(nb.rows_recv, nb.rows_send[: W * nl * B], [c for c in nb.send_counts_ids], [c for c in nb.recv_counts_ids])
@@ -105,15 +100,15 @@ class NcclComm:
     def sparse_backward(self, eng) -> None:
         nb, W, B, D, lib = eng._nb, self.world, eng.B, eng.D, self.lib
         nl = len(nb.owned[self.rank])
-        s = torch.cuda.current_stream(self.dev).cuda_stream
+        s = stream_ptr(self.dev)
         nb.grad_send.copy_(eng.demb.index_select(0, nb.perm).view(-1, D))
         self.launches += 1
         self._a2a(nb.grad_recv[: W * nl * B], nb.grad_send, nb.recv_counts_ids, nb.send_counts_ids)     # C4
         n = W * nl * B
         if n:
             ctx = eng.group.ctx
-            _chk(lib.dr_cuda_sparse_accumulate(ptr(ctx.structs()), ptr(nb.tmap), W * nl, D, ptr(eng.pos), None, B, n, ptr(nb.grad_recv), 1, 0, 0, 1,
-                                               None, None, ptr(ctx.gsum), s), "accumulate")
+            check(lib.dr_cuda_sparse_accumulate(ptr(ctx.structs()), ptr(nb.tmap), W * nl, D, ptr(eng.pos), None, B, n, ptr(nb.grad_recv), 1, 0, 0, 1,
+                                                None, None, ptr(ctx.gsum), s), "accumulate")
             self.launches += 1
         eng.group.apply()
 
@@ -121,9 +116,9 @@ class NcclComm:
         if self.world > 1:
             dist.all_reduce(eng.grads, group=self.group)                                                                              # C1
             self.launches += 1
-        s = torch.cuda.current_stream(self.dev).cuda_stream
-        _chk(self.lib.dr_cuda_dense_apply(ptr(eng.params), ptr(eng.grads), ptr(eng.s0) if eng.s0 is not None else None,
-                                          ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), 1.0, None, s), "dense_apply")
+        s = stream_ptr(self.dev)
+        check(self.lib.dr_cuda_dense_apply(ptr(eng.params), ptr(eng.grads), ptr(eng.s0) if eng.s0 is not None else None,
+                                           ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), 1.0, None, s), "dense_apply")
         self.launches += 1
 
 
@@ -171,7 +166,7 @@ class BaselineDLRM:
             for p in net.parameters():
                 p.grad.copy_(flat[o:o + p.numel()].view_as(p)); o += p.numel()
         self.opt.step()
-        _chk(eng.lib.dr_cuda_advance_hyper(ptr(eng.hp_dev), torch.cuda.current_stream(self.dev).cuda_stream), "advance")
+        check(eng.lib.dr_cuda_advance_hyper(ptr(eng.hp_dev), stream_ptr(self.dev)), "advance")
         self.loss.copy_(loss.detach() * self.world)
         self.launches += 120      # ~60 ATen/cuBLAS kernels fwd+bwd+optimizer; only our table kernels are "ours"
 

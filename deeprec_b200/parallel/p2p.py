@@ -22,8 +22,9 @@ import torch
 import torch.distributed as dist
 
 from .. import _native
-from .._native import ptr
-from .sparse_pipeline import CH_DENSE, Peers, bind as _bind_sp
+from .._cuda_sigs import Peers
+from .._native import check, ptr, stream_ptr
+from .sparse_pipeline import CH_DENSE
 
 vp = C.c_void_p
 
@@ -31,38 +32,6 @@ vp = C.c_void_p
 class _RawCuda:
     def __init__(self, addr: int, nbytes: int):
         self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (addr, False), "version": 3}
-
-
-def _bind(lib):
-    if getattr(lib, "_comm_bound", False):
-        return
-    i64, INT, P = C.c_int64, C.c_int, C.c_void_p
-    PP = C.POINTER(Peers)
-    sigs = {
-        "dr_cuda_set_device": [INT], "dr_cuda_get_device": [],
-        "dr_comm_alloc": [i64, C.POINTER(vp)], "dr_comm_free": [P], "dr_comm_get_handle": [P, P],
-        "dr_comm_open_handle": [P, C.POINTER(vp)], "dr_comm_close_handle": [P], "dr_comm_can_access_peer": [INT, INT],
-        "dr_comm_barrier": [PP, P, INT, INT, INT, P],
-        "dr_comm_allreduce_apply": [PP, INT, P, P, P, i64, P, P, P],
-        "dr_nvls_supported": [INT],
-        "dr_nvls_create": [i64, INT, INT, C.POINTER(vp), C.POINTER(C.c_int)],
-        "dr_nvls_import": [INT, i64, INT, INT, C.POINTER(vp)],
-        "dr_nvls_add_device": [P],
-        "dr_nvls_bind": [P, C.POINTER(vp), C.POINTER(vp)],
-        "dr_nvls_allreduce_apply": [P, P, P, P, i64, P, P, P, P],
-        "dr_nvls_allreduce_2phase": [P, P, INT, INT, P, P, P, i64, P, P, P],
-    }
-    for name, args in sigs.items():
-        fn = getattr(lib, name)
-        fn.argtypes, fn.restype = args, INT
-    lib.dr_nvls_size.argtypes, lib.dr_nvls_size.restype = [i64, INT], i64
-    _bind_sp(lib)
-    lib._comm_bound = True
-
-
-def _chk(rc, what):
-    if rc != 0:
-        raise RuntimeError(f"deeprec_cuda comm: {what} failed with code {rc}")
 
 
 class SymmetricBuffer:
@@ -73,10 +42,10 @@ class SymmetricBuffer:
         nbytes = max(256, int(nbytes))
         self.comm, self.nbytes = comm, nbytes
         local = vp()
-        _chk(lib.dr_comm_alloc(nbytes, C.byref(local)), "alloc")
+        check(lib.dr_comm_alloc(nbytes, C.byref(local)), "alloc")
         self.local = local.value
         handle = (C.c_char * 64)()
-        _chk(lib.dr_comm_get_handle(vp(self.local), handle), "ipc_get_handle")
+        check(lib.dr_comm_get_handle(vp(self.local), handle), "ipc_get_handle")
         handles: List[bytes] = [None] * comm.world
         dist.all_gather_object(handles, bytes(handle.raw), group=comm.group)
         self.peers = Peers()
@@ -87,7 +56,7 @@ class SymmetricBuffer:
             else:
                 p = vp()
                 buf = C.create_string_buffer(handles[r], 64)
-                _chk(lib.dr_comm_open_handle(buf, C.byref(p)), f"ipc_open_handle(rank {r})")
+                check(lib.dr_comm_open_handle(buf, C.byref(p)), f"ipc_open_handle(rank {r})")
                 self.peers.ptr[r] = p.value
                 self._opened.append(p.value)
         self._raw = torch.as_tensor(_RawCuda(self.local, nbytes), device=comm.dev)
@@ -111,8 +80,7 @@ class P2PComm:
     def __init__(self, rank: int, world: int, dev: torch.device, group=None):
         self.rank, self.world, self.dev, self.group = rank, world, dev, group
         self.lib = _native.cuda()
-        _bind(self.lib)
-        _chk(self.lib.dr_cuda_set_device(dev.index), "set_device")
+        check(self.lib.dr_cuda_set_device(dev.index), "set_device")
         for r in range(world):
             if r != rank and not self.lib.dr_comm_can_access_peer(dev.index, r):
                 raise RuntimeError(f"GPU {dev.index} cannot access peer {r}: NVLink P2P is required")
@@ -121,9 +89,6 @@ class P2PComm:
         self._buffers: List[SymmetricBuffer] = [self.signals]
         self.launches = 0            # kernels of the step's all-reduce / rendezvous calls (the pipeline counts its own DENSE signal)
         dist.barrier(group=group)
-
-    def _s(self):
-        return vp(torch.cuda.current_stream(self.dev).cuda_stream)
 
     def symmetric(self, nbytes: int) -> SymmetricBuffer:
         b = SymmetricBuffer(self, nbytes)
@@ -207,7 +172,7 @@ class P2PComm:
 
     def barrier(self, channel: int) -> None:
         """Stand-alone device-side rank barrier (tests / utilities; the training step does not use it)."""
-        _chk(self.lib.dr_comm_barrier(self.signals.peers_ref(), ptr(self.epochs), channel, self.rank, self.world, self._s()), "barrier")
+        check(self.lib.dr_comm_barrier(self.signals.peers_ref(), ptr(self.epochs), channel, self.rank, self.world, stream_ptr(self.dev)), "barrier")
 
     def dense_allreduce_update(self, eng) -> None:
         """DENSE flag + one-shot all-reduce fused with the optimizer (the kernel polls the flags itself)."""
@@ -215,29 +180,29 @@ class P2PComm:
         sp.signal(CH_DENSE)
         if getattr(self, "nvls", None) is not None and eng.P * 4 >= self.NVLS_2PHASE_BYTES:
             # large dense nets: reduce-scatter (multimem.ld_reduce) + in-switch broadcast (multimem.st), then the optimizer from local memory
-            _chk(self.lib.dr_nvls_allreduce_2phase(vp(self.nvls["mc"]), vp(self.nvls["local"]), self.rank, self.world, ptr(eng.params),
-                                                   ptr(eng.s0) if eng.s0 is not None else None, ptr(eng.s1) if eng.s1 is not None else None, eng.P,
-                                                   ptr(eng.hp_dev), sp.sync_ref(), self._s()), "nvls_allreduce_2phase")
+            check(self.lib.dr_nvls_allreduce_2phase(vp(self.nvls["mc"]), vp(self.nvls["local"]), self.rank, self.world, ptr(eng.params),
+                                                    ptr(eng.s0) if eng.s0 is not None else None, ptr(eng.s1) if eng.s1 is not None else None, eng.P,
+                                                    ptr(eng.hp_dev), sp.sync_ref(), stream_ptr(self.dev)), "nvls_allreduce_2phase")
             self.launches += 2
             return
         if getattr(self, "nvls", None) is not None:     # in-switch reduction: one multimem.ld_reduce per 16 B instead of W peer loads
-            _chk(self.lib.dr_nvls_allreduce_apply(vp(self.nvls["mc"]), ptr(eng.params), ptr(eng.s0) if eng.s0 is not None else None,
-                                                  ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), self._s()),
-                 "nvls_allreduce_apply")
+            check(self.lib.dr_nvls_allreduce_apply(vp(self.nvls["mc"]), ptr(eng.params), ptr(eng.s0) if eng.s0 is not None else None,
+                                                   ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), stream_ptr(self.dev)),
+                  "nvls_allreduce_apply")
             self.launches += 1
             return
-        _chk(self.lib.dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, ptr(eng.params), ptr(eng.s0) if eng.s0 is not None else None,
-                                                   ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), self._s()),
-             "allreduce_apply")
+        check(self.lib.dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, ptr(eng.params), ptr(eng.s0) if eng.s0 is not None else None,
+                                                    ptr(eng.s1) if eng.s1 is not None else None, eng.P, ptr(eng.hp_dev), None, sp.sync_ref(), stream_ptr(self.dev)),
+              "allreduce_apply")
         self.launches += 1
 
     def wait_dense(self, sp) -> None:
         """In-kernel rendezvous on the DENSE flags without any reduction (forward-only passes)."""
         if getattr(self, "nvls", None) is not None:
-            _chk(self.lib.dr_nvls_allreduce_apply(vp(self.nvls["mc"]), None, None, None, 0, None, None, sp.sync_ref(), self._s()), "wait_dense")
+            check(self.lib.dr_nvls_allreduce_apply(vp(self.nvls["mc"]), None, None, None, 0, None, None, sp.sync_ref(), stream_ptr(self.dev)), "wait_dense")
         else:
-            _chk(self.lib.dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, None, None, None, 0, None, None, sp.sync_ref(), self._s()),
-                 "wait_dense")
+            check(self.lib.dr_comm_allreduce_apply_sync(self.grads_buf.peers_ref(), self.world, None, None, None, 0, None, None, sp.sync_ref(), stream_ptr(self.dev)),
+                  "wait_dense")
         self.launches += 1
 
     def allreduce(self, out: torch.Tensor, two_phase: bool = False) -> None:
@@ -245,12 +210,12 @@ class P2PComm:
         gradient buffer itself holds the sum afterwards."""
         self.barrier(3)
         if getattr(self, "nvls", None) is not None and two_phase:
-            _chk(self.lib.dr_nvls_allreduce_2phase(vp(self.nvls["mc"]), vp(self.nvls["local"]), self.rank, self.world, None, None, None, out.numel(), None,
-                                                   None, self._s()), "nvls_allreduce_2phase")
+            check(self.lib.dr_nvls_allreduce_2phase(vp(self.nvls["mc"]), vp(self.nvls["local"]), self.rank, self.world, None, None, None, out.numel(), None,
+                                                    None, stream_ptr(self.dev)), "nvls_allreduce_2phase")
             self.barrier(5)                         # every slice owner has broadcast its slice: my local buffer now holds the full sum
             out.copy_(self.nvls["tensor"][: out.numel()])
         elif getattr(self, "nvls", None) is not None:
-            _chk(self.lib.dr_nvls_allreduce_apply(vp(self.nvls["mc"]), None, None, None, out.numel(), None, ptr(out), None, self._s()), "nvls_allreduce")
+            check(self.lib.dr_nvls_allreduce_apply(vp(self.nvls["mc"]), None, None, None, out.numel(), None, ptr(out), None, stream_ptr(self.dev)), "nvls_allreduce")
         else:
-            _chk(self.lib.dr_comm_allreduce_apply(self.grads_buf.peers_ref(), self.world, None, None, None, out.numel(), None, ptr(out), self._s()), "allreduce")
+            check(self.lib.dr_comm_allreduce_apply(self.grads_buf.peers_ref(), self.world, None, None, None, out.numel(), None, ptr(out), stream_ptr(self.dev)), "allreduce")
         self.barrier(4)        # nobody overwrites its contribution before every rank has read it

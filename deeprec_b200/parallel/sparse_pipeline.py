@@ -16,34 +16,14 @@ from typing import List, Optional, Sequence
 import torch
 
 from .. import _native
-from .._native import ptr
+from .._cuda_sigs import Peers, SpBags, SpGeom, SpSync
+from .._native import check, ptr, stream_ptr
 
-vp, i32, i64 = C.c_void_p, C.c_int32, C.c_int64
+vp = C.c_void_p
 CH_DEDUP, CH_ROWS, CH_GRAD, CH_DENSE = 0, 1, 2, 3
 
 
 MAX_TABLES = 256          # kSpMaxTables in csrc/cuda/sparse_pipeline.cu
-
-
-class Peers(C.Structure):
-    """Mirror of DrPeers (csrc/cuda/sp_sync.cuh)."""
-    _fields_ = [("ptr", vp * 16)]
-
-
-class SpSync(C.Structure):
-    """Mirror of DrSpSync."""
-    _fields_ = [("flags", Peers), ("state", vp), ("rank", i32), ("W", i32)]
-
-
-class SpGeom(C.Structure):
-    """Mirror of DrSpGeom."""
-    _fields_ = [("col_table", vp), ("hoff", vp), ("boff", vp), ("C", i32), ("T", i32), ("W", i32), ("rank", i32), ("B", i64),
-                ("dim", i32), ("ldinv", i32), ("pad_key", i64)]
-
-
-class SpBags(C.Structure):
-    """Mirror of DrSpBags."""
-    _fields_ = [("off", vp), ("comb", vp), ("col_bag", vp), ("F", i32)]
 
 
 COMBINERS = {"sum": 0, "mean": 1, "sqrtn": 2}
@@ -86,45 +66,6 @@ def _next_pow2(n: int) -> int:
     return p
 
 
-def _chk(rc, what):
-    if rc != 0:
-        raise RuntimeError(f"deeprec_cuda sparse pipeline: {what} failed with code {rc}")
-
-
-def bind(lib):
-    if getattr(lib, "_sp_bound", False):
-        return lib
-    INT, P = C.c_int, vp
-    GP, SP, PP, BP = C.POINTER(SpGeom), C.POINTER(SpSync), C.POINTER(Peers), C.POINTER(SpBags)
-    sigs = {
-        "dr_sp_init_scratch": [P, i64, P],
-        "dr_sp_dedup": [P, GP, P, P, P, P, P, P, P, SP, P],
-        "dr_sp_segsum": [P, P, GP, P, SP, P],
-        "dr_sp_gather": [P, P, GP, P, SP, P],
-        "dr_sp_pool": [P, P, GP, BP, P, P, SP, P],
-        "dr_sp_pool_segsum": [P, P, P, GP, BP, P, SP, P],
-        "dr_sp_linear_fwd": [P, P, GP, P, SP, P],
-        "dr_sp_linear_bwd": [P, P, GP, P, SP, P],
-        "dr_sp_lookup": [P, P, GP, i64, PP, PP, PP, PP, PP, INT, P, P, P, P, P, i64, SP, P],
-        "dr_sp_grad": [P, P, GP, i64, PP, P, P, P, P, SP, P],
-        "dr_sp_reset": [GP, i64, P, P, P, P, P],
-        "dr_sp_signal": [SP, INT, P],
-        "dr_sp_step_end": [P, P],
-        "dr_sp_stats": [GP, P, P, P],
-        "dr_cuda_dot_interaction_fwd_u": [P, i64, P, P, INT, INT, INT, i64, P, i64, SP, P],
-        "dr_cuda_dot_interaction_bwd_u": [P, i64, P, i64, P, P, INT, INT, INT, i64, P, i64, P, i64, i64, P],
-        "dr_cuda_dlrm_inter_gemm": [P, i64, P, P, INT, INT, INT, i64, P, i64, INT, P, P, i64, P, i64, SP, P],
-        "dr_comm_allreduce_apply_sync": [PP, INT, P, P, P, i64, P, P, SP, P],
-    }
-    for name, args in sigs.items():
-        if not hasattr(lib, name) and _native.emu_active():
-            continue                             # wgmma translation units are not part of the emulation build
-        fn = getattr(lib, name)
-        fn.argtypes, fn.restype = args, INT
-    lib._sp_bound = True
-    return lib
-
-
 class _LocalBuffer:
     """world == 1 stand-in for parallel.p2p.SymmetricBuffer: a plain device allocation that is its own (only) peer."""
 
@@ -151,7 +92,7 @@ class SparsePipeline:
     def __init__(self, dev: torch.device, rank: int, world: int, col_table: Sequence[int], num_tables: int, batch: int, dim: int, comm=None,
                  pad_key: int = -1, with_grad: bool = True):
         self.dev, self.rank, self.W, self.comm = dev, rank, world, comm
-        self.lib = bind(_native.cuda())
+        self.lib = _native.cuda()
         self.C, self.T, self.B, self.dim = len(col_table), num_tables, batch, dim
         self.ldinv = (self.C + 3) // 4 * 4
         if world > 1 and comm is None:
@@ -209,7 +150,7 @@ class SparsePipeline:
         s = SpSync()
         s.flags, s.state, s.rank, s.W = self.flags_buf.peers, self.state.data_ptr(), rank, world
         self.sync = s
-        _chk(self.lib.dr_sp_init_scratch(vp(self.scr_buf.local), self.Htot, self._s()), "init_scratch")
+        check(self.lib.dr_sp_init_scratch(vp(self.scr_buf.local), self.Htot, stream_ptr(self.dev)), "init_scratch")
         if not _native.emu_active():
             torch.cuda.synchronize(dev)
         if world > 1:
@@ -217,11 +158,6 @@ class SparsePipeline:
         self.launches = 0
 
     # ------------------------------------------------------------------------------------------------------------------
-    def _s(self):
-        if _native.emu_active():
-            return None
-        return vp(torch.cuda.current_stream(self.dev).cuda_stream)
-
     def sync_ref(self):
         return C.byref(self.sync)
 
@@ -231,29 +167,29 @@ class SparsePipeline:
     def dedup(self, ids: torch.Tensor) -> None:
         """ids: int64 [C, B] (column-major id columns of the local batch)."""
         assert ids.shape == (self.C, self.B) and ids.dtype == torch.int64
-        _chk(self.lib.dr_sp_dedup(ptr(ids), self.geom_ref(), vp(self.scr_buf.local), ptr(self.inv), ptr(self.invT), vp(self.bkt_key_buf.local), vp(self.bkt_gs_buf.local),
-                                  vp(self.bcnt_buf.local), ptr(self.ugrad) if self.ugrad is not None else None, self.sync_ref(), self._s()), "dedup")
+        check(self.lib.dr_sp_dedup(ptr(ids), self.geom_ref(), vp(self.scr_buf.local), ptr(self.inv), ptr(self.invT), vp(self.bkt_key_buf.local), vp(self.bkt_gs_buf.local),
+                                   vp(self.bcnt_buf.local), ptr(self.ugrad) if self.ugrad is not None else None, self.sync_ref(), stream_ptr(self.dev)), "dedup")
         self.launches += 1
 
     def lookup(self, ctx, table_map: torch.Tensor, train: bool) -> None:
         """Owner side: probe / insert the keys every source bucketed for this rank and push their rows into the sources' urow."""
-        _chk(self.lib.dr_sp_lookup(ptr(ctx.structs()), ptr(table_map), self.geom_ref(), self.max_bcap, self.bkt_key_buf.peers_ref(),
-                                   self.bkt_gs_buf.peers_ref(), self.bcnt_buf.peers_ref(), self.scr_buf.peers_ref(), self.urow_buf.peers_ref(),
-                                   int(train), ptr(self.own_pos), ptr(self.own_gs), ptr(self.own_cnt),
-                                   ptr(ctx.ulist) if train else None, ptr(ctx.nuniq) if train else None,
-                                   ctx.ulist.numel() if train else 0, self.sync_ref(), self._s()), "lookup")
+        check(self.lib.dr_sp_lookup(ptr(ctx.structs()), ptr(table_map), self.geom_ref(), self.max_bcap, self.bkt_key_buf.peers_ref(),
+                                    self.bkt_gs_buf.peers_ref(), self.bcnt_buf.peers_ref(), self.scr_buf.peers_ref(), self.urow_buf.peers_ref(),
+                                    int(train), ptr(self.own_pos), ptr(self.own_gs), ptr(self.own_cnt),
+                                    ptr(ctx.ulist) if train else None, ptr(ctx.nuniq) if train else None,
+                                    ctx.ulist.numel() if train else 0, self.sync_ref(), stream_ptr(self.dev)), "lookup")
         self.launches += 1
 
     def gather(self, out: torch.Tensor) -> None:
         """Requester side: out[b, c, :] = urow[inv[b, c]] (bf16 [B, C, dim]); the kernel waits for every owner's ROWS flag."""
         assert out.shape == (self.B, self.C, self.dim) and out.dtype == torch.bfloat16 and out.is_contiguous()
-        _chk(self.lib.dr_sp_gather(ptr(self.urow), ptr(self.inv), self.geom_ref(), ptr(out), self.sync_ref(), self._s()), "gather")
+        check(self.lib.dr_sp_gather(ptr(self.urow), ptr(self.inv), self.geom_ref(), ptr(out), self.sync_ref(), stream_ptr(self.dev)), "gather")
         self.launches += 1
 
     def segsum(self, demb: torch.Tensor) -> None:
         """Requester side: pre-reduce the per-sample gradient rows (bf16 [C, B, dim]) per distinct key into ugrad; raises GRAD."""
         assert demb.shape == (self.C, self.B, self.dim) and demb.dtype == torch.bfloat16
-        _chk(self.lib.dr_sp_segsum(ptr(demb), ptr(self.invT), self.geom_ref(), ptr(self.ugrad), self.sync_ref(), self._s()), "segsum")
+        check(self.lib.dr_sp_segsum(ptr(demb), ptr(self.invT), self.geom_ref(), ptr(self.ugrad), self.sync_ref(), stream_ptr(self.dev)), "segsum")
         self.launches += 1
 
     def pool(self, out: torch.Tensor, w: torch.Tensor, bags: Bags) -> None:
@@ -262,7 +198,7 @@ class SparsePipeline:
         assert out.shape == (self.B, bags.F, self.dim) and out.dtype == torch.bfloat16 and out.is_contiguous()
         assert w.shape == (bags.F, self.B) and w.dtype == torch.float32 and w.is_contiguous()
         assert bags.col_bag.numel() == self.C
-        _chk(self.lib.dr_sp_pool(ptr(self.urow), ptr(self.inv), self.geom_ref(), bags.ref(), ptr(out), ptr(w), self.sync_ref(), self._s()), "pool")
+        check(self.lib.dr_sp_pool(ptr(self.urow), ptr(self.inv), self.geom_ref(), bags.ref(), ptr(out), ptr(w), self.sync_ref(), stream_ptr(self.dev)), "pool")
         self.launches += 1
 
     def pool_segsum(self, dpool: torch.Tensor, w: torch.Tensor, bags: Bags) -> None:
@@ -271,15 +207,15 @@ class SparsePipeline:
         assert dpool.shape == (bags.F, self.B, self.dim) and dpool.dtype == torch.bfloat16 and dpool.is_contiguous()
         assert w.shape == (bags.F, self.B) and w.dtype == torch.float32 and w.is_contiguous()
         assert bags.col_bag.numel() == self.C and self.ugrad is not None
-        _chk(self.lib.dr_sp_pool_segsum(ptr(dpool), ptr(w), ptr(self.invT), self.geom_ref(), bags.ref(), ptr(self.ugrad), self.sync_ref(), self._s()),
-             "pool_segsum")
+        check(self.lib.dr_sp_pool_segsum(ptr(dpool), ptr(w), ptr(self.invT), self.geom_ref(), bags.ref(), ptr(self.ugrad), self.sync_ref(), stream_ptr(self.dev)),
+              "pool_segsum")
         self.launches += 1
 
     def linear_fwd(self, out: torch.Tensor) -> None:
         """Requester side: out[b] = sum over the id columns c of float(urow[inv[b, c], 0]) (fp32 [B], summed in column order); padding adds
         nothing.  The linear (wide) logit read in place from the unique rows; the kernel waits for every owner's ROWS flag."""
         assert out.shape == (self.B,) and out.dtype == torch.float32 and out.is_contiguous()
-        _chk(self.lib.dr_sp_linear_fwd(ptr(self.urow), ptr(self.inv), self.geom_ref(), ptr(out), self.sync_ref(), self._s()), "linear_fwd")
+        check(self.lib.dr_sp_linear_fwd(ptr(self.urow), ptr(self.inv), self.geom_ref(), ptr(out), self.sync_ref(), stream_ptr(self.dev)), "linear_fwd")
         self.launches += 1
 
     def linear_bwd(self, dlogit: torch.Tensor) -> None:
@@ -287,7 +223,7 @@ class SparsePipeline:
         64-bit fixed-point sums, elements 1.. stay zero); raises GRAD.  Takes the place of segsum for a linear group."""
         assert dlogit.shape == (self.B,) and dlogit.dtype == torch.float32 and dlogit.is_contiguous()
         assert self.ugrad is not None, "linear_bwd needs a pipeline built with with_grad=True"
-        _chk(self.lib.dr_sp_linear_bwd(ptr(dlogit), ptr(self.invT), self.geom_ref(), ptr(self.ugrad), self.sync_ref(), self._s()), "linear_bwd")
+        check(self.lib.dr_sp_linear_bwd(ptr(dlogit), ptr(self.invT), self.geom_ref(), ptr(self.ugrad), self.sync_ref(), stream_ptr(self.dev)), "linear_bwd")
         self.launches += 1
 
     def ugrad_rows(self) -> torch.Tensor:
@@ -296,24 +232,24 @@ class SparsePipeline:
 
     def grad(self, ctx, table_map: torch.Tensor) -> None:
         """Owner side: pull the sources' pre-reduced gradient rows into gsum[unique] (k_apply follows)."""
-        _chk(self.lib.dr_sp_grad(ptr(ctx.structs()), ptr(table_map), self.geom_ref(), self.max_bcap, self.ugrad_buf.peers_ref(), ptr(self.own_pos),
-                                 ptr(self.own_gs), ptr(self.own_cnt), ptr(ctx.gsum), self.sync_ref(), self._s()), "grad")
+        check(self.lib.dr_sp_grad(ptr(ctx.structs()), ptr(table_map), self.geom_ref(), self.max_bcap, self.ugrad_buf.peers_ref(), ptr(self.own_pos),
+                                  ptr(self.own_gs), ptr(self.own_cnt), ptr(ctx.gsum), self.sync_ref(), stream_ptr(self.dev)), "grad")
         self.launches += 1
 
     def reset(self) -> None:
-        _chk(self.lib.dr_sp_reset(self.geom_ref(), self.max_bcap, vp(self.scr_buf.local), vp(self.bkt_gs_buf.local), vp(self.bcnt_buf.local),
-                                  ptr(self.state), self._s()), "reset")
+        check(self.lib.dr_sp_reset(self.geom_ref(), self.max_bcap, vp(self.scr_buf.local), vp(self.bkt_gs_buf.local), vp(self.bcnt_buf.local),
+                                   ptr(self.state), stream_ptr(self.dev)), "reset")
         self.launches += 1
 
     def signal(self, channel: int) -> None:
-        _chk(self.lib.dr_sp_signal(self.sync_ref(), channel, self._s()), "signal")
+        check(self.lib.dr_sp_signal(self.sync_ref(), channel, stream_ptr(self.dev)), "signal")
         self.launches += 1
 
     def step_end(self) -> None:
-        _chk(self.lib.dr_sp_step_end(ptr(self.state), self._s()), "step_end")
+        check(self.lib.dr_sp_step_end(ptr(self.state), stream_ptr(self.dev)), "step_end")
         self.launches += 1
 
     def unique_count(self) -> int:
         """Distinct (table, key) pairs of the batch last deduplicated (valid between dedup() and reset(); host sync)."""
-        _chk(self.lib.dr_sp_stats(self.geom_ref(), vp(self.bcnt_buf.local), ptr(self._stats), self._s()), "stats")
+        check(self.lib.dr_sp_stats(self.geom_ref(), vp(self.bcnt_buf.local), ptr(self._stats), stream_ptr(self.dev)), "stats")
         return int(self._stats[0].item())
