@@ -105,6 +105,7 @@ _sig("dr_cuda_bn_apply", [P, i64, INT, i64, P, P, P, i64, S])
 _sig("dr_cuda_bn_bwd_finalize", [P, P, INT, i64, P, P, P, P, P, P, f32, S])
 _sig("dr_cuda_bn_bwd_apply", [P, P, i64, INT, i64, P, P, P, P, P, P, INT, S])
 _sig("dr_cuda_head", [P, i64, i64, INT, P, P, P, f32, P, P, P, P, P, INT, INT, P, S])
+_sig("dr_cuda_det_colsum", [P, INT, i64, INT, P, P, S])
 _sig("dr_cuda_pack_weights", [P, INT, INT, P, P, INT, S])
 _sig("dr_cuda_cast_pad", [P, i64, INT, P, INT, S])
 _sig("dr_cuda_l2_flush", [P, i64, f32, S])

@@ -274,18 +274,66 @@ inline float* dr_workspace(int slot, size_t nfloat, cudaStream_t s) {
 }
 enum { kWsGemmStats = 0, kWsGemmDw = 1, kWsColstats = 2, kWsHead = 3, kWsBnBwd = 4 };
 
-// dst0[c] += scale * sum_r ws[r * ld + c],  dst1[c] += scale * sum_r ws[r * ld + n + c]   (c < n, rows summed in order; dst1 may be null)
-static __global__ void k_det_colsum(const float* __restrict__ ws, int rows, int64_t ld, int n, float* __restrict__ dst0, float* __restrict__ dst1,
-                                    float scale) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= n) return;
-  float s0 = 0.f, s1 = 0.f;
-  for (int r = 0; r < rows; ++r) {
-    s0 += ws[(int64_t)r * ld + c];
-    if (dst1) s1 += ws[(int64_t)r * ld + n + c];
+// k_det_colsum: for every column c of a range, dst[c] += s with s = ((0.f + ws[0][c]) + ws[1][c]) + ... + ws[rows-1][c], one fp32 add after
+// the other in row order, so the result does not depend on this kernel's grid.  What makes it fast is memory parallelism alone: a block owns
+// 8 columns of one range (one 32-byte sector of a row), its 256 threads, 32 row groups of 8, stage kDetColsumChunk rows of them at a time
+// through shared memory (16 loads in flight per thread, the next chunk's loads issued before the current chunk is added), and the 8 threads
+// of row group 0 run the columns' add chains out of shared memory.  Narrow blocks keep a block's rows few and its loads many per chunk.
+constexpr int kDetColsumCols = 8, kDetColsumThreads = 256, kDetColsumPer = 16, kDetColsumMaxRanges = 4;
+constexpr int kDetColsumGroups = kDetColsumThreads / kDetColsumCols;   // row groups
+constexpr int kDetColsumChunk = kDetColsumGroups * kDetColsumPer;      // rows staged per chunk
+struct DetColsumRange { int64_t col; int n; float* dst; };            // workspace columns [col, col + n) are added into dst[0, n)
+struct DetColsumRanges { DetColsumRange r[kDetColsumMaxRanges]; int count; };
+
+__device__ __forceinline__ void det_colsum_stage(float (&v)[kDetColsumPer], const float* __restrict__ src, int64_t ld, int row0, int rows, bool live) {
+#pragma unroll
+  for (int j = 0; j < kDetColsumPer; ++j) {
+    const int row = row0 + j * kDetColsumGroups;
+    v[j] = (live && row < rows) ? src[(int64_t)row * ld] : 0.f;
   }
-  dst0[c] += scale * s0;
-  if (dst1) dst1[c] += scale * s1;
+}
+
+static __global__ void __launch_bounds__(kDetColsumThreads) k_det_colsum(const float* __restrict__ ws, int rows, int64_t ld, DetColsumRanges rs) {
+  int blk = blockIdx.x;
+  DetColsumRange rg = rs.r[0];
+#pragma unroll
+  for (int i = 1; i < kDetColsumMaxRanges; ++i) {     // constant indices: the ranges are read from the parameter bank, not copied to local memory
+    const int nb = (rg.n + kDetColsumCols - 1) / kDetColsumCols;
+    if (i < rs.count && blk >= nb) { blk -= nb; rg = rs.r[i]; }
+  }
+  const int lane = threadIdx.x % kDetColsumCols, grp = threadIdx.x / kDetColsumCols;
+  const int c = blk * kDetColsumCols + lane;
+  const bool live = c < rg.n;
+  const float* src = ws + rg.col + c;
+  __shared__ float tile[2][kDetColsumChunk][kDetColsumCols];
+  float v[kDetColsumPer];
+  det_colsum_stage(v, src, ld, grp, rows, live);
+  float acc = 0.f;
+  // one barrier per chunk: chunk k + 2 overwrites buffer k & 1 only after every thread passed chunk k + 1's barrier, which row group 0
+  // reaches after it has added chunk k
+  for (int r0 = 0, buf = 0; r0 < rows; r0 += kDetColsumChunk, buf ^= 1) {
+#pragma unroll
+    for (int j = 0; j < kDetColsumPer; ++j) tile[buf][grp + j * kDetColsumGroups][lane] = v[j];
+    __syncthreads();
+    if (r0 + kDetColsumChunk < rows) det_colsum_stage(v, src, ld, r0 + kDetColsumChunk + grp, rows, live);
+    if (grp == 0) {
+      const int nr = min(kDetColsumChunk, rows - r0);
+#pragma unroll 16
+      for (int k = 0; k < nr; ++k) acc += tile[buf][k][lane];
+    }
+  }
+  if (grp == 0 && live) rg.dst[c] += acc;
+}
+
+// One k_det_colsum launch over up to kDetColsumMaxRanges column ranges of the workspace ws [rows][ld]; ranges with a null dst are skipped.
+template <int N>
+inline void det_colsum(const float* ws, int rows, int64_t ld, const DetColsumRange (&ranges)[N], cudaStream_t s) {
+  static_assert(N <= kDetColsumMaxRanges, "more column ranges than one k_det_colsum launch takes");
+  DetColsumRanges rs{};
+  int blocks = 0;
+  for (const DetColsumRange& r : ranges)
+    if (r.dst && r.n > 0) { rs.r[rs.count++] = r; blocks += (r.n + kDetColsumCols - 1) / kDetColsumCols; }
+  if (blocks) k_det_colsum<<<blocks, kDetColsumThreads, 0, s>>>(ws, rows, ld, rs);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {

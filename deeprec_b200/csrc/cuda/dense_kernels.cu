@@ -403,7 +403,7 @@ int dr_cuda_colstats(const void* u, const void* v, int64_t B, int N, int64_t ldu
   DR_PDL_LAUNCH((k_colstats), grid, 256, rows_par * 2 * N * sizeof(float), s, (const __nv_bfloat16*)u, (const __nv_bfloat16*)v, B, N, ldu, ldv, part,
                 S2 ? 1 : 0);
   DR_LAUNCH_CHECK();
-  k_det_colsum<<<(N + 127) / 128, 128, 0, s>>>(part, grid, 2 * (int64_t)N, N, S1, S2, 1.f);
+  det_colsum(part, grid, 2 * (int64_t)N, {{0, N, S1}, {N, N, S2}}, s);
   DR_LAUNCH_CHECK();
   return 0;
 }
@@ -468,7 +468,7 @@ int dr_cuda_bn_bwd_apply_v2(const void* dy, const void* a, int64_t B, int N, int
                 c1, c2, (__nv_bfloat16*)da, relu_mask, part);
   DR_LAUNCH_CHECK();
   if (dbias) {
-    k_det_colsum<<<(N + 127) / 128, 128, 0, s>>>(part, grid, (int64_t)N, N, dbias, nullptr, 1.f);
+    det_colsum(part, grid, (int64_t)N, {{0, N, dbias}}, s);
     DR_LAUNCH_CHECK();
   }
   return 0;
@@ -491,12 +491,18 @@ int dr_cuda_head(const void* h, int64_t ldh, int64_t B, int K, const float* w, c
   if (K == 256) HEAD(1); else if (K == 512) HEAD(2); else HEAD(4);
 #undef HEAD
   DR_LAUNCH_CHECK();
-  const int64_t L = 2 * (int64_t)K + 2;
-  if (train) {
-    k_det_colsum<<<(K + 127) / 128, 128, 0, s>>>(part, grid, L, K, dw, nullptr, 1.f);
-    if (dbias_h) k_det_colsum<<<(K + 127) / 128, 128, 0, s>>>(part + K, grid, L, K, dbias_h, nullptr, 1.f);
-  }
-  k_det_colsum<<<1, 1, 0, s>>>(part + 2 * K, grid, L, 1, loss_sum, train ? db : nullptr, 1.f);
+  // the four sums of part [grid][2K + 2] (dw | dbias_h | loss | db) in one launch
+  det_colsum(part, grid, 2 * (int64_t)K + 2,
+             {{0, K, train ? dw : nullptr}, {K, K, train ? dbias_h : nullptr}, {2 * K, 1, loss_sum}, {2 * K + 1, 1, train ? db : nullptr}}, s);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// dst0[c] += sum_r ws[r * ld + c],  dst1[c] += sum_r ws[r * ld + n + c]   (c < n; dst1 may be null): the ordered reduction of block
+// partials that every batch sum above ends with (k_det_colsum, common.cuh), on its own
+int dr_cuda_det_colsum(const float* ws, int rows, int64_t ld, int n, float* dst0, float* dst1, cudaStream_t s) {
+  if (rows < 0 || n < 0) return -2;
+  det_colsum(ws, rows, ld, {{0, n, dst0}, {n, n, dst1}}, s);
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -579,7 +579,7 @@ int dr_cuda_gemm_tn_ex(const void* A, int64_t lda, const void* B, int64_t ldb, i
      : N <= 64 ? launch_tn_sel<64>(ta, B, M, N, K, ldb, ep, max_ctas, s)
                : launch_tn_sel<128>(ta, B, M, N, K, ldb, ep, max_ctas, s);
   if (rc || !S1) return rc;
-  k_det_colsum<<<(N + 127) / 128, 128, 0, s>>>(ws, m_tiles, 2 * (int64_t)N, N, S1, S2, 1.f);
+  det_colsum(ws, m_tiles, 2 * (int64_t)N, {{0, N, S1}, {N, N, S2}}, s);
   DR_LAUNCH_CHECK();
   return 0;
 }
