@@ -4,9 +4,14 @@
 //                  bf16 out (optional fp32 copy); the same kernel with FP8 = true multiplies E4M3 operands and applies a per-column
 //                  scale (serving MLP, dr_cuda_gemm_fp8_tn).
 //                  Persistent and warp-specialised: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers that
-//                  each own 64 rows of a 128-row tile, issue wgmma.mma_async straight from the 128B-swizzled K-major smem tiles and
-//                  run the fused epilogue from their accumulator registers.  A 4-stage smem ring of mbarrier-guarded stages keeps
-//                  the loads of the next tile in flight while the consumers finish the current one.
+//                  issue wgmma.mma_async straight from the 128B-swizzled K-major smem tiles and run the fused epilogue from their
+//                  accumulator registers.  A 4-stage smem ring of mbarrier-guarded stages keeps the loads of the next tile in flight
+//                  while the consumers finish the current one.
+//                  bf16 streaming at K < 512 (the default there): ping-pong consumers.  Each warpgroup owns whole 128-row tiles, alternate tiles of
+//                  the schedule, so one warpgroup's epilogue overlaps the other's MMAs; the aux tile arrives by TMA into the
+//                  warpgroup's output buffer and the bf16 tile leaves by TMA store.  FP8 / MX, BRES, CL2 and bf16 at K >= 512:
+//                  cooperative consumers,
+//                  each warpgroup owns 64 rows of every tile and stores straight from registers.
 //                  Variants: BRES (B-resident: a CTA keeps one [BLOCK_N, K] weight slab in smem for its whole life and streams only
 //                  A) and CL2 (thread-block cluster of 2 CTAs on vertically adjacent tiles: each CTA loads half of the B tile and
 //                  multicasts it to both, halving the B traffic from L2).
@@ -49,9 +54,10 @@ PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// 2-D tensor map: dims {inner, outer}, row pitch in bytes, box {box_inner, box_outer}, 128B swizzle; out-of-bounds elements read as 0.
+// 2-D tensor map: dims {inner, outer}, row pitch in bytes, box {box_inner, box_outer}, 128B swizzle unless given; out-of-bounds elements
+// read as 0 and are not written by stores.
 int make_tmap(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, uint64_t pitch_bytes, uint32_t box_inner, uint32_t box_outer,
-              CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
+              CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return -100;
   cuuint64_t dims[2] = {inner, outer};
@@ -59,7 +65,7 @@ int make_tmap(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, u
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : -101 - (int)r;
 }
 
@@ -88,16 +94,32 @@ __device__ __forceinline__ uint32_t mx_word(const uint32_t* sf, int r, int num_k
   return __ldg(sf + ((int64_t)(r >> 7) * num_kb + kb) * 128 + (r & 31) * 4 + ((r & 127) >> 5));
 }
 
-template <int BLOCK_N, bool BRES>
+// PP (ping-pong): each consumer warpgroup owns whole 128-row tiles and has its own output tile buffer (the aux tile lands there first)
+// and its own statistics rows.  The output tile is stored by TMA in boxes of kBoxCols columns x 128 rows, kRowBytes per box row, with
+// the tensor map's swizzle (128B / 64B / 32B for 64 / 32 / 16 columns): a warp's fragment accesses hit 32 different banks.
+template <int BLOCK_N, bool BRES, bool PP = false>
 struct SmemLayoutTN {
   static constexpr int kABytes = BLOCK_M * 128;
   static constexpr int kBBytes = BLOCK_N * 128;
   static constexpr int kSt = BRES ? 3 : kStages;
   static constexpr int kStageBytes = BRES ? kABytes : kABytes + kBBytes;
   static constexpr int kBResBytes = BRES ? kMaxKbRes * kBBytes : 0;
-  static constexpr int kStatBytes = 2 * 8 * BLOCK_N * 4;      // [S1 | S2][consumer warp][column]
-  static constexpr int kTotal = kBResBytes + kSt * kStageBytes + kStatBytes + 256 /*barriers*/ + 1024 /*align slack*/;
+  static constexpr int kBoxCols = BLOCK_N < 64 ? BLOCK_N : 64;
+  static constexpr int kRowBytes = kBoxCols * 2;
+  static constexpr int kBoxBytes = BLOCK_M * kRowBytes;
+  static constexpr int kOutBytes = PP ? BLOCK_M * BLOCK_N * 2 : 0;   // per consumer warpgroup
+  static constexpr int kStatBytes = (PP ? 2 : 1) * 2 * 8 * BLOCK_N * 4;   // [warpgroup][S1 | S2][16-row group][column]
+  static constexpr int kTotal = kBResBytes + kSt * kStageBytes + 2 * kOutBytes + kStatBytes + 256 /*barriers*/ + 1024 /*align slack*/;
 };
+
+// byte offset of (row, col) in a PP output tile buffer, in the layout the TMA swizzle gives it (16-byte chunk index ^ row bits)
+template <int BLOCK_N>
+__device__ __forceinline__ uint32_t out_tile_offset(int row, int col) {
+  using L = SmemLayoutTN<BLOCK_N, false, true>;
+  uint32_t off = (uint32_t)(row * L::kRowBytes + (col % L::kBoxCols) * 2);
+  off ^= ((off >> 7) & (L::kRowBytes / 16 - 1)) << 4;
+  return (uint32_t)(col / L::kBoxCols) * L::kBoxBytes + off;
+}
 
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
@@ -118,6 +140,15 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank
       ::"r"(smem_u32(bar)), "r"(rank) : "memory");
 }
 __device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// named barrier of one consumer warpgroup (PP: the two warpgroups never wait for each other)
+__device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
+// PP mainloop order: warpgroup wg waits on barrier 4 + wg until the other warpgroup has arrived there after its mainloop
+__device__ __forceinline__ void order_wait(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(4 + wg) : "memory"); }
+__device__ __forceinline__ void order_signal(int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(5 - wg) : "memory"); }
+// this thread's bulk stores have finished reading shared memory (their global writes may still be in flight)
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 __device__ __forceinline__ uint16_t pack_e4m3x2(float a, float b) {
   uint16_t r;
@@ -125,22 +156,26 @@ __device__ __forceinline__ uint16_t pack_e4m3x2(float a, float b) {
   return r;
 }
 
-template <int BLOCK_N, bool BRES, bool CL2, bool FP8, bool MX = false>
+template <int BLOCK_N, bool BRES, bool CL2, bool FP8, bool MX = false, bool PP = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K, Epilogue ep) {
-  using L = SmemLayoutTN<BLOCK_N, BRES>;
+k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+          const __grid_constant__ CUtensorMap tmAux, int M, int N, int K, Epilogue ep) {
+  static_assert(!PP || (!BRES && !CL2 && !FP8), "ping-pong consumers: bf16 streaming kernel only");
+  using L = SmemLayoutTN<BLOCK_N, BRES, PP>;
   constexpr int kSt = L::kSt;
   constexpr int kAcc = BLOCK_N / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem_al = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* bres_base = smem_al;                                  // [kMaxKbRes][BLOCK_N x 128 B] resident weight slab (BRES only)
   uint8_t* ring = smem_al + L::kBResBytes;
-  float* sS1 = reinterpret_cast<float*>(ring + kSt * L::kStageBytes);
+  uint8_t* out_tiles = ring + kSt * L::kStageBytes;              // PP: [warpgroup][kOutBytes]
+  float* sS1 = reinterpret_cast<float*>(out_tiles + 2 * L::kOutBytes);
   float* sS2 = sS1 + 8 * BLOCK_N;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sS2 + 8 * BLOCK_N);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sS1) + L::kStatBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kSt;
   uint64_t* bfull_bar = bars + 2 * kSt;
+  uint64_t* aux_bar = bars + 2 * kSt + 1;                        // PP: [warpgroup] aux tile landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = CL2 ? cluster_ctarank() : 0;
@@ -160,17 +195,22 @@ k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < kSt; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], CL2 ? 16 : 8); }
+    // a stage is released by every consumer warp that read it: the 8 of both warpgroups (x 2 CTAs for CL2), or the 4 of the one PP
+    // warpgroup that owns its tile
+    for (int i = 0; i < kSt; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], PP ? 4 : CL2 ? 16 : 8); }
     mbar_init(bfull_bar, 1);
+    mbar_init(&aux_bar[0], 1);
+    mbar_init(&aux_bar[1], 1);
     fence_mbar_init();
   }
   __syncthreads();
   if constexpr (CL2) cluster_sync_all();     // the peer's barriers are initialised before any multicast lands on them
   pdl_sync();      // everything above overlapped the previous kernel's tail; nothing before this touched global memory
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ================= TMA producer =================
-    if (lane == 0) {
+    if constexpr (PP) setmaxnreg_dec<40>();    // registers go to the consumers, which hold a whole 128-row accumulator tile each
+    if (warp == 0 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       if constexpr (BRES) {
         if (unit0 < num_units) {          // the whole [BLOCK_N, K] weight slab, once
@@ -197,7 +237,148 @@ k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         }
       }
     }
-  } else if (warp >= 4) {
+  } else if constexpr (PP) {
+    // ================= ping-pong consumers: warpgroup wg owns the whole tiles wg, wg + 2, ... of this CTA's schedule =================
+    // The producer fills the ring in schedule order, so while one warpgroup runs its epilogue the other's k-blocks are already landing
+    // and its MMAs run.  Tile i of the schedule holds ring slots i * num_kb ... (i + 1) * num_kb - 1 (slot s: stage s % kSt, phase
+    // (s / kSt) & 1).  The mainloops run in tile order (order_wait / order_signal): a parity wait on slot s is only sound once slot
+    // s - kSt has completed, and every slot before tile i has when the mainloop of tile i - 1 is done.  The epilogue stages the bf16
+    // tile in the warpgroup's smem buffer and stores it with TMA; with an aux operand the buffer first receives the aux tile (TMA,
+    // aux_bar[wg]), and every thread overwrites exactly the aux elements it read.
+    setmaxnreg_inc<232>();
+    const int wg = (warp >> 2) - 1, wl = warp & 3, t = threadIdx.x & 127;
+    uint8_t* obuf = out_tiles + wg * L::kOutBytes;
+    float* wS1 = sS1 + wg * 2 * 8 * BLOCK_N;
+    float* wS2 = wS1 + 8 * BLOCK_N;
+    const bool has_aux = ep.mask_src != nullptr;
+    const bool stats = ep.S1 != nullptr;
+    uint32_t aux_phase = 0;
+    for (int i = wg; unit0 + i * unit_step < num_units; i += 2) {
+      const int u = unit0 + i * unit_step;
+      const int m_blk = tile_m(u), n_blk = tile_n(u);
+      if (has_aux && t == 0) {
+        tma_store_wait_read();                          // the previous tile's store has left the buffer
+        mbar_expect_tx(&aux_bar[wg], L::kOutBytes);
+#pragma unroll
+        for (int b = 0; b < BLOCK_N / L::kBoxCols; ++b)
+          tma_load_2d(obuf + b * L::kBoxBytes, &tmAux, &aux_bar[wg], n_blk * BLOCK_N + b * L::kBoxCols, m_blk * BLOCK_M);
+      }
+      float acc[2][kAcc];                               // [64-row half][wgmma fragment]
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < kAcc; ++r) acc[h][r] = 0.f;
+      int prev = -1;
+      if (i > 0) order_wait(wg);                        // the mainloop of tile i - 1 (the other warpgroup's) is done
+      for (int kb = 0; kb < num_kb; ++kb) {
+        const int slot = i * num_kb + kb, stage = slot % kSt;
+        mbar_wait(&full_bar[stage], (uint32_t)(slot / kSt) & 1u);
+        const uint32_t sa = smem_u32(ring + stage * L::kStageBytes);
+        const uint64_t adesc0 = gmma_desc_sw128(sa, 16, 1024);
+        const uint64_t adesc1 = gmma_desc_sw128(sa + 64 * 128, 16, 1024);
+        const uint64_t bdesc = gmma_desc_sw128(sa + L::kABytes, 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_bf16<BLOCK_N, 0, 0>(acc[0], adesc0 + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1);
+          wgmma_bf16<BLOCK_N, 0, 0>(acc[1], adesc1 + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+      }
+      if (unit0 + (i + 1) * unit_step < num_units) order_signal(wg);   // only a tile that exists waits for this arrival
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc[0]);
+      wgmma_fence_acc(acc[1]);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      if (has_aux) {
+        mbar_wait(&aux_bar[wg], aux_phase);
+        aux_phase ^= 1;
+      } else {
+        if (t == 0) tma_store_wait_read();
+        wg_bar_sync(wg);
+      }
+      // ---- epilogue: the arithmetic and the statistics' summation order of the cooperative epilogue below, row group g = 4 half + wl
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int lrow0 = half * 64 + wl * 16 + (lane >> 2);
+        const int row0 = m_blk * BLOCK_M + lrow0;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int lcol = 8 * j + 2 * (lane & 3);
+          const int col = n_blk * BLOCK_N + lcol;
+          const bool col_ok = col < N;
+          float b0 = 0.f, b1 = 0.f;
+          if (col_ok && ep.bias) { b0 = __ldg(ep.bias + col); b1 = __ldg(ep.bias + col + 1); }
+          float p1[2] = {0.f, 0.f}, p2[2] = {0.f, 0.f};
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = row0 + 8 * h;
+            const bool ok = col_ok && row < M;
+            float v0 = acc[half][4 * j + 2 * h] + b0;
+            float v1 = acc[half][4 * j + 2 * h + 1] + b1;
+            if (ep.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            uint32_t* sp = reinterpret_cast<uint32_t*>(obuf + out_tile_offset<BLOCK_N>(lrow0 + 8 * h, lcol));
+            float w0 = 0.f, w1 = 0.f;
+            if (has_aux && ok) {
+              const float2 w = unpack_bf16x2(*sp);
+              w0 = w.x; w1 = w.y;
+              if (ep.aux_mode == 1) { if (!(w0 > 0.f)) v0 = 0.f; if (!(w1 > 0.f)) v1 = 0.f; }
+            }
+            *sp = pack_bf16x2(v0, v1);                  // rows >= M and columns >= N are clipped by the store's tensor map
+            if (ok) {
+              if (ep.out_f32) *reinterpret_cast<float2*>(ep.out_f32 + (int64_t)row * ep.ldc + col) = make_float2(v0, v1);
+              if (stats) {
+                p1[0] += v0; p1[1] += v1;
+                const float a0 = ep.aux_mode == 2 ? w0 : v0, a1 = ep.aux_mode == 2 ? w1 : v1;
+                p2[0] += v0 * a0; p2[1] += v1 * a1;
+              }
+            }
+          }
+          if (stats) {
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+#pragma unroll
+              for (int o = 4; o < 32; o <<= 1) {
+                p1[c] += __shfl_xor_sync(0xffffffffu, p1[c], o);
+                p2[c] += __shfl_xor_sync(0xffffffffu, p2[c], o);
+              }
+            }
+            if (lane < 4) {
+              float* r1 = wS1 + (4 * half + wl) * BLOCK_N + 8 * j + 2 * lane;
+              float* r2 = wS2 + (4 * half + wl) * BLOCK_N + 8 * j + 2 * lane;
+              r1[0] = p1[0]; r1[1] = p1[1]; r2[0] = p2[0]; r2[1] = p2[1];
+            }
+          }
+        }
+      }
+      fence_proxy_async();                              // the generic-proxy tile writes are visible to the TMA store
+      wg_bar_sync(wg);
+      if (t == 0) {
+#pragma unroll
+        for (int b = 0; b < BLOCK_N / L::kBoxCols; ++b)
+          tma_store_2d(&tmOut, obuf + b * L::kBoxBytes, n_blk * BLOCK_N + b * L::kBoxCols, m_blk * BLOCK_M);
+        tma_store_commit();
+      }
+      if (stats) {                                      // the tile's column sums, row groups added in row order -> workspace row m_blk
+        for (int c = t; c < BLOCK_N; c += 128) {
+          const int col = n_blk * BLOCK_N + c;
+          if (col < N) {
+            float a1 = 0.f, a2 = 0.f;
+#pragma unroll
+            for (int g = 0; g < 8; ++g) { a1 += wS1[g * BLOCK_N + c]; a2 += wS2[g * BLOCK_N + c]; }
+            ep.stat_ws[(int64_t)m_blk * 2 * N + col] = a1;
+            ep.stat_ws[(int64_t)m_blk * 2 * N + N + col] = a2;
+          }
+        }
+        wg_bar_sync(wg);
+      }
+    }
+    if (t == 0) tma_store_wait_all();                   // the output is in global memory before the CTA retires (PDL dependents read it)
+  } else {
     // ================= consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of every tile =================
     // (warps 1-3 of the producer warpgroup have no role: wgmma is issued by whole warpgroups only)
     const int wg = (warp >> 2) - 1;
@@ -459,16 +640,26 @@ __global__ void k_dw_reduce(const float* __restrict__ part, int splits, int Mo, 
   }
 }
 
-template <int BN, bool BRES, bool CL2, bool FP8, bool MX = false>
+template <int BN, bool BRES, bool CL2, bool FP8, bool MX = false, bool PP = false>
 int launch_tn(const CUtensorMap& ta, const void* B, int M, int N, int K, int64_t ldb, const Epilogue& ep, int max_ctas, cudaStream_t s) {
-  CUtensorMap tb;
+  CUtensorMap tb, tout = {}, taux = {};
   const uint32_t box_rows = CL2 ? BN / 2 : BN;
   int rc = FP8 ? make_tmap(&tb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, 128, box_rows, CU_TENSOR_MAP_DATA_TYPE_UINT8)
                : make_tmap(&tb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, BLOCK_K, box_rows);
   if (rc) return rc;
-  using L = SmemLayoutTN<BN, BRES>;
+  using L = SmemLayoutTN<BN, BRES, PP>;
   static_assert(L::kTotal <= 227 * 1024, "shared-memory budget");
-  auto kern = k_gemm_tn<BN, BRES, CL2, FP8, MX>;
+  if constexpr (PP) {       // output and aux tiles in the kernel's swizzled smem layout; dims {N, M}: stores never pass column N or row M
+    const CUtensorMapSwizzle sw = L::kRowBytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : L::kRowBytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                                                                        : CU_TENSOR_MAP_SWIZZLE_32B;
+    rc = make_tmap(&tout, ep.out, (uint64_t)N, (uint64_t)M, (uint64_t)ep.ldc * 2, L::kBoxCols, BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, sw);
+    if (rc) return rc;
+    if (ep.mask_src) {
+      rc = make_tmap(&taux, ep.mask_src, (uint64_t)N, (uint64_t)M, (uint64_t)ep.ld_mask * 2, L::kBoxCols, BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, sw);
+      if (rc) return rc;
+    }
+  }
+  auto kern = k_gemm_tn<BN, BRES, CL2, FP8, MX, PP>;
   static DrPerDeviceOnce attr_once; bool& attr_set = attr_once();
   if (!attr_set) {
     DR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
@@ -488,9 +679,9 @@ int launch_tn(const CUtensorMap& ta, const void* B, int M, int N, int K, int64_t
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    DR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ta, tb, M, N, K, ep));
+    DR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, ta, tb, tout, taux, M, N, K, ep));
   } else {
-    DR_PDL_LAUNCH(kern, grid, kGemmThreads, L::kTotal, s, ta, tb, M, N, K, ep);
+    DR_PDL_LAUNCH(kern, grid, kGemmThreads, L::kTotal, s, ta, tb, tout, taux, M, N, K, ep);
   }
   DR_LAUNCH_CHECK();
   return 0;
@@ -527,6 +718,11 @@ int launch_tn_sel(const CUtensorMap& ta, const void* B, int M, int N, int K, int
   if (BN >= 64 && gemm_2cta_enabled()) return launch_tn<BN, false, true, false>(ta, B, M, N, K, ldb, ep, max_ctas, s);
   if (gemm_bres_enabled() && (K + BLOCK_K - 1) / BLOCK_K <= kMaxKbRes && (N + BN - 1) / BN <= max_ctas)
     return launch_tn<BN, true, false, false>(ta, B, M, N, K, ldb, ep, max_ctas, s);
+  // the ping-pong kernel reads the aux tile by TMA, which needs a 16-byte aligned base and pitch; the contract does not ask that of
+  // mask_src / ld_mask, so any other aux operand runs the cooperative kernel (same results bit for bit).  At K >= 512 the mainloop
+  // outweighs the epilogue and the cooperative kernel was the faster one on an H100 (the three K = 512 calls of the DLRM step, 5-12 %)
+  const bool aux_tma = !ep.mask_src || ((((uintptr_t)ep.mask_src) & 15) == 0 && ep.ld_mask % 8 == 0 && ep.ld_mask >= N);
+  if (aux_tma && K < 512) return launch_tn<BN, false, false, false, false, true>(ta, B, M, N, K, ldb, ep, max_ctas, s);
   return launch_tn<BN, false, false, false>(ta, B, M, N, K, ldb, ep, max_ctas, s);
 }
 
