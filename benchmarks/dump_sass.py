@@ -14,6 +14,7 @@ WANT = {  # object file -> kernel-name substrings to dump in full
     "comm_kernels.cu.o": ["k_allreduce_apply", "k_rank_barrier"],
     "fused_interaction_gemm.cu.o": ["k_dlrm_inter_gemm"],
     "interaction_kernels.cu.o": ["k_dot_fwd_tcILb1", "k_dot_bwd_tcILb1"],
+    "mha_kernels.cu.o": ["k_mha_fwdILi8ELi64", "k_mha_bwdILi8ELi64"],
     "gemm_wgmma.cu.o": ["k_gemm_tnILi128ELb0ELb0ELb0ELb0", "k_gemm_tnILi128ELb0ELb1ELb0ELb0", "k_gemm_tnILi64ELb0ELb0ELb1ELb1",
                         "k_gemm_nt_splitkILi128"],
     "tier_kernels.cu.o": ["k_tier_miss_list", "k_tier_evict"],

@@ -30,8 +30,8 @@ from deeprec_b200.models.zoo import CRITEO_MODELS, build_model  # noqa: E402
 
 
 def engine_main(a):
-    """BASELINE configs #3 (DeepFM) and #4 (DIN, 1B-id behaviour table with admission) on the fused engine, 1-8 GPUs; DIEN on the same
-    id layout; DSSM and the multi-task models (ESMM, MMoE, DBMTL, PLE, SimpleMultiTask) over pooled history bags."""
+    """BASELINE configs #3 (DeepFM) and #4 (DIN, 1B-id behaviour table with admission) on the fused engine, 1-8 GPUs; DIEN and BST on the
+    same id layout; DSSM and the multi-task models (ESMM, MMoE, DBMTL, PLE, SimpleMultiTask) over pooled history bags."""
     import torch.distributed as dist
     from deeprec_b200.models.rec_engine import POOLED_SEQ_MODELS, criteo_engine, din_engine, din_ids, pooled_seq_engine, taobao_engine_batch
     world, rank, lr = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0")), int(os.environ.get("LOCAL_RANK", "0"))
@@ -67,9 +67,9 @@ def engine_main(a):
             ids, y, _ = taobao_engine_batch(b) if eng.labels.dim() == 2 else (din_ids(b), b["labels"], None)
             host.append((ids.pin_memory(), y.pin_memory(), None))
         extra = {"item_id_space": a.id_space, "bags": "sum"}
-    elif name not in ("din", "dien"):
+    elif name not in ("din", "dien", "bst"):
         raise SystemExit(f"--engine: no fused-engine adapter for {name}")
-    else:                                       # DIN, and DIEN with both GRUs on the fused recurrence kernels
+    else:                                       # DIN; DIEN with both GRUs on the fused recurrence kernels; BST with its encoder block on the fused attention kernels
         eng = din_engine(model, a.batch, 50, table_rows=(10_000_000, min(a.id_space, 200_000_000), 10_000), optimizer=a.optimizer,
                          filter_freq=a.filter_freq, steps_to_live=100000, device=dev, rank=rank, world_size=world, comm=comm,
                          tiered={1: {"cache_rows": a.tier_rows, "strategy": 0}} if a.tier_rows > 0 else None)      # table 1 = the 1B-id behaviour (item) table

@@ -109,7 +109,7 @@ _sig("dr_cuda_det_colsum", [P, INT, i64, INT, P, P, S])
 _sig("dr_cuda_pack_weights", [P, INT, INT, P, P, INT, S])
 _sig("dr_cuda_cast_pad", [P, i64, INT, P, INT, S])
 _sig("dr_cuda_l2_flush", [P, i64, f32, S])
-# interactions, GRU, DIN attention, fused element-wise ops
+# interactions, GRU, self-attention, DIN attention, fused element-wise ops
 _sig("dr_cuda_dot_interaction_fwd", [P, i64, P, i64, i64, INT, INT, i64, P, i64, S])
 _sig("dr_cuda_dot_interaction_bwd", [P, i64, P, i64, P, i64, i64, INT, INT, i64, P, i64, P, i64, i64, S])
 _sig("dr_cuda_dot_interaction_fwd_u", [P, i64, P, P, INT, INT, INT, i64, P, i64, SP, S])
@@ -119,6 +119,8 @@ _sig("dr_cuda_fm_fwd", [P, i64, i64, INT, INT, i64, P, i64, P, S])
 _sig("dr_cuda_fm_bwd", [P, i64, P, i64, i64, P, INT, INT, i64, P, i64, i64, INT, S])
 _sig("dr_cuda_gru_fwd", [P, P, P, P, INT, INT, INT, P, S])
 _sig("dr_cuda_gru_bwd", [P, P, P, P, P, P, INT, INT, INT, P, P, P, P, P, S])
+_sig("dr_cuda_mha_fwd", [P, P, INT, INT, INT, INT, P, S])
+_sig("dr_cuda_mha_bwd", [P, P, P, P, INT, INT, INT, INT, P, S])
 _sig("dr_cuda_din_attention_fwd", [P, P, P, i64, INT, INT, P, P, INT, P, P, INT, P, f32, P, S])
 _sig("dr_cuda_din_attention_bwd", [P, P, P, P, i64, INT, INT, P, P, INT, P, P, INT, P, f32, P, P, P, P, P, P, P, P, S])
 _sig("dr_cuda_layer_norm_fwd", [P, i64, INT, P, P, f32, P, P, P, S])

@@ -51,7 +51,7 @@ def get_arg_parser():
                         "roles with `python -m deeprec_b200.parallel.ps_train`")
     p.add_argument("--timeline", type=int, default=0)
     p.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
-    p.add_argument("--engine", action="store_true", help="fused sm_90a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / DIN / DIEN, and DSSM / ESMM / MMoE / DBMTL / PLE / SimpleMultiTask over pooled history bags, through FusedRecEngine (models/rec_engine.py)")
+    p.add_argument("--engine", action="store_true", help="fused sm_90a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / DIN / DIEN / BST, and DSSM / ESMM / MMoE / DBMTL / PLE / SimpleMultiTask over pooled history bags, through FusedRecEngine (models/rec_engine.py)")
     p.add_argument("--log_every", type=int, default=20)
     p.add_argument("--watchdog", type=float, default=0, help="seconds without a finished step before the job dumps stacks and exits 86")
     return p
@@ -86,9 +86,9 @@ def main(argv=None) -> int:
         # under the model's own dense net (models/rec_engine.py; 1..8 GPUs when launched with torchrun / parallel.launch)
         from deeprec_b200.models import zoo
         from deeprec_b200.models.rec_engine import POOLED_SEQ_MODELS, criteo_engine, din_engine, din_ids, pooled_seq_engine, taobao_engine_batch
-        if name not in zoo.CRITEO_MODELS and name not in ("din", "dien") and name not in POOLED_SEQ_MODELS:
+        if name not in zoo.CRITEO_MODELS and name not in ("din", "dien", "bst") and name not in POOLED_SEQ_MODELS:
             raise SystemExit(f"--engine: no fused-engine adapter for {name} "
-                             f"(dlrm, {', '.join(sorted(zoo.CRITEO_MODELS))}, din, dien, {', '.join(POOLED_SEQ_MODELS)})")
+                             f"(dlrm, {', '.join(sorted(zoo.CRITEO_MODELS))}, din, dien, bst, {', '.join(POOLED_SEQ_MODELS)})")
         import torch.distributed as dist
         world, rank, lrank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0")), int(os.environ.get("LOCAL_RANK", "0"))
         torch.cuda.set_device(lrank)
@@ -103,7 +103,7 @@ def main(argv=None) -> int:
         kw = dict(optimizer=a.optimizer, learning_rate=a.learning_rate, filter_freq=2 if a.ev_filter else 0,
                   steps_to_live=4000 if a.ev_elimination == "gstep" else 0, device=dev, rank=rank, world_size=world, comm=comm,
                   micro_batch_num=a.micro_batch)
-        if name in ("din", "dien"):
+        if name in ("din", "dien", "bst"):
             L = 20
             eng = din_engine(model, a.batch_size, L, table_rows=(100000, 200000, 1000), **kw)
 

@@ -380,15 +380,24 @@ class BST(_SeqBase):
         self.final = mlp(final_hidden_units, self.emb_dim + 2 * D2, device=dev)
         self.out = nn.Linear(final_hidden_units[-1], 1, device=dev)
 
-    def forward(self, b):
-        u, q, k, mask = self._embed(b)
+    def head(self, u, q, k, mask, encoder=None):
+        """Dense part on already-looked-up embeddings (user [B, D], target [B, 2D], history [B, L, 2D] zero-padded, mask [B, L]): one encoder
+        block over [history; target] (S = L + 1 positions, the target always valid), masked mean pooling, the final MLP.  ``encoder=None`` runs
+        the block as ``self.enc(x, src_key_padding_mask=...)``; otherwise ``encoder(x, self.enc, valid)`` (:func:`nn.fused_encoder_layer`, what
+        :func:`models.rec_engine.din_engine` passes) with ``valid`` the bool [B, S] key mask."""
+        S = k.shape[1] + 1
+        if S > self.pos.shape[0]:
+            raise ValueError(f"BST: history length {S - 1} exceeds the positional table ({self.pos.shape[0] - 1})")
         x = torch.cat([k, q.unsqueeze(1)], 1)
-        x = x + self.pos[: x.shape[1]]
-        pad = torch.cat([~mask, torch.zeros(mask.shape[0], 1, dtype=torch.bool, device=mask.device)], 1)
-        h = self.enc(x, src_key_padding_mask=pad)
-        valid = (~pad).unsqueeze(-1).to(h.dtype)
-        pooled = (h * valid).sum(1) / valid.sum(1).clamp_min(1)
+        x = x + self.pos[:S]
+        valid = torch.cat([mask, torch.ones(mask.shape[0], 1, dtype=torch.bool, device=mask.device)], 1)
+        h = self.enc(x, src_key_padding_mask=~valid) if encoder is None else encoder(x, self.enc, valid)
+        v = valid.unsqueeze(-1).to(h.dtype)
+        pooled = (h * v).sum(1) / v.sum(1).clamp_min(1)
         return self.out(self.final(torch.cat([u, q, pooled], -1))).squeeze(-1)
+
+    def forward(self, b):
+        return self.head(*self._embed(b))
 
 
 class DSSM(_SeqBase):

@@ -9,6 +9,8 @@
     csrc/cuda/interaction_kernels.cu.
   * ``fused_gru``: a single-layer GRU over tail-padded sequences for training -- the input projection on the wgmma GEMM, the recurrence
     forward and backward through time on csrc/cuda/rnn_kernels.cu.
+  * ``fused_encoder_layer``: a post-norm Transformer encoder layer with a key-padding mask for training -- in_proj, out_proj and the FFN on
+    the wgmma GEMM, the multi-head self-attention core forward and backward on csrc/cuda/mha_kernels.cu.
 
 The reference runs these through cuBLAS (stream_executor/cuda/cuda_blas.cc) and ~10 TF ops per interaction
 (modelzoo/dlrm/train.py:163-236, modelzoo/deepfm/train.py:178-187).  CPU tensors fall back to the equivalent torch expression.
@@ -314,3 +316,74 @@ def fused_gru(x: torch.Tensor, gru: nn.GRU, lengths: torch.Tensor) -> torch.Tens
         raise ValueError(f"fused_gru: hidden size {H} is not supported on CUDA (one of {GRU_HIDDEN})")
     gi = _FusedMLPFn.apply(x.reshape(B * L, I).to(torch.bfloat16), False, gru.weight_ih_l0, gru.bias_ih_l0)
     return _GRURecurrenceFn.apply(gi.contiguous(), gru.weight_hh_l0, gru.bias_hh_l0, lengths.to(device=x.device, dtype=torch.int32).contiguous(), B, L)
+
+
+# ---- Transformer encoder layer -----------------------------------------------------------------------------------------------
+MHA_HEAD_DIMS = (8, 16, 32)           # head sizes csrc/cuda/mha_kernels.cu is compiled for
+MHA_MAX_LEN = 128                     # longest sequence it takes
+
+
+class _MHACoreFn(torch.autograd.Function):
+    """qkv bf16 [B S, 3E] (in_proj output, [q | k | v] per token), valid uint8 [B, S] (key mask) -> o bf16 [B S, E]: softmax(q k^T / sqrt(dh)
+    + key mask) v per (sample, head).  The backward recomputes the probabilities from qkv; it returns d(qkv) bf16 [B S, 3E]."""
+
+    @staticmethod
+    def forward(ctx, qkv, valid, B: int, S: int, heads: int):
+        E = qkv.shape[1] // 3
+        o = torch.empty(B * S, E, dtype=torch.bfloat16, device=qkv.device)
+        check(_native.cuda().dr_cuda_mha_fwd(ptr(qkv), ptr(valid), B, S, E, heads, ptr(o), stream_ptr()), "mha_fwd")
+        ctx.save_for_backward(qkv, valid, o)
+        ctx.shape = (B, S, heads)
+        return o
+
+    @staticmethod
+    def backward(ctx, do):
+        qkv, valid, o = ctx.saved_tensors
+        B, S, heads = ctx.shape
+        dqkv = torch.empty_like(qkv)
+        do = do.to(torch.bfloat16).contiguous()
+        check(_native.cuda().dr_cuda_mha_bwd(ptr(qkv), ptr(valid), ptr(o), ptr(do), B, S, qkv.shape[1] // 3, heads, ptr(dqkv), stream_ptr()),
+              "mha_bwd")
+        return dqkv, None, None, None, None
+
+
+def _check_encoder_layer(layer: nn.TransformerEncoderLayer) -> None:
+    at = layer.self_attn
+    if layer.norm_first:
+        raise ValueError("fused_encoder_layer: needs a post-norm layer (norm_first=False)")
+    if getattr(layer, "activation_relu_or_gelu", 0) != 1:
+        raise ValueError("fused_encoder_layer: needs the ReLU activation")
+    if not at.batch_first:
+        raise ValueError("fused_encoder_layer: needs batch_first=True")
+    if (at.in_proj_weight is None or at.in_proj_bias is None or at.out_proj.bias is None or layer.linear1.bias is None or layer.linear2.bias is None
+            or layer.norm1.bias is None or layer.norm2.bias is None or at.bias_k is not None):
+        raise ValueError("fused_encoder_layer: needs a layer with biases (and a packed in_proj, no bias_k / bias_v)")
+    if layer.training and max(at.dropout, layer.dropout.p, layer.dropout1.p, layer.dropout2.p) > 0:
+        raise ValueError("fused_encoder_layer: dropout > 0 while training is not supported")
+
+
+def fused_encoder_layer(x: torch.Tensor, layer: nn.TransformerEncoderLayer, valid: torch.Tensor) -> torch.Tensor:
+    """``layer(x, src_key_padding_mask=~valid)`` for a post-norm, batch-first, ReLU ``nn.TransformerEncoderLayer`` with biases over
+    ``x`` [B, S, E] with key mask ``valid`` (bool [B, S], True = the position takes part as a key; every query row is computed).  Trains the
+    module's own parameters, so state-dict names and the op-program export keep working.
+
+    CUDA: in_proj, the attention core (csrc/cuda/mha_kernels.cu: mma.sync, fp32 softmax, no atomics), out_proj and the FFN (linear1 + ReLU +
+    linear2, one node) on the wgmma GEMMs with bf16 activations and fp32 weight gradients; the residual adds and ``norm1`` / ``norm2`` are the
+    module's own, in ``x``'s dtype.  dh = E / heads must be one of ``MHA_HEAD_DIMS`` and S at most ``MHA_MAX_LEN``.  One deliberate
+    difference: a sample with no valid key gives attention output 0 where PyTorch gives NaN.  CPU: the module itself."""
+    _check_encoder_layer(layer)
+    if not x.is_cuda:
+        return layer(x, src_key_padding_mask=~valid.to(torch.bool))
+    B, S, E = x.shape
+    at = layer.self_attn
+    heads = at.num_heads
+    if E % heads or E // heads not in MHA_HEAD_DIMS or S > MHA_MAX_LEN:
+        raise ValueError(f"fused_encoder_layer: head size {E / heads:g} (E = {E}, {heads} heads) and S = {S} are not supported on CUDA "
+                         f"(head size one of {MHA_HEAD_DIMS}, S <= {MHA_MAX_LEN})")
+    x2 = x.reshape(B * S, E)
+    qkv = _FusedMLPFn.apply(x2.to(torch.bfloat16), False, at.in_proj_weight, at.in_proj_bias)
+    o = _MHACoreFn.apply(qkv.contiguous(), valid.to(device=x.device, dtype=torch.uint8).contiguous(), B, S, heads)
+    a = _FusedMLPFn.apply(o, False, at.out_proj.weight, at.out_proj.bias)
+    h = layer.norm1(x2 + a.to(x.dtype))
+    f = _FusedMLPFn.apply(h.to(torch.bfloat16), False, layer.linear1.weight, layer.linear1.bias, layer.linear2.weight, layer.linear2.bias)
+    return layer.norm2(h + f.to(h.dtype)).reshape(B, S, E)
