@@ -1,6 +1,5 @@
 // Minimal JSON reader (objects, arrays, strings, numbers, bools, null) for ModelConfig / saved_model.json / serving_versions.json.
-// Used by the CPU serving runtime (csrc/host/cpu_serving.cc).  The GPU runtime (csrc/cuda/serving_runtime.cu) still carries its own copy of
-// these ~40 lines: it was validated on hardware before this header existed and is only touched when a GPU is available to re-test it.
+// Used by both serving runtimes (csrc/host/cpu_serving.cc, csrc/cuda/serving_runtime.cu) and the saved-model reader (saved_model.h).
 #pragma once
 #include <cstdio>
 #include <cstdlib>

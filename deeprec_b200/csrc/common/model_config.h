@@ -17,6 +17,8 @@
 #include <string>
 #include <vector>
 
+#include "mini_json.h"
+
 namespace drcfg {
 
 struct Compat {
@@ -43,8 +45,7 @@ inline bool Known(const std::string& k) {
   return false;
 }
 
-// J: a parsed JSON object with get(key) / n(key, default) / s(key, default) and an `obj` key-value list (drjson::JVal, serve::JVal)
-template <class J> Compat ParseCompat(const J& j, const char* who) {
+inline Compat ParseCompat(const drjson::JVal& j, const char* who) {
   Compat c;
   for (const auto& kv : j.obj) if (!Known(kv.first)) c.unknown.push_back(kv.first);
   static const char* kStructural[] = {"use_per_session_threads", "use_multi_stream", "inter_op_parallelism_threads", "model_update_inter_threads", "kmp_blocktime",

@@ -29,6 +29,7 @@
 #include "../common/bundle.h"
 #include "../common/model_config.h"
 #include "../common/predict_pb.h"
+#include "../common/saved_model.h"
 #include "table.cuh"
 
 // kernel launchers from the other translation units of this library
@@ -87,6 +88,7 @@ int dr_cuda_head(const void* h, int64_t ldh, int64_t B, int K, const float* w, c
 }
 
 namespace serve {
+using namespace drsm;
 
 // ---- device placement optimisation (ModelConfig "enable_device_placement_optimization", the reference's gpu_device_placement_pass.cc: the embedding
 // layer stays on the CPU for GPU inference) -- the tables live in the HOST engine (libdeeprec_host.so next to this library, bound at run time so
@@ -116,43 +118,9 @@ struct HostApi {
   }
 };
 
-// ---------------------------------------------------------------------------------------------------------------
-// minimal JSON (objects, arrays, strings, numbers, bools) -- enough for ModelConfig / saved_model.json / state files
-// ---------------------------------------------------------------------------------------------------------------
-struct JVal {
-  enum T { NUL, NUM, STR, ARR, OBJ, BOOL } t = NUL;
-  double num = 0; std::string str; std::vector<JVal> arr; std::vector<std::pair<std::string, JVal>> obj;
-  const JVal* get(const std::string& k) const { for (auto& kv : obj) if (kv.first == k) return &kv.second; return nullptr; }
-  double n(const std::string& k, double d) const { auto* v = get(k); return v && (v->t == NUM || v->t == BOOL) ? v->num : d; }
-  std::string s(const std::string& k, const std::string& d) const { auto* v = get(k); return v && v->t == STR ? v->str : d; }
-};
-struct JParser {
-  const char* p; const char* e; bool ok = true;
-  void ws() { while (p < e && (*p == ' ' || *p == '\n' || *p == '\t' || *p == '\r')) ++p; }
-  JVal parse() { ws(); JVal v; if (p >= e) { ok = false; return v; }
-    if (*p == '{') { v.t = JVal::OBJ; ++p; ws(); if (p < e && *p == '}') { ++p; return v; }
-      while (ok) { ws(); JVal k = parse(); if (k.t != JVal::STR) { ok = false; break; } ws(); if (p >= e || *p != ':') { ok = false; break; } ++p;
-        v.obj.emplace_back(k.str, parse()); ws(); if (p < e && *p == ',') { ++p; continue; } if (p < e && *p == '}') { ++p; break; } ok = false; } return v; }
-    if (*p == '[') { v.t = JVal::ARR; ++p; ws(); if (p < e && *p == ']') { ++p; return v; }
-      while (ok) { v.arr.push_back(parse()); ws(); if (p < e && *p == ',') { ++p; continue; } if (p < e && *p == ']') { ++p; break; } ok = false; } return v; }
-    if (*p == '"') { v.t = JVal::STR; ++p; while (p < e && *p != '"') { if (*p == '\\' && p + 1 < e) { ++p; char c = *p; v.str.push_back(c == 'n' ? '\n' : c == 't' ? '\t' : c); } else v.str.push_back(*p); ++p; } if (p < e) ++p; else ok = false; return v; }
-    if (!strncmp(p, "true", 4)) { v.t = JVal::BOOL; v.num = 1; p += 4; return v; }
-    if (!strncmp(p, "false", 5)) { v.t = JVal::BOOL; v.num = 0; p += 5; return v; }
-    if (!strncmp(p, "null", 4)) { p += 4; return v; }
-    char* end = nullptr; v.num = strtod(p, &end); if (end == p) { ok = false; return v; } v.t = JVal::NUM; p = end; return v; }
-};
-static bool ParseJson(const std::string& s, JVal* out) { JParser ps{s.data(), s.data() + s.size()}; *out = ps.parse(); return ps.ok; }
-static bool ReadFile(const std::string& path, std::string* out) {
-  FILE* f = fopen(path.c_str(), "rb"); if (!f) return false;
-  char buf[65536]; size_t n; out->clear();
-  while ((n = fread(buf, 1, sizeof(buf), f)) > 0) out->append(buf, n);
-  fclose(f); return true;
-}
-
 #define SV_CUDA(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { fprintf(stderr, "[deeprec_serving] %s: %s\n", #expr, cudaGetErrorString(_e)); return false; } } while (0)
 
 static uint16_t f2bf(float f) { uint32_t u; memcpy(&u, &f, 4); uint32_t r = 0x7FFF + ((u >> 16) & 1); return (uint16_t)((u + r) >> 16); }
-static int pad8(int n) { return (n + 7) / 8 * 8; }
 
 struct DevBuf {      // owning, move-only device allocation
   void* p = nullptr; size_t n = 0;
@@ -169,24 +137,6 @@ template <typename T> static bool Upload(DevBuf& b, const std::vector<T>& h) {
   if (!b.alloc(h.size() * sizeof(T))) return false;
   return cudaMemcpy(b.p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
 }
-
-// Op program (saved_model.json "arch": "program", serving/export.py::export_saved_model_program): the inference graph of a Criteo-style model
-// other than DLRM as a list of ops over [B, width] buffers; buffer 0 = dense inputs, buffer 1 = embeddings [B, T * D].  Same format and
-// op set as the CPU runtime (csrc/host/cpu_serving.cc); here LINEAR runs on the wgmma GEMM and the rest on program_kernels.cu.
-enum POpKind { P_CONCAT, P_LINEAR, P_AFFINE, P_FM, P_CROSS, P_MUL_ADD, P_ADD, P_LAYERNORM, P_MUL, P_SLICE,
-               P_VALID_MASK, P_SEQ_ZIP, P_SEQ_MASK, P_SEQ_SUM, P_DIN_ATT, P_PRELU, P_SOFTMAX, P_COSINE, P_TILE, P_GRU, P_SEQ_LAST, P_MHA, P_SEQ_MEAN, P_NUM_OPS };     // sequence-model ops: see cpu_serving.cc
-// rows1 / P_TILE: sample-aware graph compression (serving/export.py::compress_sample_aware): user-side ops run once per request on row 0
-// len on LINEAR / LAYERNORM: applied at each of `len` positions of a [B, len * w] sequence buffer (DIEN / BST; the buffer must be un-padded so that it
-// IS a [B * len, w] matrix); mode: din_attention output (0 weighted sum, 1 softmax weights); heads: mha
-struct POp { int kind = 0, out = 0; std::vector<int> in; bool relu = false, rows1 = false; float eps = 1e-5f; int start = 0, len = 0, mode = 0, heads = 1; std::string name; };
-struct Arch {
-  int num_dense = 13, T = 0, D = 16; std::vector<int> bot, top; float bn_eps = 1e-3f; int Zp = 0, inter = 0;
-  bool program = false; std::vector<POp> ops; int nbuf = 2, out_buf = -1;
-  // requests carry R id rows; lookup column c reads request row id_map[c] from table col_table[c] (both identity, C == T, unless several
-  // columns share a feature (Wide&Deep) or a table (DIN: target item + L history positions))
-  int R = 0, C = 0; std::vector<int> id_map, col_table;
-  int n_out = 1;        // multi-task programs: the output buffer holds n_out logits per row, the response n_out probabilities per row
-};
 
 struct LayerW {
   int N, K, Kp; DevBuf w_bf16, bias;
@@ -223,23 +173,11 @@ struct DeviceModel {
   DevBuf structs;      // DrDeviceTable[T] on the device
   DevBuf col_table;    // int32 [C]: table of every lookup column (program models; identity otherwise)
   // device placement optimisation: the tables live in the host engine instead (HostEV handles, owned), col_handles[c] = table of lookup column c
-  bool host_resident = false; std::vector<void*> host_tables, col_handles; std::vector<int64_t> host_sample_keys;
+  bool host_resident = false; std::vector<void*> host_tables, col_handles;
   ~DeviceModel() { if (host_resident) for (void* h : host_tables) if (h) HostApi::Get().destroy(h); }
 };
 
-static bool ReadTensor(dr::BundleReader& r, const std::string& name, std::vector<uint8_t>* out, std::vector<int64_t>* shape = nullptr) {
-  auto* e = r.Find(name); if (!e) return false;
-  out->resize((size_t)e->nbytes);
-  if (shape) *shape = e->shape;
-  return r.Read(*e, out->data(), 1) == 0;
-}
-template <typename T> static bool ReadVec(dr::BundleReader& r, const std::string& name, std::vector<T>* out, std::vector<int64_t>* shape = nullptr) {
-  if constexpr (std::is_same<T, float>::value) return dr::ReadAsFloat(r, name, out, shape);    // bf16 / f16 / int8(+scale) tensors of a converted model
-  std::vector<uint8_t> raw; if (!ReadTensor(r, name, &raw, shape)) return false;
-  out->resize(raw.size() / sizeof(T)); memcpy(out->data(), raw.data(), raw.size()); return true;
-}
-
-// BatchNorm (moving statistics) of layer l-1 folded into Linear l:  W' = W diag(s), b' = b + W t
+// fp8 path: E4M3 copy of a layer's fp32 weights W' [N, Kp], one scale per output channel
 static bool QuantizeLayer(LayerW& L, const std::vector<float>& w_folded /*[N, Kp]*/) {
   L.Kp16 = pad16(L.Kp);
   DevBuf tmp;
@@ -267,312 +205,153 @@ static bool ApplyActScales(DenseParams& dp) {
 static int prog_npad(int w) { return w <= 16 ? 16 : w <= 32 ? 32 : pad8(w); }
 static int prog_ld(const Arch& a, const std::vector<int>& width, int id) { return id == 0 ? pad8(a.num_dense) : id == 1 ? a.C * a.D : prog_npad(width[(size_t)id]); }
 
-// weights + buffer widths of a program model; every shape is checked against the widths implied by the op list
+// Device layout of a program model's weights: LINEAR as bf16 [Np, Kp] with zero pad rows / columns, GRU's input projection as bf16 [3H, I],
+// the other vectors fp32.  The checks here are the kernels' own: a sequence buffer is a [B * len, w] matrix only when its rows are not
+// padded, the GEMM's 8-element rule, the recurrence kernel's H <= 126 and the attention kernel's head width <= 64.
 static bool BuildProgram(dr::BundleReader& r, const Arch& a, std::shared_ptr<DenseParams>* out) {
+  ProgramData p;
+  if (!ReadProgram(r, a, &p)) return false;
   auto dp = std::make_shared<DenseParams>();
-  dp->width.assign((size_t)a.nbuf, 0); dp->width[0] = a.num_dense; dp->width[1] = a.C * a.D;
   dp->pdata.resize(a.ops.size());
   for (size_t i = 0; i < a.ops.size(); ++i) {
-    const POp& op = a.ops[i]; auto& d = dp->pdata[i];
-    const int w0 = dp->width[(size_t)op.in[0]];
-    int w = w0;
-    const std::string base = "prog/" + op.name + "/";
-    std::vector<float> v0, v1;
+    const POp& op = a.ops[i]; const OpTensors& t = p.ops[i]; auto& d = dp->pdata[i];
+    const int w0 = p.width[(size_t)op.in[0]];
+    const bool unpadded = prog_ld(a, p.width, op.in[0]) == w0;
+    d.H1 = t.H1; d.H2 = t.H2;
+    if ((!t.v0.empty() && !Upload(d.v0, t.v0)) || (!t.v1.empty() && !Upload(d.v1, t.v1))) return false;
     switch (op.kind) {
-      case P_CONCAT: w = 0; for (int b : op.in) w += dp->width[(size_t)b]; break;
-      case P_LINEAR: {                                               // len > 0: the same Linear at each of len positions ([B, len * K] == [B * len, K])
-        std::vector<float> W, b;
-        const int S = op.len > 0 ? op.len : 1;
-        if (w0 % S) return false;
-        const int K = w0 / S;
-        if (!ReadVec(r, base + "kernel", &W) || !ReadVec(r, base + "bias", &b) || b.empty() || W.size() != b.size() * (size_t)K) return false;
-        const int N = (int)b.size();
-        // a sequence GEMM needs both buffers un-padded (row pitch == width) and K, N on the GEMM's 8-element rule with no output padding
-        if (S > 1 && (prog_ld(a, dp->width, op.in[0]) != w0 || K % 8 || prog_npad(N) != N || prog_npad(S * N) != S * N)) return false;
-        const int Np = prog_npad(N), Kp = S > 1 ? K : prog_ld(a, dp->width, op.in[0]);
+      case P_LINEAR: {                                               // len > 1: [B, len * K] == [B * len, K], no output padding either
+        const int S = op.len > 0 ? op.len : 1, N = t.N, K = t.K;
+        if (S > 1 && (!unpadded || K % 8 || prog_npad(N) != N || prog_npad(S * N) != S * N)) return false;
+        const int Np = prog_npad(N), Kp = S > 1 ? K : prog_ld(a, p.width, op.in[0]);
         std::vector<uint16_t> wb((size_t)Np * Kp, 0); std::vector<float> bias((size_t)Np, 0.f);     // zero rows / columns: pad outputs are exact zeros
-        for (int n = 0; n < N; ++n) { bias[(size_t)n] = b[(size_t)n]; for (int k = 0; k < K; ++k) wb[(size_t)n * Kp + k] = f2bf(W[(size_t)n * K + k]); }
+        for (int n = 0; n < N; ++n) { bias[(size_t)n] = t.b[(size_t)n]; for (int k = 0; k < K; ++k) wb[(size_t)n * Kp + k] = f2bf(t.W[(size_t)n * K + k]); }
         d.L.N = N; d.L.K = K; d.L.Kp = Kp; d.L.Np = Np;
         if (!Upload(d.L.w_bf16, wb) || !Upload(d.L.bias, bias)) return false;
-        w = N * S; break;
-      }
-      case P_LAYERNORM: {                                            // len > 0: per position of an un-padded sequence buffer
-        const int S = op.len > 0 ? op.len : 1;
-        if (w0 % S || (S > 1 && prog_ld(a, dp->width, op.in[0]) != w0)) return false;
-        if (!ReadVec(r, base + "scale", &v0) || !ReadVec(r, base + "shift", &v1) || (int)v0.size() != w0 / S || (int)v1.size() != w0 / S) return false;
-        if (!Upload(d.v0, v0) || !Upload(d.v1, v1)) return false;
         break;
       }
-      case P_AFFINE:
-        if (!ReadVec(r, base + "scale", &v0) || !ReadVec(r, base + "shift", &v1) || (int)v0.size() != w0 || (int)v1.size() != w0) return false;
-        if (!Upload(d.v0, v0) || !Upload(d.v1, v1)) return false;
-        break;
-      case P_FM: if (op.in[0] != 1) return false; w = a.D; break;
-      case P_CROSS:
-        if (!ReadVec(r, base + "w", &v0) || !ReadVec(r, base + "b", &v1) || (int)v0.size() != w0 || (int)v1.size() != w0 || dp->width[(size_t)op.in[1]] != w0) return false;
-        if (!Upload(d.v0, v0) || !Upload(d.v1, v1)) return false;
-        break;
-      case P_MUL_ADD: if (dp->width[(size_t)op.in[1]] != w0 || dp->width[(size_t)op.in[2]] != w0) return false; break;
-      case P_MUL:
-      case P_ADD: if (dp->width[(size_t)op.in[1]] != w0) return false; break;
-      case P_SLICE: if (op.start < 0 || op.len <= 0 || op.start + op.len > w0) return false; w = op.len; break;
-      case P_VALID_MASK: if (op.start < 0 || op.len <= 0 || op.start + op.len > a.C) return false; w = op.len; break;
-      case P_SEQ_ZIP: {
-        const int wb = dp->width[(size_t)op.in[1]];
-        if (op.len <= 0 || w0 % op.len || wb % op.len) return false;
-        w = w0 + wb; break;
-      }
-      case P_SEQ_MASK: if (op.len <= 0 || w0 % op.len || dp->width[(size_t)op.in[1]] != op.len) return false; break;
-      case P_SEQ_SUM: if (op.len <= 0 || w0 % op.len) return false; w = w0 / op.len; break;
-      case P_PRELU: if (!ReadVec(r, base + "alpha", &v0) || (int)v0.size() != w0 || !Upload(d.v0, v0)) return false; break;
-      case P_SOFTMAX: break;
-      case P_TILE: break;
+      case P_LAYERNORM: if (op.len > 1 && !unpadded) return false; break;
       case P_GRU: {                                                  // input projection on the GEMM ([B * L, I] x W_ih^T + b_ih -> [B * L, 3H]), recurrence kernel
-        std::vector<float> wih, whh, bih, bhh;
-        if (op.len <= 0 || w0 % op.len || !ReadVec(r, base + "w_ih", &wih) || !ReadVec(r, base + "w_hh", &whh) || !ReadVec(r, base + "b_ih", &bih) || !ReadVec(r, base + "b_hh", &bhh)) return false;
-        const int I = w0 / op.len, H3 = (int)bih.size(), H = H3 / 3;
-        if (H <= 0 || H3 != 3 * H || (int)bhh.size() != H3 || (int)wih.size() != H3 * I || (int)whh.size() != H3 * H) return false;
-        if (prog_ld(a, dp->width, op.in[0]) != w0 || I % 8 || H3 % 8 || H > 126) return false;       // un-padded input sequence, GEMM 8-element rule
-        std::vector<uint16_t> wb((size_t)H3 * I);
-        for (size_t i2 = 0; i2 < wb.size(); ++i2) wb[i2] = f2bf(wih[i2]);
-        d.L.N = H3; d.L.K = I; d.L.Kp = I; d.L.Np = H3; d.H1 = H;
-        if (!Upload(d.L.w_bf16, wb) || !Upload(d.L.bias, bih) || !Upload(d.v0, whh) || !Upload(d.v1, bhh)) return false;
-        w = op.len * H; break;
-      }
-      case P_SEQ_LAST:
-      case P_SEQ_MEAN: if (op.len <= 0 || w0 % op.len || dp->width[(size_t)op.in[1]] != op.len) return false; w = w0 / op.len; break;
-      case P_MHA: {
-        if (op.len <= 0 || w0 % (3 * op.len) || dp->width[(size_t)op.in[1]] != op.len) return false;
-        const int E = w0 / (3 * op.len);
-        if (op.heads <= 0 || E % op.heads || E / op.heads > 64) return false;
-        w = op.len * E; break;
-      }
-      case P_COSINE: if (dp->width[(size_t)op.in[1]] != w0) return false; w = 1; break;
-      case P_DIN_ATT: {
-        const int wk = dp->width[(size_t)op.in[1]], L = dp->width[(size_t)op.in[2]];
-        if (L <= 0 || wk != L * w0 || op.mode < 0 || op.mode > 1) return false;
-        if (op.mode == 1) w = L;                                     // the softmax weights themselves (DIEN)
-        static const char* kT[] = {"w1", "b1", "w2", "b2", "w3", "b3"};
-        std::vector<std::vector<float>> t(6);
-        for (int i2 = 0; i2 < 6; ++i2) if (!ReadVec(r, base + kT[i2], &t[(size_t)i2])) return false;
-        d.H1 = (int)t[1].size(); d.H2 = (int)t[3].size();
-        if (d.H1 <= 0 || d.H2 <= 0 || (int)t[0].size() != d.H1 * 4 * w0 || (int)t[2].size() != d.H2 * d.H1 || (int)t[4].size() != d.H2 || t[5].size() != 1) return false;
-        d.b3 = t[5][0];
-        d.att.resize(5);
-        for (int i2 = 0; i2 < 5; ++i2) if (!Upload(d.att[(size_t)i2], t[(size_t)i2])) return false;
+        if (!unpadded || t.K % 8 || t.N % 8 || t.H1 > 126) return false;
+        std::vector<uint16_t> wb(t.W.size());
+        for (size_t k = 0; k < wb.size(); ++k) wb[k] = f2bf(t.W[k]);
+        d.L.N = t.N; d.L.K = t.K; d.L.Kp = t.K; d.L.Np = t.N;
+        if (!Upload(d.L.w_bf16, wb) || !Upload(d.L.bias, t.b)) return false;
         break;
       }
-      default: return false;
+      case P_MHA: if (w0 / (3 * op.len) / op.heads > 64) return false; break;
+      case P_DIN_ATT:
+        d.b3 = t.att[5][0]; d.att.resize(5);
+        for (int k = 0; k < 5; ++k) if (!Upload(d.att[(size_t)k], t.att[(size_t)k])) return false;
+        break;
+      default: break;
     }
-    if (w <= 0) return false;
-    dp->width[(size_t)op.out] = w;
   }
-  if (dp->width[(size_t)a.out_buf] < a.n_out) return false;
+  dp->width = std::move(p.width);
   *out = dp;
   return true;
 }
 
+// DLRM: bf16 weights (and their E4M3 copy for the fp8 path) of the BatchNorm-folded layers
 static bool BuildDense(dr::BundleReader& r, const Arch& a, std::shared_ptr<DenseParams>* out, bool want_fp8 = false) {
   if (a.program) return BuildProgram(r, a, out);
+  DlrmDense t;
+  if (!ReadDlrmDense(r, a, &t)) return false;
   auto dp = std::make_shared<DenseParams>();
-  dp->bot.reserve(a.bot.size()); dp->top.reserve(a.top.size());
-  std::vector<float> s_prev, t_prev;
-  int k = a.num_dense;
-  for (size_t l = 0; l < a.bot.size(); ++l) {
-    const std::string nm = "mlp_bot_" + std::to_string(l);
-    int N = a.bot[l], Kp = pad8(k);
-    std::vector<float> W, b, gamma, beta, mean, var;
-    if (!ReadVec(r, "dense/" + nm + "/kernel", &W) || !ReadVec(r, "dense/" + nm + "/bias", &b) || !ReadVec(r, "dense/" + nm + "/bn_gamma", &gamma) ||
-        !ReadVec(r, "dense/" + nm + "/bn_beta", &beta) || !ReadVec(r, "bn/" + nm + "/moving_mean", &mean) || !ReadVec(r, "bn/" + nm + "/moving_variance", &var)) return false;
-    if ((int)W.size() != N * Kp) return false;
-    std::vector<uint16_t> wb((size_t)N * Kp); std::vector<float> bias(N), wf((size_t)N * Kp);
-    for (int n = 0; n < N; ++n) {
-      double acc = b[n];
-      for (int kk = 0; kk < Kp; ++kk) {
-        float w = W[(size_t)n * Kp + kk];
-        if (l > 0 && kk < k) { acc += (double)w * t_prev[kk]; w *= s_prev[kk]; }
-        wb[(size_t)n * Kp + kk] = f2bf(w); wf[(size_t)n * Kp + kk] = w;
-      }
-      bias[n] = (float)acc;
-    }
-    dp->bot.emplace_back(); auto& dst = dp->bot.back(); dst.N = N; dst.K = k; dst.Kp = Kp;
-    if (!Upload(dst.w_bf16, wb) || !Upload(dst.bias, bias)) return false;
-    if (want_fp8 && !QuantizeLayer(dst, wf)) return false;
-    s_prev.assign(N, 0.f); t_prev.assign(N, 0.f);
-    for (int n = 0; n < N; ++n) { float rs = 1.0f / std::sqrt(var[n] + a.bn_eps); s_prev[n] = gamma[n] * rs; t_prev[n] = beta[n] - mean[n] * s_prev[n]; }
-    k = N;
-  }
-  if (!Upload(dp->last_scale, s_prev) || !Upload(dp->last_shift, t_prev)) return false;
-  k = a.inter;
-  for (size_t l = 0; l < a.top.size(); ++l) {
-    const std::string nm = "mlp_top_" + std::to_string(l);
-    int N = a.top[l], Kp = pad8(k);
-    std::vector<float> W, b;
-    if (!ReadVec(r, "dense/" + nm + "/kernel", &W) || !ReadVec(r, "dense/" + nm + "/bias", &b) || (int)W.size() != N * Kp) return false;
-    std::vector<uint16_t> wb(W.size());
-    for (size_t i = 0; i < W.size(); ++i) wb[i] = f2bf(W[i]);
-    dp->top.emplace_back(); auto& dst = dp->top.back(); dst.N = N; dst.K = k; dst.Kp = Kp;
-    if (!Upload(dst.w_bf16, wb) || !Upload(dst.bias, b)) return false;
-    if (want_fp8 && !QuantizeLayer(dst, W)) return false;
-    k = N;
-  }
-  std::vector<float> hw, hb;
-  if (!ReadVec(r, "dense/logits/kernel", &hw) || !ReadVec(r, "dense/logits/bias", &hb)) return false;
-  if (!Upload(dp->head_w, hw) || !Upload(dp->head_b, hb)) return false;
+  auto layer = [&](const DenseLayer& s, LayerW& L) {
+    L.N = s.N; L.K = s.K; L.Kp = s.Kp;
+    std::vector<uint16_t> wb(s.W.size());
+    for (size_t i = 0; i < wb.size(); ++i) wb[i] = f2bf(s.W[i]);
+    return Upload(L.w_bf16, wb) && Upload(L.bias, s.b) && (!want_fp8 || QuantizeLayer(L, s.W));
+  };
+  dp->bot.resize(t.bot.size()); dp->top.resize(t.top.size());
+  for (size_t l = 0; l < t.bot.size(); ++l) if (!layer(t.bot[l], dp->bot[l])) return false;
+  for (size_t l = 0; l < t.top.size(); ++l) if (!layer(t.top[l], dp->top[l])) return false;
+  if (!Upload(dp->last_scale, t.last_scale) || !Upload(dp->last_shift, t.last_shift) || !Upload(dp->head_w, t.head_w) || !Upload(dp->head_b, t.head_b)) return false;
   *out = dp;
   return true;
 }
 
 static int64_t NextPow2(int64_t n) { int64_t p = 1; while (p < n) p <<= 1; return p; }
 
-static bool BuildTable(dr::BundleReader& r, int t, int D, TableDev* td, int64_t extra_rows) {
-  const std::string base = "table/" + std::to_string(t);
-  std::vector<int64_t> keys, freqs, vers; std::vector<float> vals, def;
-  if (!ReadVec(r, base + "-keys", &keys) || !ReadVec(r, base + "-values", &vals) || !ReadVec(r, base + "-default", &def)) return false;
-  ReadVec(r, base + "-freqs", &freqs); ReadVec(r, base + "-versions", &vers);
-  const int64_t n = (int64_t)keys.size();
-  td->sample_keys.assign(keys.begin(), keys.begin() + std::min<int64_t>(n, 512));
+static bool BuildTable(const TableData& in, int D, TableDev* td, int64_t extra_rows) {
+  const int64_t n = (int64_t)in.keys.size();
   const int64_t rows = n + extra_rows, cap = NextPow2(std::max<int64_t>(1024, 2 * rows));
   auto& T = td->t;
   if (!td->slots.alloc((size_t)cap * sizeof(DrSlot)) ||
-      !td->rows.alloc((size_t)rows * D * 4) || !td->free_list.alloc(rows * 4 + 16) || !td->counters.alloc(32) || !Upload(td->def, def)) return false;
+      !td->rows.alloc((size_t)rows * D * 4) || !td->free_list.alloc(rows * 4 + 16) || !td->counters.alloc(32) || !Upload(td->def, in.def)) return false;
   dr_cuda_table_init_slots(td->slots.p, cap, 0);
   cudaMemset(td->counters.p, 0, 32);
   T.slots = td->slots.as<DrSlot>();
   T.rows = td->rows.as<float>(); T.free_list = td->free_list.as<int32_t>();
   T.counters = td->counters.as<int32_t>(); T.default_matrix = td->def.as<float>(); T.bloom = nullptr;
-  T.capacity = cap; T.row_capacity = rows; T.default_value_dim = (int64_t)def.size() / D; T.bloom_m = 0;
+  T.capacity = cap; T.row_capacity = rows; T.default_value_dim = (int64_t)in.def.size() / D; T.bloom_m = 0;
   T.dim = D; T.stride = D; T.num_slots = 0; T.has_scalars = 0; T.filter_type = 0; T.filter_freq = 0; T.bloom_k = 0; T.is_inference = 1;
   T.no_permission = 0.f; T.steps_to_live = 0; T.l2_weight_threshold = -1.f;
   td->n_rows = n;
   if (n) {
     DevBuf dk, dv, df, dver, kept;
-    if (!Upload(dk, keys) || !Upload(dv, vals) || !kept.alloc(4)) return false;
+    if (!Upload(dk, in.keys) || !Upload(dv, in.values) || !kept.alloc(4)) return false;
     cudaMemset(kept.p, 0, 4);
-    if (!freqs.empty()) Upload(df, freqs);
-    if (!vers.empty()) Upload(dver, vers);
-    if (dr_cuda_table_import(&T, dk.as<int64_t>(), dv.as<float>(), D, freqs.empty() ? nullptr : df.as<int64_t>(), vers.empty() ? nullptr : dver.as<int64_t>(), n, 0, 1, 0,
-                             kept.as<int32_t>(), 0) != 0) return false;
+    if (!in.freqs.empty()) Upload(df, in.freqs);
+    if (!in.versions.empty()) Upload(dver, in.versions);
+    if (dr_cuda_table_import(&T, dk.as<int64_t>(), dv.as<float>(), D, in.freqs.empty() ? nullptr : df.as<int64_t>(), in.versions.empty() ? nullptr : dver.as<int64_t>(),
+                             n, 0, 1, 0, kept.as<int32_t>(), 0) != 0) return false;
     SV_CUDA(cudaDeviceSynchronize());
   }
   return true;
 }
 
 // host-resident twin of BuildTable (device placement optimisation): the rows go into a HostEV of the host engine
-static void* BuildHostTable(dr::BundleReader& r, int t, int D, std::vector<int64_t>* sample) {
+static void* BuildHostTable(const TableData& in, int D) {
   HostApi& api = HostApi::Get();
   if (!api.ok) return nullptr;
-  const std::string base = "table/" + std::to_string(t);
-  std::vector<int64_t> keys, freqs, vers; std::vector<float> vals, def;
-  if (!ReadVec(r, base + "-keys", &keys) || !ReadVec(r, base + "-values", &vals) || !ReadVec(r, base + "-default", &def)) return nullptr;
-  ReadVec(r, base + "-freqs", &freqs); ReadVec(r, base + "-versions", &vers);
-  if (def.empty() || def.size() % (size_t)D || vals.size() != keys.size() * (size_t)D) return nullptr;
   DrEvConfig c{};
-  c.dim = D; c.num_slots = 0; c.has_scalars = 0; c.init_capacity = std::max<int64_t>(1024, (int64_t)keys.size() * 2);
-  c.default_value_dim = (int64_t)def.size() / D; c.num_partitions = 16; c.record_freq = 1; c.record_version = 1; c.l2_weight_threshold = -1.f;
+  c.dim = D; c.num_slots = 0; c.has_scalars = 0; c.init_capacity = std::max<int64_t>(1024, (int64_t)in.keys.size() * 2);
+  c.default_value_dim = (int64_t)in.def.size() / D; c.num_partitions = 16; c.record_freq = 1; c.record_version = 1; c.l2_weight_threshold = -1.f;
   void* h = api.create(&c);
   if (!h) return nullptr;
-  api.set_default(h, def.data());
-  if (!keys.empty())
-    api.import(h, keys.data(), vals.data(), D, freqs.size() == keys.size() ? freqs.data() : nullptr, vers.size() == keys.size() ? vers.data() : nullptr,
-               (int64_t)keys.size(), 0, 1, 0);
-  sample->assign(keys.begin(), keys.begin() + std::min<size_t>(keys.size(), 512));
+  api.set_default(h, in.def.data());
+  if (!in.keys.empty())
+    api.import(h, in.keys.data(), in.values.data(), D, in.freqs.empty() ? nullptr : in.freqs.data(), in.versions.empty() ? nullptr : in.versions.data(),
+               (int64_t)in.keys.size(), 0, 1, 0);
   return h;
-}
-
-static bool LoadArch(const std::string& dir, Arch* a, int64_t* version, std::string* prefix) {
-  std::string txt; JVal j;
-  if (!ReadFile(dir + "/saved_model.json", &txt) || !ParseJson(txt, &j)) return false;
-  a->num_dense = (int)j.n("num_dense", 13); a->D = (int)j.n("embedding_dim", 16); a->bn_eps = (float)j.n("bn_eps", 1e-3);
-  a->T = (int)j.n("num_tables", 0);
-  if (auto* b = j.get("mlp_bot")) for (auto& v : b->arr) a->bot.push_back((int)v.num);
-  if (auto* b = j.get("mlp_top")) for (auto& v : b->arr) a->top.push_back((int)v.num);
-  int F = a->T + 1; a->inter = a->D + F * (F - 1) / 2; a->Zp = pad8(a->inter);
-  *version = (int64_t)j.n("version", 0);
-  *prefix = dir + "/" + j.s("variables", "variables/variables");
-  a->C = a->T;
-  if (auto* ct = j.get("col_table")) {
-    if (ct->t != JVal::ARR || ct->arr.empty()) return false;
-    a->C = (int)ct->arr.size();
-    for (auto& v : ct->arr) a->col_table.push_back((int)v.num);
-  } else for (int t = 0; t < a->T; ++t) a->col_table.push_back(t);
-  for (int v : a->col_table) if (v < 0 || v >= a->T) return false;
-  a->R = (int)j.n("num_id_rows", a->C);
-  a->id_map.resize((size_t)std::max(0, a->C));
-  for (int c = 0; c < a->C; ++c) a->id_map[(size_t)c] = c;
-  if (auto* im = j.get("id_map")) {
-    if (im->t != JVal::ARR || (int)im->arr.size() != a->C) return false;
-    for (int c = 0; c < a->C; ++c) a->id_map[(size_t)c] = (int)im->arr[(size_t)c].num;
-  }
-  for (int v : a->id_map) if (v < 0 || v >= a->R) return false;
-  if (a->R <= 0) return false;
-  if (j.s("arch", "") == "program") {
-    a->program = true;
-    std::vector<std::string> names = {"dense", "emb"};
-    auto id_of = [&](const std::string& n) { for (size_t i = 0; i < names.size(); ++i) if (names[i] == n) return (int)i; return -1; };
-    static const char* kNames[] = {"concat", "linear", "affine", "fm", "cross", "mul_add", "add", "layernorm", "mul", "slice",
-                                   "valid_mask", "seq_zip", "seq_mask", "seq_sum", "din_attention", "prelu", "softmax", "cosine", "tile", "gru", "seq_last", "mha", "seq_mean"};
-    static const int kArity[] = {-1, 1, 1, 1, 2, 3, 2, 1, 2, 1, 1, 2, 2, 1, 3, 1, 1, 2, 1, 1, 2, 2, 2};
-    const JVal* pr = j.get("program");
-    if (!pr || pr->t != JVal::ARR) return false;
-    std::vector<bool> rows1_buf(2, false);
-    for (const JVal& o : pr->arr) {
-      POp op; op.name = o.s("out", ""); op.relu = o.n("relu", 0) != 0; op.eps = (float)o.n("eps", 1e-5); op.kind = -1;
-      op.start = (int)o.n("start", 0); op.len = (int)o.n("len", 0); op.rows1 = o.n("rows1", 0) != 0; op.mode = (int)o.n("mode", 0); op.heads = (int)o.n("heads", 1);
-      const std::string kind = o.s("op", "");
-      for (int k = 0; k < P_NUM_OPS; ++k) if (kind == kNames[k]) op.kind = k;
-      const JVal* in = o.get("in");
-      if (op.kind < 0 || op.name.empty() || !in || id_of(op.name) >= 0) return false;
-      for (const JVal& v : in->arr) { const int id = id_of(v.str); if (id < 0) return false; op.in.push_back(id); }    // inputs must already exist
-      if ((kArity[op.kind] >= 0 && (int)op.in.size() != kArity[op.kind]) || op.in.empty()) return false;
-      // a buffer computed at batch 1 holds one valid row: only rows1 ops and TILE may read it
-      if (op.kind == P_TILE && op.rows1) return false;
-      if (!op.rows1 && op.kind != P_TILE) for (int id : op.in) if (id < (int)rows1_buf.size() && rows1_buf[(size_t)id]) return false;
-      op.out = (int)names.size(); names.push_back(op.name);
-      rows1_buf.resize(names.size(), false); rows1_buf[(size_t)op.out] = op.rows1;
-      a->ops.push_back(std::move(op));
-    }
-    a->nbuf = (int)names.size();
-    a->out_buf = id_of(j.s("output", ""));
-    if (a->out_buf >= 0 && a->out_buf < (int)rows1_buf.size() && rows1_buf[(size_t)a->out_buf]) return false;
-    a->n_out = (int)j.n("num_outputs", 1);
-    if (a->n_out < 1 || a->n_out > 16) return false;
-    // the embedding buffer doubles as a GEMM operand: its row pitch T * D must obey the 16-byte rule; rows are gathered as float4 groups
-    return a->T > 0 && a->out_buf >= 2 && a->D % 4 == 0 && (a->C * a->D) % 8 == 0;
-  }
-  return a->T > 0 && !a->bot.empty() && !a->top.empty() && a->bot.back() == a->D;
 }
 
 static std::shared_ptr<DeviceModel> LoadModel(const std::string& dir, int64_t extra_rows, bool want_fp8 = false, bool host_tables = false) {
   auto m = std::make_shared<DeviceModel>();
+  const Arch& a = m->arch;
   std::string prefix;
-  if (!LoadArch(dir, &m->arch, &m->version, &prefix)) { fprintf(stderr, "[deeprec_serving] bad saved_model.json in %s\n", dir.c_str()); return nullptr; }
+  // a program's embedding buffer doubles as a GEMM operand: its row pitch C * D must obey the 16-byte rule; rows are gathered as float4 groups
+  if (!ParseArch(dir, &m->arch, &m->version, &prefix) || (a.program && (a.D % 4 || (a.C * a.D) % 8))) {
+    fprintf(stderr, "[deeprec_serving] bad saved_model.json in %s\n", dir.c_str()); return nullptr;
+  }
   dr::BundleReader r(prefix);
   if (!r.ok()) { fprintf(stderr, "[deeprec_serving] cannot open bundle %s\n", prefix.c_str()); return nullptr; }
-  if (!BuildDense(r, m->arch, &m->dense, want_fp8 && !m->arch.program)) { fprintf(stderr, "[deeprec_serving] dense parameters incomplete in %s\n", prefix.c_str()); return nullptr; }
-  if (host_tables) {                                                 // device placement optimisation: embedding layer on the CPU
-    m->host_resident = true;
-    for (int t = 0; t < m->arch.T; ++t) {
-      std::vector<int64_t> sample;
-      void* h = BuildHostTable(r, t, m->arch.D, &sample);
-      if (!h) { fprintf(stderr, "[deeprec_serving] host table %d incomplete (or libdeeprec_host.so missing)\n", t); return nullptr; }
-      m->host_tables.push_back(h);
-      m->host_sample_keys.insert(m->host_sample_keys.end(), sample.begin(), sample.end());
-      m->tables.emplace_back(new TableDev());
-      m->tables.back()->sample_keys = sample;
-    }
-    for (int c = 0; c < m->arch.C; ++c) m->col_handles.push_back(m->host_tables[(size_t)m->arch.col_table[(size_t)c]]);
-    m->path = dir;
-    return m;
-  }
+  if (!BuildDense(r, a, &m->dense, want_fp8 && !a.program)) { fprintf(stderr, "[deeprec_serving] dense parameters incomplete in %s\n", prefix.c_str()); return nullptr; }
+  m->host_resident = host_tables;                                    // device placement optimisation: embedding layer on the CPU
   std::vector<DrDeviceTable> structs;
-  for (int t = 0; t < m->arch.T; ++t) {
+  for (int t = 0; t < a.T; ++t) {
     m->tables.emplace_back(new TableDev());
-    if (!BuildTable(r, t, m->arch.D, m->tables.back().get(), extra_rows)) { fprintf(stderr, "[deeprec_serving] table %d incomplete\n", t); return nullptr; }
-    structs.push_back(m->tables.back()->t);
+    TableDev& dev = *m->tables.back();
+    TableData td;
+    if (!ReadTable(r, t, a.D, &td)) { fprintf(stderr, "[deeprec_serving] table %d incomplete\n", t); return nullptr; }
+    dev.sample_keys.assign(td.keys.begin(), td.keys.begin() + std::min<size_t>(td.keys.size(), 512));
+    if (host_tables) {
+      void* h = BuildHostTable(td, a.D);
+      if (!h) { fprintf(stderr, "[deeprec_serving] host table %d not created (libdeeprec_host.so missing?)\n", t); return nullptr; }
+      m->host_tables.push_back(h);
+    } else {
+      if (!BuildTable(td, a.D, &dev, extra_rows)) { fprintf(stderr, "[deeprec_serving] table %d not created\n", t); return nullptr; }
+      structs.push_back(dev.t);
+    }
   }
-  if (!Upload(m->structs, structs)) return nullptr;
-  { std::vector<int32_t> ct(m->arch.col_table.begin(), m->arch.col_table.end()); if (!Upload(m->col_table, ct)) return nullptr; }
+  if (host_tables) {
+    for (int c = 0; c < a.C; ++c) m->col_handles.push_back(m->host_tables[(size_t)a.col_table[(size_t)c]]);
+  } else {
+    std::vector<int32_t> ct(a.col_table.begin(), a.col_table.end());
+    if (!Upload(m->structs, structs) || !Upload(m->col_table, ct)) return nullptr;
+  }
   m->path = dir;
   return m;
 }
@@ -838,20 +617,13 @@ struct ServingModel {
   ~ServingModel() { stop = true; if (updater.joinable()) updater.join(); }
 };
 
-#pragma pack(push, 1)
-struct ReqHeader { uint32_t magic, version, batch, num_dense, num_sparse, reserved; };
-struct RespHeader { uint32_t magic, batch, status, reserved; int64_t model_version; };
-#pragma pack(pop)
-constexpr uint32_t kReqMagic = 0x51525244;   // "DRRQ"
-constexpr uint32_t kRespMagic = 0x53525244;  // "DRRS"
-
 static int Predict(ServingModel* sm, const void* in, int in_size, void** out, int* out_size, int hint) {
   auto m = std::atomic_load(&sm->model);
-  if (!m || in_size < (int)sizeof(ReqHeader)) return 500;
-  ReqHeader h; memcpy(&h, in, sizeof(h));
+  if (!m || in_size < (int)sizeof(drpb::WireReq)) return 500;
+  drpb::WireReq h; memcpy(&h, in, sizeof(h));
   const Arch& a = m->arch;
   const size_t need = sizeof(h) + (size_t)h.batch * h.num_dense * 4 + (size_t)h.num_sparse * h.batch * 8;
-  if (h.magic != kReqMagic || (int)h.num_dense != a.num_dense || (int)h.num_sparse != a.R || h.batch == 0 || (size_t)in_size < need) return 500;
+  if (h.magic != drpb::kWireReqMagic || (int)h.num_dense != a.num_dense || (int)h.num_sparse != a.R || h.batch == 0 || (size_t)in_size < need) return 500;
   uint64_t pick = sm->cfg.select_policy == 1 ? (hint >= 0 ? (uint64_t)hint : std::hash<std::thread::id>()(std::this_thread::get_id())) : sm->rr.fetch_add(1);
   const size_t ns = sm->sessions.size();
   Session* sp = sm->sessions[pick % ns].get();
@@ -893,7 +665,7 @@ static int Predict(ServingModel* sm, const void* in, int in_size, void** out, in
     sm->trace.emplace_back(line);
     if (!sm->cfg.timeline_path.empty()) { FILE* f = fopen(sm->cfg.timeline_path.c_str(), "a"); if (f) { fprintf(f, "%s\n", line); fclose(f); } }
   }
-  RespHeader rh{kRespMagic, h.batch, 200, (uint32_t)(a.n_out > 1 ? a.n_out : 0), m->version};        // reserved = probabilities per row (0: one)
+  drpb::WireResp rh{drpb::kWireRespMagic, h.batch, 200, (uint32_t)(a.n_out > 1 ? a.n_out : 0), m->version};        // reserved = probabilities per row (0: one)
   *out_size = (int)(sizeof(rh) + probs.size() * 4);
   *out = malloc(*out_size);
   memcpy(*out, &rh, sizeof(rh)); memcpy(static_cast<uint8_t*>(*out) + sizeof(rh), probs.data(), probs.size() * 4);
@@ -917,11 +689,9 @@ static bool ApplyDelta(ServingModel* sm, const std::string& prefix, int64_t vers
   }
   for (int t = 0; t < m->arch.T; ++t) {
     std::vector<int64_t> keys; std::vector<float> vals;
-    const std::string base = "table/" + std::to_string(t);
-    if (!ReadVec(r, base + "-sparse_incr_keys", &keys) || keys.empty()) continue;
-    if (!ReadVec(r, base + "-sparse_incr_values", &vals)) return false;
+    if (!ReadDeltaRows(r, t, m->arch.D, &keys, &vals)) return false;
+    if (keys.empty()) continue;
     if (m->host_resident) {                                          // host engine: copy-on-write import, readers never see a torn row
-      if (vals.size() != keys.size() * (size_t)m->arch.D) return false;
       HostApi::Get().import_cow(m->host_tables[(size_t)t], keys.data(), vals.data(), m->arch.D, (int64_t)keys.size());
       continue;
     }
@@ -939,9 +709,7 @@ static bool ApplyDelta(ServingModel* sm, const std::string& prefix, int64_t vers
     sm->retired.push_back({t, retired, (int64_t)keys.size()});
   }
   std::shared_ptr<DenseParams> dp;
-  const bool has_dense = m->arch.program ? [&] { for (auto& op : m->arch.ops) if (op.kind == P_LINEAR) return r.Find("prog/" + op.name + "/kernel") != nullptr; return false; }()
-                                         : r.Find("dense/logits/kernel") != nullptr;
-  if (has_dense && BuildDense(r, m->arch, &dp, sm->cfg.fp8)) {
+  if (HasDenseBlock(r, m->arch) && BuildDense(r, m->arch, &dp, sm->cfg.fp8)) {
     if (sm->cfg.fp8 && !m->arch.program) {       // delta updates keep the calibrated activation scales of the serving model (no warm-up on deltas)
       auto old = std::atomic_load(&m->dense);
       dp->act = old->act;
@@ -960,10 +728,10 @@ static int FillWarmupBatch(ServingModel* sm, const DeviceModel& m, Session& s) {
   const Arch& a = m.arch;
   int B = std::min(256, s.max_batch);
   std::string raw;
-  if (!sm->cfg.warmup_file_name.empty() && ReadFile(sm->cfg.warmup_file_name, &raw) && raw.size() >= sizeof(ReqHeader)) {
-    ReqHeader h; memcpy(&h, raw.data(), sizeof(h));
+  if (!sm->cfg.warmup_file_name.empty() && drjson::ReadFile(sm->cfg.warmup_file_name, &raw) && raw.size() >= sizeof(drpb::WireReq)) {
+    drpb::WireReq h; memcpy(&h, raw.data(), sizeof(h));
     const size_t need = sizeof(h) + (size_t)h.batch * h.num_dense * 4 + (size_t)h.num_sparse * h.batch * 8;
-    if (h.magic == kReqMagic && (int)h.num_dense == a.num_dense && (int)h.num_sparse == a.R && h.batch > 0 && raw.size() >= need) {
+    if (h.magic == drpb::kWireReqMagic && (int)h.num_dense == a.num_dense && (int)h.num_sparse == a.R && h.batch > 0 && raw.size() >= need) {
       B = std::min<int>(h.batch, s.max_batch);
       const float* d = reinterpret_cast<const float*>(raw.data() + sizeof(h));
       const int64_t* ids = reinterpret_cast<const int64_t*>(raw.data() + sizeof(h) + (size_t)h.batch * h.num_dense * 4);
@@ -1002,54 +770,35 @@ static bool WarmUp(ServingModel* sm, const std::shared_ptr<DeviceModel>& m, cons
   return true;
 }
 
-// version file: <dir>/serving_versions.json = {"full": {"version": V, "dir": "..."}, "deltas": [{"version": v, "prefix": "..."}]}
 static void UpdaterLoop(ServingModel* sm) {
-  const std::string vf = (sm->cfg.checkpoint_dir.empty() ? sm->cfg.savedmodel_dir : sm->cfg.checkpoint_dir) + "/serving_versions.json";
   int bad = 0;
-  while (!sm->stop) {
-    for (int i = 0; i < sm->cfg.update_interval_ms / 20 && !sm->stop; ++i) std::this_thread::sleep_for(std::chrono::milliseconds(20));
-    std::string txt; JVal j;
-    if (!ReadFile(vf, &txt) || !ParseJson(txt, &j)) continue;
+  auto load_full = [&](int64_t v, const std::string& dir) {
     auto cur = std::atomic_load(&sm->model);
-    if (auto* f = j.get("full")) {
-      int64_t v = (int64_t)f->n("version", -1); std::string dir = f->s("dir", "");
-      if (cur && v > cur->version && !dir.empty()) {
-        cudaSetDevice(sm->cfg.gpu_id);
-        auto nm = LoadModel(dir, sm->cfg.extra_rows, sm->cfg.fp8, sm->cfg.host_tables);
-        if (!nm) { if (++bad > 3) fprintf(stderr, "[deeprec_serving] skipping invalid model version %lld\n", (long long)v); continue; }
-        bad = 0;
-        // The sessions' device / pinned buffers were sized from the architecture they were initialised with (Session::Init): a version with
-        // more tables, a larger D, more dense columns or wider layers would overflow them.  Such a version is rejected (logged once) -- the
-        // reference would build a fresh SessionGroup (serving/processor/serving/model_instance.cc:406-427); restart the processor for it.
-        {
-          const Arch& o = cur->arch; const Arch& n = nm->arch;
-          if (n.num_dense != o.num_dense || n.T != o.T || n.D != o.D || n.bot != o.bot || n.top != o.top || n.Zp != o.Zp || n.program != o.program || n.R != o.R || n.C != o.C || n.n_out != o.n_out) {
-            if (sm->rejected_version != v) {
-              fprintf(stderr, "[deeprec_serving] model version %lld changes the architecture (tables %d->%d, D %d->%d, dense %d->%d): rejected, sessions keep serving version %lld\n",
-                      (long long)v, o.T, n.T, o.D, n.D, o.num_dense, n.num_dense, (long long)cur->version);
-              sm->rejected_version = v;
-            }
-            continue;
-          }
-        }
-        if (!WarmUp(sm, nm)) continue;
-        std::atomic_store(&sm->model, nm);          // requests in flight keep the old model alive through their shared_ptr
-        sm->retired.clear();
-        sm->delta_version = -1;
-        sm->full_updates++;
-        continue;
+    cudaSetDevice(sm->cfg.gpu_id);
+    auto nm = LoadModel(dir, sm->cfg.extra_rows, sm->cfg.fp8, sm->cfg.host_tables);
+    if (!nm) { if (++bad > 3) fprintf(stderr, "[deeprec_serving] skipping invalid model version %lld\n", (long long)v); return; }
+    bad = 0;
+    // The sessions' device / pinned buffers were sized from the architecture they were initialised with (Session::Init): a version with
+    // more tables, a larger D, more dense columns or wider layers would overflow them.  Such a version is rejected (logged once) -- the
+    // reference would build a fresh SessionGroup (serving/processor/serving/model_instance.cc:406-427); restart the processor for it.
+    const Arch& o = cur->arch; const Arch& n = nm->arch;
+    if (n.num_dense != o.num_dense || n.T != o.T || n.D != o.D || n.bot != o.bot || n.top != o.top || n.Zp != o.Zp || n.program != o.program || n.R != o.R || n.C != o.C || n.n_out != o.n_out) {
+      if (sm->rejected_version != v) {
+        fprintf(stderr, "[deeprec_serving] model version %lld changes the architecture (tables %d->%d, D %d->%d, dense %d->%d): rejected, sessions keep serving version %lld\n",
+                (long long)v, o.T, n.T, o.D, n.D, o.num_dense, n.num_dense, (long long)cur->version);
+        sm->rejected_version = v;
       }
+      return;
     }
-    if (auto* d = j.get("deltas")) {
-      cur = std::atomic_load(&sm->model);
-      for (auto& e : d->arr) {
-        int64_t v = (int64_t)e.n("version", -1), base = (int64_t)e.n("base", -1);
-        if (cur && base == cur->version && v > std::max<int64_t>(cur->version, sm->delta_version.load())) ApplyDelta(sm, e.s("prefix", ""), v);
-      }
-    }
-  }
+    if (!WarmUp(sm, nm)) return;
+    std::atomic_store(&sm->model, nm);          // requests in flight keep the old model alive through their shared_ptr
+    sm->retired.clear();
+    sm->delta_version = -1;
+    sm->full_updates++;
+  };
+  RunUpdater(sm->cfg.checkpoint_dir.empty() ? sm->cfg.savedmodel_dir : sm->cfg.checkpoint_dir, sm->cfg.update_interval_ms, sm->stop, sm->model, sm->delta_version,
+             load_full, [&](int64_t v, const std::string& prefix) { ApplyDelta(sm, prefix, v); });
 }
-
 
 // protobuf PredictRequest (reference predict.proto wire format) -> compact request -> Predict -> PredictResponse
 static int PredictProto(ServingModel* sm, const void* in, int in_size, void** out, int* out_size, int hint) {
@@ -1082,8 +831,8 @@ extern "C" {
 void* initialize(const char* model_entry, const char* model_config, int* state) {
   using namespace serve;
   auto* sm = new ServingModel();
-  JVal j;
-  if (model_config && *model_config && !ParseJson(model_config, &j)) { *state = -1; delete sm; return nullptr; }
+  drjson::JVal j;
+  if (model_config && *model_config && !drjson::ParseJson(model_config, &j)) { *state = -1; delete sm; return nullptr; }
   Config& c = sm->cfg;
   sm->compat = drcfg::ParseCompat(j, "deeprec_cuda_serving");                 // every reference ModelConfig key classified (csrc/common/model_config.h)
   if (!sm->compat.error.empty()) { *state = -1; delete sm; return nullptr; }

@@ -42,6 +42,7 @@
 #include "../common/mini_json.h"
 #include "../common/model_config.h"
 #include "../common/predict_pb.h"
+#include "../common/saved_model.h"
 
 extern "C" {
 void* dr_host_ev_create(const DrEvConfig* cfg);
@@ -63,6 +64,7 @@ int64_t dr_redis_get(void* h, const char* key, void* out, int64_t cap);
 
 namespace cpusrv {
 using drjson::JVal;
+using namespace drsm;
 
 struct Config {
   int session_num = 2, max_batch = 4096, select_policy = 0 /*0 RR, 1 MOD*/, update_interval_ms = 1000, intra_threads = 0;
@@ -87,30 +89,6 @@ struct Config {
   bool remote = false; std::string redis_host = "127.0.0.1", redis_password, redis_prefix = "dlrm"; int redis_port = 6379, redis_db = 0, redis_timeout_ms = 2000;
 };
 
-// Op program (saved_model.json "arch": "program", written by serving/export.py::export_saved_model_program): the inference graph of a
-// Criteo-style model other than DLRM as a list of ops over [B, width] buffers; buffer 0 = dense inputs, buffer 1 = embeddings [B, T * D].
-// Sequence models (DIN): the request's id rows are COLUMNS, several of which may read the same table (`col_table`: target item + L history
-// positions -> the item table); valid_mask / seq_zip / seq_mask / seq_sum / din_attention / prelu are the ops their heads need.
-enum POpKind { P_CONCAT, P_LINEAR, P_AFFINE, P_FM, P_CROSS, P_MUL_ADD, P_ADD, P_LAYERNORM, P_MUL, P_SLICE,
-               P_VALID_MASK, P_SEQ_ZIP, P_SEQ_MASK, P_SEQ_SUM, P_DIN_ATT, P_PRELU, P_SOFTMAX, P_COSINE, P_TILE, P_GRU, P_SEQ_LAST, P_MHA, P_SEQ_MEAN, P_NUM_OPS };
-// rows1: sample-aware graph compression (serving/export.py::compress_sample_aware) -- the op depends on user-side features only, which are
-// identical for every candidate row of a ranking request: it runs at batch 1 on row 0 of its inputs; a TILE op broadcasts row 0 to the batch
-// where a per-candidate op consumes the result (reference: python/graph_optimizer/sample_awared_graph_compression.py:26).
-// len on LINEAR / LAYERNORM: the op is applied at each of `len` positions of a [B, len * w] sequence buffer (DIEN / BST); mode: din_attention output
-// (0 = weighted sum of the keys, 1 = the softmax weights); heads: mha
-struct POp { int kind = 0, out = 0; std::vector<int> in; bool relu = false, rows1 = false; float eps = 1e-5f; int start = 0, len = 0, mode = 0, heads = 1; std::string name; };
-struct Arch {
-  int num_dense = 13, T = 0, D = 16; std::vector<int> bot, top; float bn_eps = 1e-3f; int inter = 0;
-  bool program = false; std::vector<POp> ops; int nbuf = 2, out_buf = -1; std::string model_name = "dlrm";
-  // requests carry R id rows; lookup column c reads request row id_map[c] (identity unless several columns share a feature, e.g. the wide
-  // and the deep table of one Wide&Deep column) from table col_table[c] (identity unless several columns share a TABLE, e.g. DIN's target
-  // item and its L history positions).  C == T and col_table == identity for every model exported before col_table existed.
-  int R = 0, C = 0; std::vector<int> id_map, col_table;
-  // multi-task programs: the output buffer is [B, n_out] logits, the response carries n_out probabilities per row (sample-major)
-  int n_out = 1; std::vector<std::string> out_names;
-};
-static int pad8(int n) { return (n + 7) / 8 * 8; }
-
 // wt: [K][N] row-major (the batch-1 / tail path streams whole rows); wp: the same weights packed panel-major for the tiled kernels --
 // panel p = columns [32p, 32p + 32) stored as K x 32 contiguous floats (zero-padded past N), so a tile's k-loop reads consecutive
 // cache lines instead of one line every N floats (the unpacked layout defeated the hardware prefetchers: 2 KB strides, a page every 2 steps)
@@ -124,7 +102,15 @@ struct Layer {
       wp[((size_t)p * K + k) * kPanel + j] = wt[(size_t)k * N + p * kPanel + j];
   }
 };
-struct PData { Layer L; std::vector<float> v0, v1; std::vector<std::vector<float>> att; int H1 = 0, H2 = 0; Layer Lq, L1, L2; Layer Gih, Ghh; };   // weights of one program op (linear | affine scale, shift | cross w, b | prelu alpha | din_attention W1 b1 W2 b2 w3 b3)
+// Linear from an exported W [N, K] (row stride ldw): transposed to wt [K][N] and packed
+static Layer Transposed(int N, int K, const float* W, size_t ldw, std::vector<float> bias) {
+  Layer L; L.N = N; L.K = K; L.bias = std::move(bias); L.wt.resize((size_t)K * N);
+  for (int n = 0; n < N; ++n) for (int k = 0; k < K; ++k) L.wt[(size_t)k * N + n] = W[(size_t)n * ldw + k];
+  L.Pack();
+  return L;
+}
+// weights of one program op: L linear, Gih / Ghh gru, Lq / L1 / L2 din_attention (att: its W1 b1 W2 b2 w3 b3); v0, v1, H1, H2 as in OpTensors
+struct PData { Layer L; std::vector<float> v0, v1; std::vector<std::vector<float>> att; int H1 = 0, H2 = 0; Layer Lq, L1, L2; Layer Gih, Ghh; };
 struct Dense {
   std::vector<Layer> bot, top; std::vector<float> last_scale, last_shift, head_w; float head_b = 0.f;
   std::vector<PData> pdata; std::vector<int> width;                       // program models: per-op weights, per-buffer widths
@@ -184,252 +170,71 @@ struct Model {
   ~Model() { for (void* t : tables) if (t) dr_host_ev_destroy(t); }
 };
 
-template <typename T> static bool ReadVec(dr::BundleReader& r, const std::string& name, std::vector<T>* out) {
-  if constexpr (std::is_same<T, float>::value) return dr::ReadAsFloat(r, name, out);       // bf16 / f16 / int8(+scale) tensors of a converted model
-  auto* e = r.Find(name); if (!e) return false;
-  out->resize((size_t)e->nbytes / sizeof(T));
-  return r.Read(*e, out->data(), 1) == 0;
-}
-
-static bool LoadArch(const std::string& dir, Arch* a, int64_t* version, std::string* prefix) {
-  std::string txt; JVal j;
-  if (!drjson::ReadFile(dir + "/saved_model.json", &txt) || !drjson::ParseJson(txt, &j)) return false;
-  a->num_dense = (int)j.n("num_dense", 13); a->D = (int)j.n("embedding_dim", 16); a->bn_eps = (float)j.n("bn_eps", 1e-3);
-  a->T = (int)j.n("num_tables", 0);
-  if (auto* b = j.get("mlp_bot")) for (auto& v : b->arr) a->bot.push_back((int)v.num);
-  if (auto* b = j.get("mlp_top")) for (auto& v : b->arr) a->top.push_back((int)v.num);
-  const int F = a->T + 1; a->inter = a->D + F * (F - 1) / 2;
-  *version = (int64_t)j.n("version", 0);
-  *prefix = dir + "/" + j.s("variables", "variables/variables");
-  a->model_name = j.s("model", "dlrm");
-  a->C = a->T;
-  if (auto* ct = j.get("col_table")) {
-    if (ct->t != JVal::ARR || ct->arr.empty()) return false;
-    a->C = (int)ct->arr.size();
-    for (auto& v : ct->arr) a->col_table.push_back((int)v.num);
-  } else for (int t = 0; t < a->T; ++t) a->col_table.push_back(t);
-  for (int v : a->col_table) if (v < 0 || v >= a->T) return false;
-  a->R = (int)j.n("num_id_rows", a->C);
-  a->id_map.resize((size_t)std::max(0, a->C));
-  for (int c = 0; c < a->C; ++c) a->id_map[(size_t)c] = c;
-  if (auto* im = j.get("id_map")) {
-    if (im->t != JVal::ARR || (int)im->arr.size() != a->C) return false;
-    for (int c = 0; c < a->C; ++c) a->id_map[(size_t)c] = (int)im->arr[(size_t)c].num;
-  }
-  for (int v : a->id_map) if (v < 0 || v >= a->R) return false;
-  if (a->R <= 0) return false;
-  if (j.s("arch", "") == "program") {
-    a->program = true;
-    std::vector<std::string> names = {"dense", "emb"};
-    auto id_of = [&](const std::string& n) { for (size_t i = 0; i < names.size(); ++i) if (names[i] == n) return (int)i; return -1; };
-    static const char* kNames[] = {"concat", "linear", "affine", "fm", "cross", "mul_add", "add", "layernorm", "mul", "slice",
-                                   "valid_mask", "seq_zip", "seq_mask", "seq_sum", "din_attention", "prelu", "softmax", "cosine", "tile", "gru", "seq_last", "mha", "seq_mean"};
-    const JVal* pr = j.get("program");
-    if (!pr || pr->t != JVal::ARR) return false;
-    std::vector<bool> rows1_buf(2, false);
-    for (const JVal& o : pr->arr) {
-      POp op; op.name = o.s("out", ""); op.relu = o.n("relu", 0) != 0; op.eps = (float)o.n("eps", 1e-5); op.kind = -1;
-      op.start = (int)o.n("start", 0); op.len = (int)o.n("len", 0); op.rows1 = o.n("rows1", 0) != 0; op.mode = (int)o.n("mode", 0); op.heads = (int)o.n("heads", 1);
-      const std::string kind = o.s("op", "");
-      for (int k = 0; k < P_NUM_OPS; ++k) if (kind == kNames[k]) op.kind = k;
-      const JVal* in = o.get("in");
-      if (op.kind < 0 || op.name.empty() || !in || id_of(op.name) >= 0) return false;
-      for (const JVal& v : in->arr) { const int id = id_of(v.str); if (id < 0) return false; op.in.push_back(id); }    // inputs must already exist
-      static const int kArity[] = {-1, 1, 1, 1, 2, 3, 2, 1, 2, 1, 1, 2, 2, 1, 3, 1, 1, 2, 1, 1, 2, 2, 2};
-      if ((kArity[op.kind] >= 0 && (int)op.in.size() != kArity[op.kind]) || op.in.empty()) return false;
-      // a buffer computed at batch 1 holds one valid row: only rows1 ops and TILE may read it
-      if (op.kind == P_TILE && op.rows1) return false;
-      if (!op.rows1 && op.kind != P_TILE) for (int id : op.in) if (id < (int)rows1_buf.size() && rows1_buf[(size_t)id]) return false;
-      op.out = (int)names.size(); names.push_back(op.name);
-      rows1_buf.resize(names.size(), false); rows1_buf[(size_t)op.out] = op.rows1;
-      a->ops.push_back(std::move(op));
-    }
-    a->nbuf = (int)names.size();
-    a->out_buf = id_of(j.s("output", ""));
-    if (a->out_buf >= 0 && a->out_buf < (int)rows1_buf.size() && rows1_buf[(size_t)a->out_buf]) return false;
-    a->n_out = (int)j.n("num_outputs", 1);
-    if (auto* on = j.get("output_names")) for (auto& v : on->arr) a->out_names.push_back(v.str);
-    return a->T > 0 && a->out_buf >= 2 && a->n_out >= 1 && a->n_out <= 16;
-  }
-  return a->T > 0 && !a->bot.empty() && !a->top.empty() && a->bot.back() == a->D;
-}
-
-// weights + buffer widths of a program model; every shape is checked against the widths implied by the op list
+// program weights in the layout of the CPU kernels: Linear / GRU weights transposed and packed, the DIN attention's first layer split
 static bool BuildProgram(dr::BundleReader& r, const Arch& a, std::shared_ptr<Dense>* out) {
+  ProgramData p;
+  if (!ReadProgram(r, a, &p)) return false;
   auto dp = std::make_shared<Dense>();
-  dp->width.assign((size_t)a.nbuf, 0); dp->width[0] = a.num_dense; dp->width[1] = a.C * a.D;
   dp->pdata.resize(a.ops.size());
   for (size_t i = 0; i < a.ops.size(); ++i) {
-    const POp& op = a.ops[i]; PData& d = dp->pdata[i];
-    const int w0 = dp->width[(size_t)op.in[0]];
-    int w = w0;
-    const std::string base = "prog/" + op.name + "/";
-    switch (op.kind) {
-      case P_CONCAT: w = 0; for (int b : op.in) w += dp->width[(size_t)b]; break;
-      case P_LINEAR: {                                               // len > 0: the same Linear at each of len positions of a [B, len * K] sequence
-        std::vector<float> W, b;
-        const int S = op.len > 0 ? op.len : 1;
-        if (w0 % S) return false;
-        const int K = w0 / S;
-        if (!ReadVec(r, base + "kernel", &W) || !ReadVec(r, base + "bias", &b) || b.empty() || W.size() != b.size() * (size_t)K) return false;
-        d.L.N = (int)b.size(); d.L.K = K; d.L.bias = b; d.L.wt.resize(W.size());
-        for (int n = 0; n < d.L.N; ++n) for (int k = 0; k < K; ++k) d.L.wt[(size_t)k * d.L.N + n] = W[(size_t)n * K + k];
-        d.L.Pack();
-        w = d.L.N * S; break;
-      }
-      case P_LAYERNORM: {                                            // len > 0: per position of a [B, len * w] sequence
-        const int S = op.len > 0 ? op.len : 1;
-        if (w0 % S || !ReadVec(r, base + "scale", &d.v0) || !ReadVec(r, base + "shift", &d.v1) || (int)d.v0.size() != w0 / S || (int)d.v1.size() != w0 / S) return false;
-        break;
-      }
-      case P_AFFINE: if (!ReadVec(r, base + "scale", &d.v0) || !ReadVec(r, base + "shift", &d.v1) || (int)d.v0.size() != w0 || (int)d.v1.size() != w0) return false; break;
-      case P_FM: if (op.in[0] != 1) return false; w = a.D; break;
-      case P_CROSS: if (!ReadVec(r, base + "w", &d.v0) || !ReadVec(r, base + "b", &d.v1) || (int)d.v0.size() != w0 || (int)d.v1.size() != w0 || dp->width[(size_t)op.in[1]] != w0) return false; break;
-      case P_MUL_ADD: if (dp->width[(size_t)op.in[1]] != w0 || dp->width[(size_t)op.in[2]] != w0) return false; break;
-      case P_MUL:
-      case P_ADD: if (dp->width[(size_t)op.in[1]] != w0) return false; break;
-      case P_SLICE: if (op.start < 0 || op.len <= 0 || op.start + op.len > w0) return false; w = op.len; break;
-      case P_VALID_MASK: if (op.start < 0 || op.len <= 0 || op.start + op.len > a.C) return false; w = op.len; break;      // [B, len]: 1 where the id of column start + l is >= 0
-      case P_SEQ_ZIP: {                                              // a [B, L * Wa], b [B, L * Wb] -> [B, L * (Wa + Wb)], position-wise concat
-        const int wb = dp->width[(size_t)op.in[1]];
-        if (op.len <= 0 || w0 % op.len || wb % op.len) return false;
-        w = w0 + wb; break;
-      }
-      case P_SEQ_MASK: if (op.len <= 0 || w0 % op.len || dp->width[(size_t)op.in[1]] != op.len) return false; break;       // x [B, L * W] * mask [B, L]
-      case P_SEQ_SUM: if (op.len <= 0 || w0 % op.len) return false; w = w0 / op.len; break;                                 // sum over the L positions
-      case P_PRELU: if (!ReadVec(r, base + "alpha", &d.v0) || (int)d.v0.size() != w0) return false; break;
-      case P_SOFTMAX: break;                                           // row-wise softmax (mixture-of-experts gates)
-      case P_TILE: break;                                              // row 0 of a once-per-request buffer -> every row of the batch
-      case P_GRU: {                                                    // x [B, L * I] -> every hidden state [B, L * H] (PyTorch gate order r, z, n; h0 = 0)
-        std::vector<float> wih, whh, bih, bhh;
-        if (op.len <= 0 || w0 % op.len || !ReadVec(r, base + "w_ih", &wih) || !ReadVec(r, base + "w_hh", &whh) || !ReadVec(r, base + "b_ih", &bih) || !ReadVec(r, base + "b_hh", &bhh)) return false;
-        const int I = w0 / op.len, H3 = (int)bih.size(), H = H3 / 3;
-        if (H <= 0 || H3 != 3 * H || (int)bhh.size() != H3 || (int)wih.size() != H3 * I || (int)whh.size() != H3 * H) return false;
-        d.Gih.N = H3; d.Gih.K = I; d.Gih.bias = bih; d.Gih.wt.resize(wih.size());
-        for (int n = 0; n < H3; ++n) for (int k = 0; k < I; ++k) d.Gih.wt[(size_t)k * H3 + n] = wih[(size_t)n * I + k];
-        d.Ghh.N = H3; d.Ghh.K = H; d.Ghh.bias = bhh; d.Ghh.wt.resize(whh.size());
-        for (int n = 0; n < H3; ++n) for (int k = 0; k < H; ++k) d.Ghh.wt[(size_t)k * H3 + n] = whh[(size_t)n * H + k];
-        d.Gih.Pack(); d.Ghh.Pack(); d.H1 = H;
-        w = op.len * H; break;
-      }
-      case P_SEQ_LAST: if (op.len <= 0 || w0 % op.len || dp->width[(size_t)op.in[1]] != op.len) return false; w = w0 / op.len; break;
-      case P_SEQ_MEAN: if (op.len <= 0 || w0 % op.len || dp->width[(size_t)op.in[1]] != op.len) return false; w = w0 / op.len; break;
-      case P_MHA: {                                                    // qkv [B, S * 3E] (per position [q | k | v]), valid [B, S] -> [B, S * E]
-        if (op.len <= 0 || w0 % (3 * op.len) || dp->width[(size_t)op.in[1]] != op.len) return false;
-        const int E = w0 / (3 * op.len);
-        if (op.heads <= 0 || E % op.heads) return false;
-        w = op.len * E; break;
-      }
-      case P_COSINE: if (dp->width[(size_t)op.in[1]] != w0) return false; w = 1; break;     // cosine similarity of two [B, W] towers -> [B, 1]
-      case P_DIN_ATT: {                                              // q [B, W], k [B, L * W], mask [B, L] -> [B, W]
-        const int wk = dp->width[(size_t)op.in[1]], L = dp->width[(size_t)op.in[2]];
-        if (L <= 0 || wk != L * w0 || op.mode < 0 || op.mode > 1) return false;
-        if (op.mode == 1) w = L;                                       // the softmax weights themselves (DIEN)
-        d.att.resize(6);
-        static const char* kT[] = {"w1", "b1", "w2", "b2", "w3", "b3"};
-        for (int i2 = 0; i2 < 6; ++i2) if (!ReadVec(r, base + kT[i2], &d.att[(size_t)i2])) return false;
-        d.H1 = (int)d.att[1].size(); d.H2 = (int)d.att[3].size();
-        if (d.H1 <= 0 || d.H2 <= 0 || (int)d.att[0].size() != d.H1 * 4 * w0 || (int)d.att[2].size() != d.H2 * d.H1 || (int)d.att[4].size() != d.H2 || d.att[5].size() != 1) return false;
-        {
-          // first layer split (the algebra of csrc/cuda/attention_kernels.cu): W1 [q | k | q - k | q * k] = (Wa + Wc) q + (Wb - Wc) k + Wd (q * k);
-          // the q term is one batched GEMM per request, the per-position work is ONE [rows, 2W] x [2W, H1] GEMM over [k | q * k]
-          const int W = w0, H1 = d.H1, H2 = d.H2; const float* W1 = d.att[0].data(); const float* W2 = d.att[2].data();
-          d.Lq.N = H1; d.Lq.K = W; d.Lq.bias = d.att[1]; d.Lq.wt.assign((size_t)W * H1, 0.f);
-          d.L1.N = H1; d.L1.K = 2 * W; d.L1.bias.assign((size_t)H1, 0.f); d.L1.wt.assign((size_t)2 * W * H1, 0.f);
-          for (int h = 0; h < H1; ++h) for (int c = 0; c < W; ++c) {
-            const float wa = W1[(size_t)h * 4 * W + c], wb = W1[(size_t)h * 4 * W + W + c], wc = W1[(size_t)h * 4 * W + 2 * W + c], wd = W1[(size_t)h * 4 * W + 3 * W + c];
-            d.Lq.wt[(size_t)c * H1 + h] = wa + wc; d.L1.wt[(size_t)c * H1 + h] = wb - wc; d.L1.wt[(size_t)(W + c) * H1 + h] = wd;
-          }
-          d.L2.N = H2; d.L2.K = H1; d.L2.bias = d.att[3]; d.L2.wt.assign((size_t)H1 * H2, 0.f);
-          for (int m2 = 0; m2 < H2; ++m2) for (int h = 0; h < H1; ++h) d.L2.wt[(size_t)h * H2 + m2] = W2[(size_t)m2 * H1 + h];
-          d.Lq.Pack(); d.L1.Pack(); d.L2.Pack();
+    OpTensors& t = p.ops[i]; PData& d = dp->pdata[i];
+    switch (a.ops[i].kind) {
+      case P_LINEAR: d.L = Transposed(t.N, t.K, t.W.data(), (size_t)t.K, t.b); break;
+      case P_GRU: d.Gih = Transposed(t.N, t.K, t.W.data(), (size_t)t.K, t.b); d.Ghh = Transposed(t.N, t.H1, t.v0.data(), (size_t)t.H1, t.v1); break;
+      case P_DIN_ATT: {
+        // first layer split (the algebra of csrc/cuda/attention_kernels.cu): W1 [q | k | q - k | q * k] = (Wa + Wc) q + (Wb - Wc) k + Wd (q * k);
+        // the q term is one batched GEMM per request, the per-position work is ONE [rows, 2W] x [2W, H1] GEMM over [k | q * k]
+        const int W = p.width[(size_t)a.ops[i].in[0]], H1 = t.H1; const float* W1 = t.att[0].data();
+        d.Lq.N = H1; d.Lq.K = W; d.Lq.bias = t.att[1]; d.Lq.wt.assign((size_t)W * H1, 0.f);
+        d.L1.N = H1; d.L1.K = 2 * W; d.L1.bias.assign((size_t)H1, 0.f); d.L1.wt.assign((size_t)2 * W * H1, 0.f);
+        for (int h = 0; h < H1; ++h) for (int c = 0; c < W; ++c) {
+          const float wa = W1[(size_t)h * 4 * W + c], wb = W1[(size_t)h * 4 * W + W + c], wc = W1[(size_t)h * 4 * W + 2 * W + c], wd = W1[(size_t)h * 4 * W + 3 * W + c];
+          d.Lq.wt[(size_t)c * H1 + h] = wa + wc; d.L1.wt[(size_t)c * H1 + h] = wb - wc; d.L1.wt[(size_t)(W + c) * H1 + h] = wd;
         }
+        d.Lq.Pack(); d.L1.Pack();
+        d.L2 = Transposed(t.H2, H1, t.att[2].data(), (size_t)H1, t.att[3]);
         break;
       }
-      default: return false;
+      default: break;
     }
-    if (w <= 0) return false;
-    dp->width[(size_t)op.out] = w;
+    d.v0 = std::move(t.v0); d.v1 = std::move(t.v1); d.att = std::move(t.att); d.H1 = t.H1; d.H2 = t.H2;
   }
-  if (dp->width[(size_t)a.out_buf] < a.n_out) return false;            // the output buffer holds n_out logits per row
+  dp->width = std::move(p.width);
   dp->plan = std::make_shared<ProgPlan>(a.ops, a.nbuf);
   *out = dp;
   return true;
 }
 
-// BatchNorm (moving statistics) of layer l-1 folded into Linear l:  W' = W diag(s), b' = b + W t
-static bool BuildProgram(dr::BundleReader& r, const Arch& a, std::shared_ptr<Dense>* out);
+// DLRM: the BatchNorm-folded layers transposed and packed
 static bool BuildDense(dr::BundleReader& r, const Arch& a, std::shared_ptr<Dense>* out) {
   if (a.program) return BuildProgram(r, a, out);
+  DlrmDense t;
+  if (!ReadDlrmDense(r, a, &t)) return false;
   auto dp = std::make_shared<Dense>();
-  std::vector<float> s_prev, t_prev;
-  int k = a.num_dense;
-  for (size_t l = 0; l < a.bot.size(); ++l) {
-    const std::string nm = "mlp_bot_" + std::to_string(l);
-    const int N = a.bot[l], Kp = pad8(k);
-    std::vector<float> W, b, gamma, beta, mean, var;
-    if (!ReadVec(r, "dense/" + nm + "/kernel", &W) || !ReadVec(r, "dense/" + nm + "/bias", &b) || !ReadVec(r, "dense/" + nm + "/bn_gamma", &gamma) ||
-        !ReadVec(r, "dense/" + nm + "/bn_beta", &beta) || !ReadVec(r, "bn/" + nm + "/moving_mean", &mean) || !ReadVec(r, "bn/" + nm + "/moving_variance", &var)) return false;
-    if ((int)W.size() != N * Kp || (int)b.size() != N) return false;
-    Layer L; L.N = N; L.K = k; L.wt.assign((size_t)k * N, 0.f); L.bias.resize(N);
-    for (int n = 0; n < N; ++n) {
-      double acc = b[n];
-      for (int kk = 0; kk < k; ++kk) {
-        float w = W[(size_t)n * Kp + kk];
-        if (l > 0) { acc += (double)w * t_prev[kk]; w *= s_prev[kk]; }
-        L.wt[(size_t)kk * N + n] = w;
-      }
-      L.bias[n] = (float)acc;
-    }
-    L.Pack();
-    dp->bot.push_back(std::move(L));
-    s_prev.assign(N, 0.f); t_prev.assign(N, 0.f);
-    for (int n = 0; n < N; ++n) { const float rs = 1.0f / std::sqrt(var[n] + a.bn_eps); s_prev[n] = gamma[n] * rs; t_prev[n] = beta[n] - mean[n] * s_prev[n]; }
-    k = N;
-  }
-  dp->last_scale = s_prev; dp->last_shift = t_prev;
-  k = a.inter;
-  for (size_t l = 0; l < a.top.size(); ++l) {
-    const std::string nm = "mlp_top_" + std::to_string(l);
-    const int N = a.top[l], Kp = pad8(k);
-    std::vector<float> W, b;
-    if (!ReadVec(r, "dense/" + nm + "/kernel", &W) || !ReadVec(r, "dense/" + nm + "/bias", &b) || (int)W.size() != N * Kp || (int)b.size() != N) return false;
-    Layer L; L.N = N; L.K = k; L.wt.resize((size_t)k * N); L.bias = b;
-    for (int n = 0; n < N; ++n) for (int kk = 0; kk < k; ++kk) L.wt[(size_t)kk * N + n] = W[(size_t)n * Kp + kk];
-    L.Pack();
-    dp->top.push_back(std::move(L));
-    k = N;
-  }
-  std::vector<float> hb;
-  if (!ReadVec(r, "dense/logits/kernel", &dp->head_w) || !ReadVec(r, "dense/logits/bias", &hb) || hb.empty() || (int)dp->head_w.size() < k) return false;
-  dp->head_b = hb[0];
+  for (const DenseLayer& L : t.bot) dp->bot.push_back(Transposed(L.N, L.K, L.W.data(), (size_t)L.Kp, L.b));
+  for (const DenseLayer& L : t.top) dp->top.push_back(Transposed(L.N, L.K, L.W.data(), (size_t)L.Kp, L.b));
+  dp->last_scale = std::move(t.last_scale); dp->last_shift = std::move(t.last_shift); dp->head_w = std::move(t.head_w); dp->head_b = t.head_b[0];
   *out = dp;
   return true;
 }
 
-static void* BuildTable(dr::BundleReader& r, int t, int D, std::vector<int64_t>* sample) {
-  const std::string base = "table/" + std::to_string(t);
-  std::vector<int64_t> keys, freqs, vers; std::vector<float> vals, def;
-  if (!ReadVec(r, base + "-keys", &keys) || !ReadVec(r, base + "-values", &vals) || !ReadVec(r, base + "-default", &def)) return nullptr;
-  ReadVec(r, base + "-freqs", &freqs); ReadVec(r, base + "-versions", &vers);
-  if (def.empty() || def.size() % (size_t)D || vals.size() != keys.size() * (size_t)D) return nullptr;
+static void* BuildTable(const TableData& in, int D) {
   DrEvConfig c{};
-  c.dim = D; c.num_slots = 0; c.has_scalars = 0; c.init_capacity = std::max<int64_t>(1024, (int64_t)keys.size() * 2);
-  c.default_value_dim = (int64_t)def.size() / D; c.num_partitions = 16; c.record_freq = 1; c.record_version = 1;
+  c.dim = D; c.num_slots = 0; c.has_scalars = 0; c.init_capacity = std::max<int64_t>(1024, (int64_t)in.keys.size() * 2);
+  c.default_value_dim = (int64_t)in.def.size() / D; c.num_partitions = 16; c.record_freq = 1; c.record_version = 1;
   c.l2_weight_threshold = -1.f;
   void* h = dr_host_ev_create(&c);                            // created writable for the import below; serving only ever calls Lookup
-  dr_host_ev_set_default(h, def.data());
-  if (!keys.empty())
-    dr_host_ev_import(h, keys.data(), vals.data(), D, freqs.size() == keys.size() ? freqs.data() : nullptr,
-                      vers.size() == keys.size() ? vers.data() : nullptr, (int64_t)keys.size(), 0, 1, 0);
-  sample->assign(keys.begin(), keys.begin() + std::min<size_t>(keys.size(), 64));
+  dr_host_ev_set_default(h, in.def.data());
+  if (!in.keys.empty())
+    dr_host_ev_import(h, in.keys.data(), in.values.data(), D, in.freqs.empty() ? nullptr : in.freqs.data(), in.versions.empty() ? nullptr : in.versions.data(),
+                      (int64_t)in.keys.size(), 0, 1, 0);
   return h;
 }
 
 static std::shared_ptr<Model> LoadModel(const std::string& dir, bool remote = false) {
   auto m = std::make_shared<Model>();
   std::string prefix;
-  if (!LoadArch(dir, &m->arch, &m->version, &prefix)) { fprintf(stderr, "[deeprec_cpu_serving] bad saved_model.json in %s\n", dir.c_str()); return nullptr; }
+  if (!ParseArch(dir, &m->arch, &m->version, &prefix)) { fprintf(stderr, "[deeprec_cpu_serving] bad saved_model.json in %s\n", dir.c_str()); return nullptr; }
   dr::BundleReader r(prefix);
   if (!r.ok()) { fprintf(stderr, "[deeprec_cpu_serving] cannot open bundle %s\n", prefix.c_str()); return nullptr; }
   if (!BuildDense(r, m->arch, &m->dense)) { fprintf(stderr, "[deeprec_cpu_serving] dense parameters incomplete in %s\n", prefix.c_str()); return nullptr; }
@@ -440,11 +245,12 @@ static std::shared_ptr<Model> LoadModel(const std::string& dir, bool remote = fa
     m->defaults.push_back(std::move(def));
   }
   for (int t = 0; t < m->arch.T && !remote; ++t) {
-    std::vector<int64_t> sample;
-    void* h = BuildTable(r, t, m->arch.D, &sample);
+    TableData td;
+    void* h = ReadTable(r, t, m->arch.D, &td) ? BuildTable(td, m->arch.D) : nullptr;
     if (!h) { fprintf(stderr, "[deeprec_cpu_serving] table %d incomplete\n", t); return nullptr; }
     m->tables.push_back(h);
-    for (size_t i = 0; i < 64; ++i) m->sample_keys[(size_t)t * 64 + i] = sample.empty() ? 0 : sample[i % sample.size()];
+    const size_t ns = std::min<size_t>(td.keys.size(), 64);
+    for (size_t i = 0; i < 64; ++i) m->sample_keys[(size_t)t * 64 + i] = ns ? td.keys[i % ns] : 0;
   }
   for (int c = 0; c < m->arch.C && !remote; ++c) m->col_handles.push_back(m->tables[(size_t)m->arch.col_table[(size_t)c]]);
   m->path = dir;
@@ -1264,53 +1070,33 @@ static bool ApplyDelta(ServingModel* sm, const std::string& prefix, int64_t vers
   if (!r.ok()) return false;
   for (int t = 0; t < m->arch.T && !m->tables.empty(); ++t) {      // (remote mode: the trainer inserts delta rows into the feature store itself)
     std::vector<int64_t> keys; std::vector<float> vals;
-    const std::string base = "table/" + std::to_string(t);
-    if (!ReadVec(r, base + "-sparse_incr_keys", &keys) || keys.empty()) continue;
-    if (!ReadVec(r, base + "-sparse_incr_values", &vals) || vals.size() != keys.size() * (size_t)m->arch.D) return false;
+    if (!ReadDeltaRows(r, t, m->arch.D, &keys, &vals)) return false;
+    if (keys.empty()) continue;
     dr_host_ev_import_cow(m->tables[(size_t)t], keys.data(), vals.data(), m->arch.D, (int64_t)keys.size());   // copy-on-write: readers never see a torn row
   }
   std::shared_ptr<Dense> dp;
-  const bool has_dense = m->arch.program ? (!m->arch.ops.empty() && [&] { for (auto& op : m->arch.ops) if (op.kind == P_LINEAR) return r.Find("prog/" + op.name + "/kernel") != nullptr; return false; }())
-                                         : r.Find("dense/logits/kernel") != nullptr;
-  if (has_dense && BuildDense(r, m->arch, &dp)) std::atomic_store(&m->dense, dp);
+  if (HasDenseBlock(r, m->arch) && BuildDense(r, m->arch, &dp)) std::atomic_store(&m->dense, dp);
   sm->delta_version = version;
   sm->delta_updates++;
   return true;
 }
 
-// version file: <dir>/serving_versions.json = {"full": {"version": V, "dir": "..."}, "deltas": [{"version": v, "base": V, "prefix": "..."}]}
 static void UpdaterLoop(ServingModel* sm) {
-  const std::string vf = (sm->cfg.checkpoint_dir.empty() ? sm->cfg.savedmodel_dir : sm->cfg.checkpoint_dir) + "/serving_versions.json";
   int bad = 0;
 #ifdef _OPENMP
   if (sm->compat.update_intra_threads > 0) omp_set_num_threads(sm->compat.update_intra_threads);    // model_update_intra_threads: the hot update's imports / packing run on this thread's team
 #endif
-  while (!sm->stop) {
-    for (int i = 0; i < std::max(1, sm->cfg.update_interval_ms / 20) && !sm->stop; ++i) std::this_thread::sleep_for(std::chrono::milliseconds(20));
-    std::string txt; JVal j;
-    if (!drjson::ReadFile(vf, &txt) || !drjson::ParseJson(txt, &j)) continue;
-    auto cur = std::atomic_load(&sm->model);
-    if (auto* f = j.get("full")) {
-      const int64_t v = (int64_t)f->n("version", -1); const std::string dir = f->s("dir", "");
-      if (cur && v > cur->version && !dir.empty()) {
-        auto nm = LoadModel(dir, sm->cfg.remote);
-        if (!nm) { if (++bad > 3) fprintf(stderr, "[deeprec_cpu_serving] skipping invalid model version %lld\n", (long long)v); continue; }
-        bad = 0;
-        if (!WarmUp(sm, nm)) continue;
-        std::atomic_store(&sm->model, nm);            // requests in flight keep the old model alive through their shared_ptr
-        sm->delta_version = -1;
-        sm->full_updates++;
-        continue;
-      }
-    }
-    if (auto* d = j.get("deltas")) {
-      cur = std::atomic_load(&sm->model);
-      for (auto& e : d->arr) {
-        const int64_t v = (int64_t)e.n("version", -1), base = (int64_t)e.n("base", -1);
-        if (cur && base == cur->version && v > std::max<int64_t>(cur->version, sm->delta_version.load())) ApplyDelta(sm, e.s("prefix", ""), v);
-      }
-    }
-  }
+  auto load_full = [&](int64_t v, const std::string& dir) {
+    auto nm = LoadModel(dir, sm->cfg.remote);
+    if (!nm) { if (++bad > 3) fprintf(stderr, "[deeprec_cpu_serving] skipping invalid model version %lld\n", (long long)v); return; }
+    bad = 0;
+    if (!WarmUp(sm, nm)) return;                  // also grows the sessions to a wider architecture
+    std::atomic_store(&sm->model, nm);            // requests in flight keep the old model alive through their shared_ptr
+    sm->delta_version = -1;
+    sm->full_updates++;
+  };
+  RunUpdater(sm->cfg.checkpoint_dir.empty() ? sm->cfg.savedmodel_dir : sm->cfg.checkpoint_dir, sm->cfg.update_interval_ms, sm->stop, sm->model, sm->delta_version,
+             load_full, [&](int64_t v, const std::string& prefix) { ApplyDelta(sm, prefix, v); });
 }
 
 }  // namespace cpusrv
