@@ -41,6 +41,7 @@ CUDA_SOURCES = [
     "cuda/attention_kernels.cu",
     "cuda/rnn_kernels.cu",              # tensor-core GRU recurrence (mma.sync): hardware only, not in EMU_SOURCES
     "cuda/mha_kernels.cu",              # tensor-core multi-head self-attention (mma.sync): hardware only, not in EMU_SOURCES
+    "cuda/sm_partition.cu",             # green-context SM partition (driver API): hardware only, not in EMU_SOURCES
 ]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

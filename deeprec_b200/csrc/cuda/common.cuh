@@ -83,8 +83,9 @@ struct DrPerDeviceOnce {
   bool& operator()() { int d = 0; cudaGetDevice(&d); return done[d & 63]; }
 };
 
-// Resident-block budget (per SM) of the sparse-path kernels.  They run on a side stream next to the wgmma GEMMs
-// (1 CTA/SM, up to ~200 KB smem, 384 threads): capping them leaves thread slots so both streams really overlap.
+// Resident-block budget (per SM) of the sparse-path kernels: their grid-stride grids are num_sms() * this many blocks.  An SM holding
+// sparse blocks cannot also take a wgmma GEMM CTA (384 threads, up to 168 registers each, ~200 KB smem), so next to the GEMMs the two
+// streams share SMs only one at a time; DLRMConfig.sparse_sms gives the sparse kernels SMs of their own instead (sm_partition.cu).
 inline int& sparse_blocks_per_sm() { static int v = 16; return v; }
 constexpr int64_t kEmptyKey = INT64_MIN;
 constexpr int64_t kTombKey = INT64_MIN + 1;

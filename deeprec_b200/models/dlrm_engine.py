@@ -25,7 +25,9 @@ Execution design (GPU-first; nothing here is a translation of the TF graph):
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
+from contextlib import nullcontext
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
 
@@ -65,7 +67,10 @@ class DLRMConfig:
     steps_to_live: int = 0
     seed: int = 1234
     overlap_embedding: bool = True              # fork the embedding branch onto a side stream inside the graph
-    sparse_blocks_per_sm: int = 4               # resident-block budget of the side-stream sparse kernels (overlap with the GEMMs)
+    sparse_blocks_per_sm: int = 4               # resident-block budget of the side-stream sparse kernels
+    # SMs of the green context the embedding branch runs in during the two overlap windows; the bottom MLP gets the rest (csrc/cuda/
+    # sm_partition.cu).  Rounded by the driver (multiples of 8 on Hopper).  0 = both branches share every SM as two streams of one context.
+    sparse_sms: int = 48
     gemm_v1: bool = False                       # A/B switch: separate statistics passes instead of the statistics fused into the GEMM epilogue
     # combine + dot interaction + top-MLP layer 0 in ONE tensor-core kernel (csrc/cuda/fused_interaction_gemm.cu).  Opt-in: the builder
     # phase and the GEMM phase of a tile share one 96 KB Z tile in shared memory and run one after the other, so the default step keeps
@@ -102,6 +107,14 @@ class DLRMEngine:
         import os as _os
         self._timing, self._events = _os.environ.get("DEEPREC_STEP_TIMING") == "1", {}
         self._side = None if self.emu else torch.cuda.Stream(device=self.dev)
+        self._dense, self._ctas = None, 0          # dense-partition stream, persistent GEMM grid cap (0 = every SM)
+        self.partition_sms = None                  # (sparse, dense) SMs the driver provisioned when sparse_sms > 0
+        if cfg.sparse_sms > 0 and cfg.overlap_embedding and not self.emu and (comm is None or getattr(comm, "unique_first", False)):
+            info, h = (C.c_int * 2)(), (C.c_void_p * 5)()
+            check(self.lib.dr_cuda_sm_partition(self.dev.index, int(cfg.sparse_sms), info, h), f"SM partition ({cfg.sparse_sms} sparse SMs)")
+            self.partition_sms = (info[0], info[1])
+            self._side = torch.cuda.ExternalStream(h[0], device=self.dev)
+            self._dense = torch.cuda.ExternalStream(h[1], device=self.dev)
         self._build_params()
         self._build_tables()
         self._build_buffers()
@@ -277,7 +290,7 @@ class DLRMEngine:
         mode = aux_mode if aux_mode is not None else (1 if mask is not None else 0)
         self._call(self.lib.dr_cuda_gemm_tn_ex, ptr(A), lda, ptr(Bm), ldb, M, N, K, ptr(bias) if bias is not None else None, int(relu),
                    ptr(mask) if mask is not None else None, ldm, mode, ptr(out), ldc, None, ptr(S1) if S1 is not None else None,
-                   ptr(S2) if S2 is not None else None, 0, int(self.cfg.gemm_v1))
+                   ptr(S2) if S2 is not None else None, self._ctas, int(self.cfg.gemm_v1))
 
     def _gemm_dw(self, dY, ldy, X, ldx, n_out, k_in, dW, ldw):
         self._call(self.lib.dr_cuda_gemm_dw, ptr(dY), ldy, ptr(X), ldx, self.B, n_out, k_in, ptr(dW), ldw, 0)
@@ -312,16 +325,47 @@ class DLRMEngine:
                    cfg.bn_eps, cfg.bn_momentum, ptr(L.running_mean), ptr(L.running_var), ptr(L.mean), ptr(L.rstd), ptr(L.scale), ptr(L.shift),
                    int(train), ptr(self.p(Ln.name + "/kernel")), ptr(self.p(Ln.name + "/bias")), Ln.N, Ln.Kp, ptr(Ln.wf_bf16), ptr(Ln.bf))
 
+    # ---- the two overlap windows.  With an SM partition the main-stream work of a window runs on the dense green context's stream, with
+    #      persistent GEMM grids sized to that context's SMs (a grid sized to the whole GPU would run as two waves there)
+    def _fork(self, main) -> None:
+        self._side.wait_stream(main)
+        if self._dense is not None:
+            self._dense.wait_stream(main)
+
+    def _dense_window(self):
+        if self._dense is None:
+            return nullcontext()
+        self._ctas = self.partition_sms[1]
+        return torch.cuda.stream(self._dense)
+
+    def _join(self, main) -> None:
+        main.wait_stream(self._side)
+        if self._dense is not None:
+            main.wait_stream(self._dense)
+            self._ctas = 0
+
     def _forward(self, train: bool) -> None:
-        lib, B, cfg = self.lib, self.B, self.cfg
+        cfg = self.cfg
         main = None if self.emu else torch.cuda.current_stream(self.dev)
         fork = cfg.overlap_embedding and not self.emu
         self._tick("f0")
         if fork:
-            self._side.wait_stream(main)
+            self._fork(main)
             with torch.cuda.stream(self._side):
                 self._embedding_forward(train)
                 self._tick("f_emb")
+        with self._dense_window() if fork else nullcontext():
+            x, ldx = self._bottom_forward(train)
+        if fork:
+            self._join(main)
+        else:
+            self._embedding_forward(train)
+            self._tick("f_emb")
+        self._tick("f_join")
+        self._top_forward(train, x, ldx)
+
+    def _bottom_forward(self, train: bool):
+        lib, B, cfg = self.lib, self.B, self.cfg
         # ---- bottom MLP.  Layer l: a_l = relu(a_{l-1} W_l'^T + b_l') with BatchNorm_{l-1} folded into (W', b'); the batch
         #      statistics of a_l come out of the GEMM epilogue, so no activation is read twice and y_l is never written.
         self._call(lib.dr_cuda_cast_pad, ptr(self.dense_in), B, cfg.num_dense, ptr(self.x0), self.x0.shape[1])
@@ -343,12 +387,10 @@ class DLRMEngine:
                 self._call(lib.dr_cuda_bn_apply, ptr(L.a), B, L.N, L.N, ptr(L.scale), ptr(L.shift), ptr(L.y), L.N)
                 x, ldx = L.y, L.N
         self._tick("f_bot")
-        if fork:
-            main.wait_stream(self._side)
-        else:
-            self._embedding_forward(train)
-            self._tick("f_emb")
-        self._tick("f_join")
+        return x, ldx
+
+    def _top_forward(self, train: bool, x, ldx) -> None:
+        lib, B, cfg = self.lib, self.B, self.cfg
         # ---- interaction + top MLP
         fused0 = self.uf and cfg.fuse_interaction_gemm and self.D == 16 and self.top[0].N <= 512 and self.inter_dim <= 384 and not self.emu
         if fused0:    # gather + Gram + lower-triangle pack + Linear(512) + ReLU in one kernel; Z only leaves the SM as a TMA store for the backward
@@ -416,10 +458,22 @@ class DLRMEngine:
         fork = cfg.overlap_embedding and not self.emu
         self._tick("b_dot")
         if fork:
-            self._side.wait_stream(main)
+            self._fork(main)
             with torch.cuda.stream(self._side):
                 self._embedding_backward()
                 self._tick("b_emb")
+        with self._dense_window() if fork else nullcontext():
+            self._bottom_backward()
+        if fork:
+            self._join(main)
+        else:
+            self._embedding_backward()
+            self._tick("b_emb")
+        self._tick("b_join")
+
+    def _bottom_backward(self) -> None:
+        lib, B, cfg = self.lib, self.B, self.cfg
+        v2 = not cfg.gemm_v1
         # ---- bottom MLP backward
         for i in range(len(self.bot) - 1, -1, -1):
             L = self.bot[i]
@@ -444,12 +498,6 @@ class DLRMEngine:
             else:
                 self._gemm_dw(L.da, L.N, self.x0, self.x0.shape[1], L.N, L.Kp, self.g(L.name + "/kernel"), L.Kp)
         self._tick("b_bot")
-        if fork:
-            main.wait_stream(self._side)
-        else:
-            self._embedding_backward()
-            self._tick("b_emb")
-        self._tick("b_join")
 
     def _dense_update(self) -> None:
         lib = self.lib
