@@ -89,6 +89,7 @@ _sig("dr_cuda_segment_sum", [P, P, i64, INT, P, S])
 # GEMM, quantisation, BatchNorm, head
 _sig("dr_cuda_gemm_tn", [P, i64, P, i64, INT, INT, INT, P, INT, P, i64, P, i64, P, INT, S])
 _sig("dr_cuda_gemm_tn_ex", [P, i64, P, i64, INT, INT, INT, P, INT, P, i64, INT, P, i64, P, P, P, INT, INT, S])
+_sig("dr_cuda_gemm_tn_cross", [P, i64, P, i64, INT, INT, INT, P, INT, P, i64, P, i64, P, i64, P, i64, INT, S])
 _sig("dr_cuda_gemm_fp8_tn", [P, i64, P, i64, INT, INT, INT, P, P, INT, P, i64, INT, f32, S])
 _sig("dr_cuda_quantize_e4m3", [P, INT, i64, INT, i64, P, INT, f32, S])
 _sig("dr_cuda_quantize_weights_e4m3", [P, INT, INT, i64, P, INT, P, S])
@@ -107,6 +108,8 @@ _sig("dr_cuda_bn_bwd_apply", [P, P, i64, INT, i64, P, P, P, P, P, P, INT, S])
 _sig("dr_cuda_head", [P, i64, i64, INT, P, P, P, f32, P, P, P, P, P, INT, INT, P, S])
 _sig("dr_cuda_det_colsum", [P, INT, i64, INT, P, P, S])
 _sig("dr_cuda_pack_weights", [P, INT, INT, P, P, INT, S])
+_sig("dr_cuda_cross_bwd", [P, i64, P, i64, P, i64, i64, INT, P, i64, P, i64, INT, P, S])
+_sig("dr_cuda_cross_split", [P, i64, P, i64, i64, INT, INT, P, i64, P, S])
 _sig("dr_cuda_cast_pad", [P, i64, INT, P, INT, S])
 _sig("dr_cuda_l2_flush", [P, i64, f32, S])
 # interactions, GRU, self-attention, DIN attention, fused element-wise ops
@@ -142,6 +145,7 @@ _sig("dr_sp_init_scratch", [P, i64, S])
 _sig("dr_sp_dedup", [P, GP, P, P, P, P, P, P, P, SP, S])
 _sig("dr_sp_segsum", [P, P, GP, P, SP, S])
 _sig("dr_sp_gather", [P, P, GP, P, SP, S])
+_sig("dr_sp_gather_pitched", [P, P, GP, P, i64, SP, S])
 _sig("dr_sp_pool", [P, P, GP, BP, P, P, SP, S])
 _sig("dr_sp_pool_segsum", [P, P, P, GP, BP, P, SP, S])
 _sig("dr_sp_linear_fwd", [P, P, GP, P, SP, S])

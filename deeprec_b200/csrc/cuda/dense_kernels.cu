@@ -390,6 +390,93 @@ inline int grid_for(int64_t n, int block, int max_blocks = num_sms() * 8) {
   return (int)b;
 }
 
+// -------------------------------------------------------------------------------------------------
+// Low-rank cross layer backward, element-wise part (DLRM-DCNv2: x_{l+1} = x0 * u + x_l, u = x_l V W + b).  Given g = dL/dx_{l+1}:
+//   du = g * x0 (bf16, the operand of the dW / dt GEMMs),  dx0 (fp32) = (init ? 0 : dx0) + g * u,  part[blockIdx.x][n] = this block's
+//   column sums of du (fp32, before the bf16 rounding), added in order by k_det_colsum.  A block covers cg column groups of 8 (blockIdx.y
+//   picks which) and rows_par = 256 / cg rows at a time; its row partials are added in row-group order, so db does not depend on timing.
+// -------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_cross_bwd(const __nv_bfloat16* __restrict__ g, int64_t ldg, const __nv_bfloat16* __restrict__ x0, int64_t ldx0,
+                                                   const __nv_bfloat16* __restrict__ u, int64_t ldu, int64_t B, int N, __nv_bfloat16* __restrict__ du,
+                                                   int64_t lddu, float* __restrict__ dx0, int64_t lddx, int init, float* __restrict__ part) {
+  pdl_sync();
+  const int groups = N / 8;
+  const int cg = groups < 256 ? groups : 256;
+  const int rows_par = 256 / cg;
+  const int tr = threadIdx.x / cg, tc = threadIdx.x % cg;
+  const int cgrp = blockIdx.y * cg + tc;
+  const bool live = tr < rows_par && cgrp < groups;
+  const int c0 = cgrp * 8;
+  float acc[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+  if (live) {
+    for (int64_t b = (int64_t)blockIdx.x * rows_par + tr; b < B; b += (int64_t)gridDim.x * rows_par) {
+      const int4 rg = ld_nc_v4(g + b * ldg + c0), rx = ld_nc_v4(x0 + b * ldx0 + c0), ru = ld_nc_v4(u + b * ldu + c0);
+      float* d = dx0 + b * lddx + c0;
+      float4 q0 = make_float4(0.f, 0.f, 0.f, 0.f), q1 = q0;
+      if (!init) { q0 = *reinterpret_cast<const float4*>(d); q1 = *reinterpret_cast<const float4*>(d + 4); }
+      float dxv[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
+      const uint32_t wg[4] = {(uint32_t)rg.x, (uint32_t)rg.y, (uint32_t)rg.z, (uint32_t)rg.w};
+      const uint32_t wx[4] = {(uint32_t)rx.x, (uint32_t)rx.y, (uint32_t)rx.z, (uint32_t)rx.w};
+      const uint32_t wu[4] = {(uint32_t)ru.x, (uint32_t)ru.y, (uint32_t)ru.z, (uint32_t)ru.w};
+      uint32_t o[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 fg = unpack_bf16x2(wg[e]), fx = unpack_bf16x2(wx[e]), fu = unpack_bf16x2(wu[e]);
+        const float d0 = fg.x * fx.x, d1 = fg.y * fx.y;
+        acc[2 * e] += d0; acc[2 * e + 1] += d1;
+        dxv[2 * e] = fmaf(fg.x, fu.x, dxv[2 * e]); dxv[2 * e + 1] = fmaf(fg.y, fu.y, dxv[2 * e + 1]);
+        o[e] = pack_bf16x2(d0, d1);
+      }
+      *reinterpret_cast<int4*>(du + b * lddu + c0) = make_int4((int)o[0], (int)o[1], (int)o[2], (int)o[3]);
+      *reinterpret_cast<float4*>(d) = make_float4(dxv[0], dxv[1], dxv[2], dxv[3]);
+      *reinterpret_cast<float4*>(d + 4) = make_float4(dxv[4], dxv[5], dxv[6], dxv[7]);
+    }
+  }
+  __shared__ float sh[256 * 8];                   // [rows_par][cg * 8]
+  if (live) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) sh[tr * cg * 8 + tc * 8 + j] = acc[j];
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < cg * 8; i += blockDim.x) {
+    const int col = blockIdx.y * cg * 8 + i;
+    if (col < N) {
+      float sum = 0.f;
+      for (int r = 0; r < rows_par; ++r) sum += sh[r * cg * 8 + i];
+      part[(int64_t)blockIdx.x * N + col] = sum;
+    }
+  }
+}
+
+// dx0 [B, (T + 1) D] (fp32, + the bf16 addend dxa if given) -> dy [B, D] (columns [0, D)) and the feature-major demb [T][B][D] (columns
+// [D (t + 1), D (t + 2)) of table t), bf16.  One thread per 8 columns of a row; D is a multiple of 8, so the 8 never straddle two features.
+__global__ void __launch_bounds__(256) k_cross_split(const float* __restrict__ dx0, int64_t lddx, const __nv_bfloat16* __restrict__ dxa, int64_t ldda,
+                                                     int64_t B, int T, int D, __nv_bfloat16* __restrict__ dy, int64_t ldy,
+                                                     __nv_bfloat16* __restrict__ demb) {
+  pdl_sync();
+  const int groups = (T + 1) * D / 8;
+  const int64_t n = B * groups;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / groups;
+    const int c = (int)(i % groups) * 8;
+    const float* src = dx0 + b * lddx + c;
+    const float4 q0 = *reinterpret_cast<const float4*>(src), q1 = *reinterpret_cast<const float4*>(src + 4);
+    float v[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
+    if (dxa) {
+      const int4 ra = ld_nc_v4(dxa + b * ldda + c);
+      const uint32_t wa[4] = {(uint32_t)ra.x, (uint32_t)ra.y, (uint32_t)ra.z, (uint32_t)ra.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) { const float2 f = unpack_bf16x2(wa[e]); v[2 * e] += f.x; v[2 * e + 1] += f.y; }
+    }
+    const int4 o = make_int4((int)pack_bf16x2(v[0], v[1]), (int)pack_bf16x2(v[2], v[3]), (int)pack_bf16x2(v[4], v[5]), (int)pack_bf16x2(v[6], v[7]));
+    const int f = c / D;
+    __nv_bfloat16* dst = f == 0 ? dy + b * ldy + c : demb + ((int64_t)(f - 1) * B + b) * D + (c - f * D);
+    *reinterpret_cast<int4*>(dst) = o;
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -522,6 +609,40 @@ int dr_cuda_cast_pad(const float* x, int64_t B, int C, void* y, int Cp, cudaStre
 
 int dr_cuda_l2_flush(float* buf, int64_t n, float v, cudaStream_t s) {
   k_l2_flush<<<num_sms() * 4, 256, 0, s>>>(buf, n, v);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// Low-rank cross layer backward, element-wise part (k_cross_bwd): du = g * x0 (bf16), dx0 (fp32) = (init ? 0 : dx0) + g * u, and
+// db += column sums of du (summed in block order).  bf16 operands: pitches multiples of 8, 16-byte aligned; dx0: pitch a multiple of 4.
+int dr_cuda_cross_bwd(const void* g, int64_t ldg, const void* x0, int64_t ldx0, const void* u, int64_t ldu, int64_t B, int N, void* du, int64_t lddu,
+                      float* dx0, int64_t lddx, int init, float* db, cudaStream_t s) {
+  if (B <= 0 || N <= 0) return 0;
+  if ((N % 8) || (ldg % 8) || (ldx0 % 8) || (ldu % 8) || (lddu % 8) || (lddx % 4)) return -2;
+  if (((uintptr_t)g | (uintptr_t)x0 | (uintptr_t)u | (uintptr_t)du | (uintptr_t)dx0) & 15) return -3;
+  if (ldg < N || ldx0 < N || ldu < N || lddu < N || lddx < N) return -5;
+  const int groups = N / 8, cg = groups < 256 ? groups : 256, rows_par = 256 / cg;
+  const int gy = (groups + cg - 1) / cg;
+  const int gx = grid_for((B + rows_par - 1) / rows_par, 2, max(1, num_sms() * 8 / gy));
+  float* part = dr_workspace(kWsCross, (size_t)gx * N, s);
+  if (!part) return -5;
+  DR_PDL_LAUNCH((k_cross_bwd), dim3(gx, gy), 256, 0, s, (const __nv_bfloat16*)g, ldg, (const __nv_bfloat16*)x0, ldx0, (const __nv_bfloat16*)u, ldu, B, N,
+                (__nv_bfloat16*)du, lddu, dx0, lddx, init, part);
+  DR_LAUNCH_CHECK();
+  det_colsum(part, gx, (int64_t)N, {{0, N, db}}, s);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// dx0 [B, (T + 1) D] fp32 (+ dxa bf16, may be null) -> dy [B, D] bf16 (pitch ldy) and demb [T][B][D] bf16
+int dr_cuda_cross_split(const float* dx0, int64_t lddx, const void* dxa, int64_t ldda, int64_t B, int T, int D, void* dy, int64_t ldy, void* demb,
+                        cudaStream_t s) {
+  if (B <= 0) return 0;
+  if (D <= 0 || (D % 8) || T < 0 || (lddx % 4) || (dxa && ldda % 8) || (ldy % 8)) return -2;
+  if (((uintptr_t)dx0 | (uintptr_t)dxa | (uintptr_t)dy | (uintptr_t)demb) & 15) return -3;
+  if (lddx < (int64_t)(T + 1) * D || (dxa && ldda < (int64_t)(T + 1) * D) || ldy < D) return -5;
+  DR_PDL_LAUNCH((k_cross_split), grid_for(B * ((T + 1) * D / 8), 256), 256, 0, s, dx0, lddx, (const __nv_bfloat16*)dxa, ldda, B, T, D,
+                (__nv_bfloat16*)dy, ldy, (__nv_bfloat16*)demb);
   DR_LAUNCH_CHECK();
   return 0;
 }

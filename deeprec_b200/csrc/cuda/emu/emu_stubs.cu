@@ -45,6 +45,36 @@ int dr_cuda_gemm_tn(const void* A, int64_t lda, const void* B, int64_t ldb, int 
   return dr_cuda_gemm_tn_ex(A, lda, B, ldb, M, N, K, bias, relu, mask_src, ld_mask, mask_src ? 1 : 0, out, ldc, out_f32, nullptr, nullptr, max_ctas, 0, s);
 }
 
+// gemm_wgmma.cu::dr_cuda_gemm_tn_cross: kind 1 out = x0 * (acc + bias) + xl (u_out = acc + bias), kind 2 out = acc + xl; same return codes.
+int dr_cuda_gemm_tn_cross(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* bias, int kind, const void* x0,
+                          int64_t ld_x0, const void* xl, int64_t ld_xl, void* out, int64_t ldc, void* u_out, int64_t ld_u, int max_ctas, cudaStream_t) {
+  (void)max_ctas;
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  if ((kind != 1 && kind != 2) || !xl || (kind == 1 && !x0)) return -4;
+  if (kind != 1) { x0 = nullptr; u_out = nullptr; }
+  if ((lda % 8) || (ldb % 8) || (ldc % 8) || (N % 8) || (ld_xl % 8) || (x0 && ld_x0 % 8) || (u_out && ld_u % 8)) return -2;
+  if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)out | (uintptr_t)xl | (uintptr_t)x0 | (uintptr_t)u_out) & 15) return -3;
+  if (lda < K || ldb < K || ldc < N || ld_xl < N || (x0 && ld_x0 < N) || (u_out && ld_u < N)) return -5;
+  const __nv_bfloat16* a = (const __nv_bfloat16*)A; const __nv_bfloat16* b = (const __nv_bfloat16*)B;
+  const __nv_bfloat16* xz = (const __nv_bfloat16*)x0; const __nv_bfloat16* xa = (const __nv_bfloat16*)xl;
+  __nv_bfloat16* o = (__nv_bfloat16*)out; __nv_bfloat16* uo = (__nv_bfloat16*)u_out;
+  for (int m = 0; m < M; ++m)
+    for (int n = 0; n < N; ++n) {
+      float acc = 0.f;
+      for (int k = 0; k < K; ++k) acc += bf(a + (int64_t)m * lda + k) * bf(b + (int64_t)n * ldb + k);
+      if (bias) acc += bias[n];
+      const float w = bf(xa + (int64_t)m * ld_xl + n);
+      if (kind == 1) {
+        if (uo) uo[(int64_t)m * ld_u + n] = __float2bfloat16(acc);
+        acc = fmaf(bf(xz + (int64_t)m * ld_x0 + n), acc, w);
+      } else {
+        acc += w;
+      }
+      o[(int64_t)m * ldc + n] = __float2bfloat16(acc);
+    }
+  return 0;
+}
+
 // gemm_wgmma.cu::dr_cuda_gemm_dw: dW[N_out,K_in](ldw, fp32, accumulated into) += dY[batch,N_out](ldy)^T * X[batch,K_in](ldx)
 int dr_cuda_gemm_dw(const void* dY, int64_t ldy, const void* X, int64_t ldx, int batch, int N_out, int K_in, float* dW, int64_t ldw, int splits, cudaStream_t) {
   (void)splits;

@@ -25,6 +25,7 @@
 #include <cuda.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -86,6 +87,17 @@ struct Epilogue {
   const uint32_t* sfa;            // MX path: UE8M0 scale words of A / B (layout of k_quantize_mxfp8, gemm_mxfp8.cu)
   const uint32_t* sfb;
 };
+
+// Epilogue kinds beyond the bias / ReLU / mask / statistics of kind 0.  The kind is a template parameter and only the new kinds take the
+// wider parameter block, so the kind-0 instantiations compile exactly as before.  The aux operand (mask_src, ld_mask) is x_l for kEpiCross
+// and the addend for kEpiResidual; both run with relu = 0 and aux_mode = 0.
+enum { kEpiPlain = 0, kEpiCross = 1, kEpiResidual = 2 };
+struct EpilogueX : Epilogue {
+  const __nv_bfloat16* x0;        // kEpiCross: the x0 factor [M, ld_x0]
+  __nv_bfloat16* u_out;           // kEpiCross: optional u = acc + bias [M, ld_u] (bf16), kept for the backward
+  int64_t ld_x0, ld_u;
+};
+template <int EPI> using EpiT = std::conditional_t<EPI == kEpiPlain, Epilogue, EpilogueX>;
 
 // UE8M0 scale byte -> 2^(b - 127)  (b = 0 is the denormal 2^-127)
 __device__ __forceinline__ float ue8m0(uint32_t b) { return b ? __uint_as_float(b << 23) : 5.877471754111438e-39f; }
@@ -156,11 +168,12 @@ __device__ __forceinline__ uint16_t pack_e4m3x2(float a, float b) {
   return r;
 }
 
-template <int BLOCK_N, bool BRES, bool CL2, bool FP8, bool MX = false, bool PP = false>
+template <int BLOCK_N, bool BRES, bool CL2, bool FP8, bool MX = false, bool PP = false, int EPI = kEpiPlain>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
-          const __grid_constant__ CUtensorMap tmAux, int M, int N, int K, Epilogue ep) {
+          const __grid_constant__ CUtensorMap tmAux, int M, int N, int K, EpiT<EPI> ep) {
   static_assert(!PP || (!BRES && !CL2 && !FP8), "ping-pong consumers: bf16 streaming kernel only");
+  static_assert(EPI == kEpiPlain || (!PP && !BRES && !CL2 && !FP8), "cross / residual epilogues: bf16 cooperative streaming kernel only");
   using L = SmemLayoutTN<BLOCK_N, BRES, PP>;
   constexpr int kSt = L::kSt;
   constexpr int kAcc = BLOCK_N / 2;
@@ -474,6 +487,15 @@ k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             w0 = __bfloat162float(ms[0]); w1 = __bfloat162float(ms[1]);
             if (ep.aux_mode == 1) { if (!(w0 > 0.f)) v0 = 0.f; if (!(w1 > 0.f)) v1 = 0.f; }
           }
+          if constexpr (EPI == kEpiCross) {               // u = acc + bias;  out = x0 * u + x_l
+            if (ok) {
+              if (ep.u_out) *reinterpret_cast<uint32_t*>(ep.u_out + (int64_t)row * ep.ld_u + col) = pack_bf16x2(v0, v1);
+              const float2 x = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(ep.x0 + (int64_t)row * ep.ld_x0 + col));
+              v0 = fmaf(x.x, v0, w0); v1 = fmaf(x.y, v1, w1);
+            }
+          } else if constexpr (EPI == kEpiResidual) {     // out = acc + aux
+            v0 += w0; v1 += w1;
+          }
           if (ok) {
             if (FP8 && !MX && ep.out_fp8) {
               *reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(ep.out) + (int64_t)row * ep.ldc + col) =
@@ -640,8 +662,8 @@ __global__ void k_dw_reduce(const float* __restrict__ part, int splits, int Mo, 
   }
 }
 
-template <int BN, bool BRES, bool CL2, bool FP8, bool MX = false, bool PP = false>
-int launch_tn(const CUtensorMap& ta, const void* B, int M, int N, int K, int64_t ldb, const Epilogue& ep, int max_ctas, cudaStream_t s) {
+template <int BN, bool BRES, bool CL2, bool FP8, bool MX = false, bool PP = false, int EPI = kEpiPlain>
+int launch_tn(const CUtensorMap& ta, const void* B, int M, int N, int K, int64_t ldb, const EpiT<EPI>& ep, int max_ctas, cudaStream_t s) {
   CUtensorMap tb, tout = {}, taux = {};
   const uint32_t box_rows = CL2 ? BN / 2 : BN;
   int rc = FP8 ? make_tmap(&tb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, 128, box_rows, CU_TENSOR_MAP_DATA_TYPE_UINT8)
@@ -659,7 +681,7 @@ int launch_tn(const CUtensorMap& ta, const void* B, int M, int N, int K, int64_t
       if (rc) return rc;
     }
   }
-  auto kern = k_gemm_tn<BN, BRES, CL2, FP8, MX, PP>;
+  auto kern = k_gemm_tn<BN, BRES, CL2, FP8, MX, PP, EPI>;
   static DrPerDeviceOnce attr_once; bool& attr_set = attr_once();
   if (!attr_set) {
     DR_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
@@ -778,6 +800,36 @@ int dr_cuda_gemm_tn_ex(const void* A, int64_t lda, const void* B, int64_t ldb, i
   det_colsum(ws, m_tiles, 2 * (int64_t)N, {{0, N, S1}, {N, N, S2}}, s);
   DR_LAUNCH_CHECK();
   return 0;
+}
+
+// Low-rank cross layer epilogues (DLRM-DCNv2, models/dlrm_engine.py), on the cooperative kernel at every K:
+//   kind 1 (cross):     out = x0 * (acc + bias) + xl        and, if u_out is given, u_out = acc + bias (bf16)
+//   kind 2 (residual):  out = acc + xl
+// with acc = A[M,K](lda) * B[N,K](ldb)^T in fp32 and the epilogue in fp32 from the bf16 operands, out rounded once to bf16.  bias may be
+// null.  Contract of dr_cuda_gemm_tn_ex for A, B and out, and for the new operands:  -2  a pitch of xl, x0 or u_out not a multiple of 8;
+// -3  xl, x0 or u_out not 16-byte aligned;  -5  ld_xl, ld_x0 or ld_u < N;  -4  an unknown kind, xl missing, or kind 1 without x0.
+int dr_cuda_gemm_tn_cross(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* bias, int kind,
+                          const void* x0, int64_t ld_x0, const void* xl, int64_t ld_xl, void* out, int64_t ldc, void* u_out, int64_t ld_u,
+                          int max_ctas, cudaStream_t s) {
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  if ((kind != kEpiCross && kind != kEpiResidual) || !xl || (kind == kEpiCross && !x0)) return -4;
+  if (kind != kEpiCross) { x0 = nullptr; u_out = nullptr; }
+  if ((lda % 8) || (ldb % 8) || (ldc % 8) || (N % 8) || (ld_xl % 8) || (x0 && ld_x0 % 8) || (u_out && ld_u % 8)) return -2;
+  if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)out | (uintptr_t)xl | (uintptr_t)x0 | (uintptr_t)u_out) & 15) return -3;
+  if (lda < K || ldb < K || ldc < N || ld_xl < N || (x0 && ld_x0 < N) || (u_out && ld_u < N)) return -5;
+  if (max_ctas <= 0) max_ctas = num_sms();
+  CUtensorMap ta;
+  int rc = make_tmap(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BLOCK_K, BLOCK_M);
+  if (rc) return rc;
+  EpilogueX ep;
+  static_cast<Epilogue&>(ep) = Epilogue{bias, (const __nv_bfloat16*)xl, out, nullptr, ldc, ld_xl, 0, 0, nullptr, nullptr, nullptr, nullptr, 0, 1.f};
+  ep.x0 = (const __nv_bfloat16*)x0; ep.u_out = (__nv_bfloat16*)u_out; ep.ld_x0 = ld_x0; ep.ld_u = ld_u;
+#define TN_EPI(BN)                                                                                                             \
+  (kind == kEpiCross ? launch_tn<BN, false, false, false, false, false, kEpiCross>(ta, B, M, N, K, ldb, ep, max_ctas, s)      \
+                     : launch_tn<BN, false, false, false, false, false, kEpiResidual>(ta, B, M, N, K, ldb, ep, max_ctas, s))
+  rc = N <= 16 ? TN_EPI(16) : N <= 32 ? TN_EPI(32) : N <= 64 ? TN_EPI(64) : TN_EPI(128);
+#undef TN_EPI
+  return rc;
 }
 
 // A/B switches for the GEMM variants (same effect as DEEPREC_GEMM_2CTA / DEEPREC_GEMM_BRES, settable at run time; return the previous value).

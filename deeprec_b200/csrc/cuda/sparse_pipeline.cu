@@ -327,11 +327,67 @@ __global__ void __launch_bounds__(256) k_sp_lookup(const DrDeviceTable* __restri
 // the same key are found with match.any; every group's leader sums its members' rows out of a 1 KB shared-memory tile and issues
 // ONE vectorised L2 reduction per 16 B chunk -- no shared-memory atomics (fp32 ATOMS are CAS loops), no sort.
 // -----------------------------------------------------------------------------------------------------------------
+// Rows wider than 64 (dim 128): the tile of a whole row would need 64 KB of shared memory and the leader 128 accumulators, so the row is
+// summed in 64-wide passes over the same key groups.  The 64-bit fixed-point L2 reductions make the result independent of the split.
+template <int LPR>
+__device__ __forceinline__ void sp_segsum_passes(const __nv_bfloat16* __restrict__ demb, const int32_t* __restrict__ invT, const DrSpGeom& g,
+                                                 unsigned long long* __restrict__ ugrad) {
+  constexpr int dim = 4 * LPR;
+  constexpr int PD = 64;                                       // columns per pass
+  constexpr int V = PD / 8;
+  static_assert(dim % PD == 0, "dim: a multiple of the pass width");
+  __shared__ __align__(16) int4 s_row[8][32][V];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t tiles = (g.B + 31) / 32;
+  const int64_t units = tiles * g.C;
+  for (int64_t u = (int64_t)blockIdx.x * 8 + warp; u < units; u += (int64_t)gridDim.x * 8) {
+    const int c = (int)(u / tiles);
+    const int64_t b = (u % tiles) * 32 + lane;
+    int32_t gs = -1;
+    if (b < g.B) gs = invT[(int64_t)c * g.B + b];
+    const bool live = gs >= 0;
+    const unsigned lm = __ballot_sync(0xffffffffu, live);
+    unsigned same = 0;
+    if (live) same = __match_any_sync(lm, gs);
+    const bool leader = live && lane == __ffs(same) - 1;       // leader of this key inside the tile
+    for (int p = 0; p < dim / PD; ++p) {
+      if (live) {
+        const int4* src = reinterpret_cast<const int4*>(demb + ((int64_t)c * g.B + b) * dim + p * PD);
+#pragma unroll
+        for (int v = 0; v < V; ++v) s_row[warp][lane][v] = ld_nc_v4(src + v);
+      }
+      __syncwarp();
+      if (leader) {
+        float acc[PD];
+#pragma unroll
+        for (int d = 0; d < PD; ++d) acc[d] = 0.f;
+        for (unsigned m = same; m; m &= m - 1) {
+          const int src_lane = __ffs(m) - 1;
+#pragma unroll
+          for (int v = 0; v < V; ++v) {
+            const int4 raw = s_row[warp][src_lane][v];
+            const uint32_t w[4] = {(uint32_t)raw.x, (uint32_t)raw.y, (uint32_t)raw.z, (uint32_t)raw.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) { const float2 f = unpack_bf16x2(w[e]); acc[8 * v + 2 * e] += f.x; acc[8 * v + 2 * e + 1] += f.y; }
+          }
+        }
+        unsigned long long* dst = ugrad + (int64_t)gs * dim + p * PD;
+#pragma unroll
+        for (int d = 0; d < PD; ++d) atomicAdd(dst + d, ugrad_fix(acc[d]));
+      }
+      __syncwarp();
+    }
+  }
+}
+
 template <int LPR /* dim / 4 */>
 __global__ void __launch_bounds__(256) k_sp_segsum(const __nv_bfloat16* __restrict__ demb /* [C][B][dim] */, const int32_t* __restrict__ invT /* [C][B] */,
                                                    DrSpGeom g, unsigned long long* __restrict__ ugrad, DrSpSync sync) {
   pdl_sync();
   constexpr int dim = 4 * LPR;
+  if constexpr (dim > 64) {
+    sp_segsum_passes<LPR>(demb, invT, g, ugrad);
+  } else {
   constexpr int V = dim / 8;                                   // int4 (8 bf16) chunks per row
   __shared__ __align__(16) int4 s_row[8][32][V];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -373,16 +429,18 @@ __global__ void __launch_bounds__(256) k_sp_segsum(const __nv_bfloat16* __restri
     }
     __syncwarp();
   }
+  }
   sp_signal_last_block(sync, SP_CH_GRAD);
 }
 
 // -----------------------------------------------------------------------------------------------------------------
-// k_sp_gather (requester): out[b][c][:] = urow[inv[b][c]]  (padding -> zeros) -- the sample-major [B, C, dim] activation generic dense
-// networks consume (models/rec_engine.py).  Waits in-kernel for every owner's ROWS flag, like the fused interaction kernels do.
+// k_sp_gather (requester): out[b * ldo + c * dim + :] = urow[inv[b][c]]  (padding -> zeros) -- the sample-major [B, C, dim] activation generic
+// dense networks consume (models/rec_engine.py, ldo = C * dim), or the embedding columns of a wider row (DLRM-DCNv2's x0).  Waits in-kernel
+// for every owner's ROWS flag, like the fused interaction kernels do.
 // -----------------------------------------------------------------------------------------------------------------
 template <int LPR>
 __global__ void __launch_bounds__(256) k_sp_gather(const __nv_bfloat16* __restrict__ urow, const int32_t* __restrict__ inv, int ldinv, int C, int64_t B,
-                                                   __nv_bfloat16* __restrict__ out, DrSpSync sync) {
+                                                   __nv_bfloat16* __restrict__ out, int64_t ldo, DrSpSync sync) {
   pdl_sync();
   sp_wait_all(sync, SP_CH_ROWS);
   constexpr int dim = 4 * LPR;
@@ -393,7 +451,7 @@ __global__ void __launch_bounds__(256) k_sp_gather(const __nv_bfloat16* __restri
     const int32_t gs = inv[b * ldinv + c];
     uint2 v = make_uint2(0u, 0u);
     if (gs >= 0) DR_LD_V2_VOLATILE_U32(v, urow + (int64_t)gs * dim + 4 * lane);
-    *reinterpret_cast<uint2*>(out + i * dim + 4 * lane) = v;
+    *reinterpret_cast<uint2*>(out + b * ldo + (int64_t)c * dim + 4 * lane) = v;
   }
 }
 
@@ -684,7 +742,7 @@ int dr_sp_segsum(const void* demb, const int32_t* invT, const DrSpGeom* g, void*
   const int grid = sp_grid((units + 7) / 8);
 #define SPS(L) DR_PDL_LAUNCH((k_sp_segsum<L>), grid, 256, 0, s, (const __nv_bfloat16*)demb, invT, *g, (unsigned long long*)ugrad, *sync)
   switch (g->dim / 4) {
-    case 2: SPS(2); break; case 4: SPS(4); break; case 8: SPS(8); break; case 16: SPS(16); break;
+    case 2: SPS(2); break; case 4: SPS(4); break; case 8: SPS(8); break; case 16: SPS(16); break; case 32: SPS(32); break;
     default: return -3;
   }
 #undef SPS
@@ -726,11 +784,14 @@ int dr_sp_grad(const DrDeviceTable* tables_dev, const int32_t* table_map, const 
   return 0;
 }
 
-int dr_sp_gather(const void* urow, const int32_t* inv, const DrSpGeom* g, void* out, const DrSpSync* sync, cudaStream_t s) {
+}  // extern "C"
+
+namespace {
+int sp_gather(const void* urow, const int32_t* inv, const DrSpGeom* g, void* out, int64_t ldo, const DrSpSync* sync, cudaStream_t s) {
   const int lpr = g->dim / 4;
   const int64_t n = g->B * g->C;
   const int grid = sp_grid((n * lpr + 255) / 256);
-#define SPGA(L) DR_PDL_LAUNCH((k_sp_gather<L>), grid, 256, 0, s, (const __nv_bfloat16*)urow, inv, g->ldinv, g->C, g->B, (__nv_bfloat16*)out, *sync)
+#define SPGA(L) DR_PDL_LAUNCH((k_sp_gather<L>), grid, 256, 0, s, (const __nv_bfloat16*)urow, inv, g->ldinv, g->C, g->B, (__nv_bfloat16*)out, ldo, *sync)
   switch (lpr) {
     case 2: SPGA(2); break; case 4: SPGA(4); break; case 8: SPGA(8); break; case 16: SPGA(16); break; case 32: SPGA(32); break;
     default: return -3;
@@ -738,6 +799,20 @@ int dr_sp_gather(const void* urow, const int32_t* inv, const DrSpGeom* g, void* 
 #undef SPGA
   DR_LAUNCH_CHECK();
   return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int dr_sp_gather(const void* urow, const int32_t* inv, const DrSpGeom* g, void* out, const DrSpSync* sync, cudaStream_t s) {
+  return sp_gather(urow, inv, g, out, (int64_t)g->C * g->dim, sync, s);
+}
+
+// dr_sp_gather into rows of pitch ldo (elements): out[b * ldo + c * dim + :] = urow[inv[b][c]].  -2: ldo not a multiple of 4 or < C * dim,
+// or out not 8-byte aligned.
+int dr_sp_gather_pitched(const void* urow, const int32_t* inv, const DrSpGeom* g, void* out, int64_t ldo, const DrSpSync* sync, cudaStream_t s) {
+  if ((ldo % 4) || ldo < (int64_t)g->C * g->dim || ((uintptr_t)out & 7)) return -2;
+  return sp_gather(urow, inv, g, out, ldo, sync, s);
 }
 
 // out: bf16 [B][F][dim] pooled bags, w_out: fp32 [F][B] the factor each bag was scaled by; waits for every owner's ROWS flag

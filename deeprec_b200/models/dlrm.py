@@ -58,10 +58,14 @@ def dot_interaction_reference(dense: torch.Tensor, embs: torch.Tensor) -> torch.
 
 
 class DLRM(nn.Module):
+    """interaction_op: "dot" (DLRM), "dcnv2" (DLRM-DCNv2: concatenation, then dcn_num_layers low-rank cross layers
+    x_{l+1} = x0 * (x_l V_l W_l + b_l) + x_l of rank dcn_low_rank_dim), anything else: the concatenation alone."""
+
     def __init__(self, num_dense: int = 13, cardinalities: Sequence[int] = (1000,) * 26, embedding_dim: int = 16,
                  mlp_bot: Sequence[int] = (512, 256, 64, 16), mlp_top: Sequence[int] = (512, 256), interaction_op: str = "dot",
                  ev_option: Optional[EmbeddingVariableOption] = None, device=None, use_ev: bool = True,
-                 bn_eps: float = 1e-3, bn_momentum: float = 0.99, name: str = "dlrm", fused_kernels: bool = False):
+                 bn_eps: float = 1e-3, bn_momentum: float = 0.99, name: str = "dlrm", fused_kernels: bool = False,
+                 dcn_num_layers: int = 3, dcn_low_rank_dim: int = 512):
         super().__init__()
         self.fused_kernels = fused_kernels
         import copy
@@ -86,9 +90,15 @@ class DLRM(nn.Module):
             k = n
         self.top = nn.Sequential(*layers)
         self.logits = nn.Linear(k, 1, device=device)
+        if interaction_op == "dcnv2":     # low-rank cross net (modelzoo/mlperf/train.py _make_low_rank_cross_net): V_l without bias, W_l with
+            n = embedding_dim * (T + 1)
+            self.cross_v = nn.ModuleList([nn.Linear(n, dcn_low_rank_dim, bias=False, device=device) for _ in range(dcn_num_layers)])
+            self.cross_w = nn.ModuleList([nn.Linear(dcn_low_rank_dim, n, device=device) for _ in range(dcn_num_layers)])
         for m in self.modules():
             if isinstance(m, nn.Linear):
-                nn.init.xavier_uniform_(m.weight); nn.init.zeros_(m.bias)
+                nn.init.xavier_uniform_(m.weight)
+                if m.bias is not None:
+                    nn.init.zeros_(m.bias)
 
     def embedding_variables(self) -> List[EmbeddingVariable]:
         return [t for t in self.tables if isinstance(t, EmbeddingVariable)]
@@ -110,6 +120,10 @@ class DLRM(nn.Module):
                 z = dot_interaction(x, embs)                    # fp32 oracle path
         else:
             z = torch.cat([x, embs.flatten(1)], dim=1)
+            if self.interaction_op == "dcnv2":
+                x0 = z
+                for v, w in zip(self.cross_v, self.cross_w):
+                    z = x0 * w(v(z)) + z
         return self.logits(self.top(z)).squeeze(-1)
 
     def loss(self, dense, ids, labels) -> torch.Tensor:

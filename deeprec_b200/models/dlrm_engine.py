@@ -76,6 +76,32 @@ class DLRMConfig:
     # phase and the GEMM phase of a tile share one 96 KB Z tile in shared memory and run one after the other, so the default step keeps
     # the two kernels.
     fuse_interaction_gemm: bool = False
+    # "dot": the DLRM interaction above.  "dcnv2": DLRM-DCNv2 (modelzoo/mlperf/train.py): x0 = [bottom | emb_0 .. emb_{T-1}] through
+    # dcn_num_layers low-rank cross layers x_{l+1} = x0 * (x_l V_l W_l + b_l) + x_l of rank dcn_low_rank_dim, then the top MLP
+    interaction_op: str = "dot"
+    dcn_num_layers: int = 3
+    dcn_low_rank_dim: int = 512
+
+# MLPerf DLRM-DCNv2 shapes (modelzoo/mlperf/train.py): DLRMConfig(**MLPERF_DCNV2, ...)
+MLPERF_DCNV2 = dict(embedding_dim=128, mlp_bot=(512, 256, 128), mlp_top=(1024, 1024, 512, 256), interaction_op="dcnv2", dcn_num_layers=3,
+                    dcn_low_rank_dim=512)
+
+
+def _check_interaction(cfg: DLRMConfig, comm) -> None:
+    if cfg.interaction_op == "dot":
+        return
+    if cfg.interaction_op != "dcnv2":
+        raise ValueError(f"interaction_op must be 'dot' or 'dcnv2', got {cfg.interaction_op!r}")
+    if cfg.embedding_dim not in (16, 32, 64, 128):
+        raise ValueError(f"dcnv2: embedding_dim must be 16, 32, 64 or 128, got {cfg.embedding_dim}")
+    if cfg.mlp_bot[-1] != cfg.embedding_dim:
+        raise ValueError("dcnv2: the bottom MLP output must equal embedding_dim (it is column block 0 of x0)")
+    if cfg.fuse_interaction_gemm:
+        raise ValueError("dcnv2: fuse_interaction_gemm fuses the dot interaction only")
+    if comm is not None and not getattr(comm, "unique_first", False):
+        raise ValueError("dcnv2: needs the unique-first sparse pipeline (the NCCL baseline comm runs the dot interaction only)")
+    if cfg.dcn_num_layers < 1 or cfg.dcn_low_rank_dim <= 0 or cfg.dcn_low_rank_dim % 8:
+        raise ValueError("dcnv2: dcn_num_layers >= 1 and dcn_low_rank_dim a positive multiple of 8")
 
 
 def _pad8(n: int) -> int:
@@ -91,7 +117,9 @@ class _Layer:
 
 class DLRMEngine:
     def __init__(self, cfg: DLRMConfig, device: Optional[torch.device] = None, rank: int = 0, world_size: int = 1, comm=None):
+        _check_interaction(cfg, comm)
         self.cfg = cfg
+        self.dcn = cfg.interaction_op == "dcnv2"
         self.rank, self.world = rank, world_size
         self.emu = _native.emu_active()          # CPU CI: the same launch sequence on the CUDA-on-CPU emulation (eager, one stream, no CUDA graph)
         self.dev = torch.device("cpu") if self.emu else (torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device()))
@@ -131,7 +159,7 @@ class DLRMEngine:
         for i, n in enumerate(cfg.mlp_bot):
             self.bot.append(_Layer(f"mlp_bot_{i}", n, k, True)); k = n
         F = self.T + 1
-        self.inter_dim = cfg.embedding_dim + F * (F - 1) // 2
+        self.inter_dim = F * cfg.embedding_dim if self.dcn else cfg.embedding_dim + F * (F - 1) // 2
         self.Zp = _pad8(self.inter_dim)
         self.top: List[_Layer] = []
         k = self.inter_dim
@@ -140,6 +168,12 @@ class DLRMEngine:
         self.head_K = k
         if cfg.mlp_bot[-1] != cfg.embedding_dim:
             raise ValueError("bottom MLP output must equal embedding_dim for the dot interaction")
+        # low-rank cross layers (dcnv2): V_l [rank, inter_dim] (no bias) and W_l [inter_dim, rank] + b_l, stored [N_out, K_in] like every Linear
+        self.cross: List[tuple] = []
+        for l in range(cfg.dcn_num_layers if self.dcn else 0):
+            self.cross.append((_Layer(f"low_rank_cross_net_{l}_v", cfg.dcn_low_rank_dim, self.inter_dim, False),
+                               _Layer(f"low_rank_cross_net_{l}_w", self.inter_dim, cfg.dcn_low_rank_dim, False)))
+        self.xlayers: List[_Layer] = [L for pair in self.cross for L in pair]
         off = 0
         self.views: Dict[str, tuple] = {}
 
@@ -152,11 +186,13 @@ class DLRMEngine:
             take(L.name + "/kernel", L.N * L.Kp); take(L.name + "/bias", L.N)
             if L.has_bn:
                 take(L.name + "/bn_gamma", L.N); take(L.name + "/bn_beta", L.N)
+        for V, W in self.cross:
+            take(V.name + "/kernel", V.N * V.Kp); take(W.name + "/kernel", W.N * W.Kp); take(W.name + "/bias", W.N)
         take("logits/kernel", self.head_K); take("logits/bias", 4)
         self.P = off
         g = torch.Generator(device="cpu").manual_seed(cfg.seed)
         flat = torch.zeros(self.P, dtype=torch.float32)
-        for L in self.bot + self.top:
+        for L in self.bot + self.top + self.xlayers:
             o, n = self.views[L.name + "/kernel"]
             lim = math.sqrt(6.0 / (L.K + L.N))                      # glorot_uniform (tf.layers.dense default)
             w = torch.zeros(L.N, L.Kp)
@@ -172,7 +208,7 @@ class DLRMEngine:
         self.s0 = torch.full((self.P,), slot0_init(self.kind, cfg.initial_accumulator_value), dtype=torch.float32, device=dev) if ns > 0 else None
         self.s1 = torch.zeros(self.P, dtype=torch.float32, device=dev) if ns > 1 else None
         # bf16 shadows for the wgmma GEMMs: W [N, Kp] and W^T [Kp, Np]
-        for L in self.bot + self.top:
+        for L in self.bot + self.top + self.xlayers:
             L.w_bf16 = torch.zeros(L.N, L.Kp, dtype=torch.bfloat16, device=dev)
             L.wt_bf16 = torch.zeros(L.Kp, L.Np, dtype=torch.bfloat16, device=dev)
             if L.has_bn:
@@ -242,7 +278,18 @@ class DLRMEngine:
         self.x0 = z(B, _pad8(self.cfg.num_dense))
         for L in self.bot:
             L.a = z(B, L.N); L.y = z(B, L.N); L.dy = z(B, L.N); L.da = z(B, L.N)
-        self.Z = z(B, self.Zp); self.dZ = z(B, self.Zp)
+        if self.dcn:
+            # x_0 .. x_L [B, (T + 1) D]: x_0 is assembled in place (bottom output | gathered rows), x_L feeds the top MLP.  u_l = x_l V_l W_l + b_l
+            # and t_l = x_l V_l are kept for the backward; g ping-pongs dL/dx_l, dx0 accumulates the x0-factor gradients in fp32.
+            N, r, nl = self.inter_dim, self.cfg.dcn_low_rank_dim, len(self.cross)
+            self.xs = [z(B, N) for _ in range(nl + 1)]
+            self.us = [z(B, N) for _ in range(nl)]
+            self.ts = [z(B, r) for _ in range(nl)]
+            self.gbuf = [z(B, N), z(B, N)]
+            self.du, self.dt, self.dx0 = z(B, N), z(B, r), z(B, N, dt=f32)
+            self.Z = self.xs[-1]; self.dZ = z(B, self.Zp)
+        else:
+            self.Z = z(B, self.Zp); self.dZ = z(B, self.Zp)
         for L in self.top:
             L.a = z(B, L.N); L.da = z(B, L.N)
         self.prob = z(B, dt=f32)
@@ -296,7 +343,7 @@ class DLRMEngine:
         self._call(self.lib.dr_cuda_gemm_dw, ptr(dY), ldy, ptr(X), ldx, self.B, n_out, k_in, ptr(dW), ldw, 0)
 
     def _pack_weights(self) -> None:
-        for L in self.bot + self.top:
+        for L in self.bot + self.top + self.xlayers:
             self._call(self.lib.dr_cuda_pack_weights, ptr(self.p(L.name + "/kernel")), L.N, L.Kp, ptr(L.w_bf16), ptr(L.wt_bf16), L.Np)
 
     # ------------------------------------------------------------------------------------------------
@@ -380,12 +427,13 @@ class DLRMEngine:
             if i + 1 < nb:
                 self._bn_fold(L, self.bot[i + 1], train)
                 x, ldx = L.a, L.N
-            else:   # last bottom layer: its normalised output feeds the interaction, materialise it ([B, 16] only)
+            else:   # last bottom layer: its normalised output feeds the interaction, materialise it ([B, D] only; dcnv2: columns [0, D) of x0)
                 self._call(lib.dr_cuda_bn_finalize, ptr(L.S1), ptr(L.S2), L.N, B, ptr(self.p(L.name + "/bn_gamma")), ptr(self.p(L.name + "/bn_beta")),
                            cfg.bn_eps, cfg.bn_momentum, ptr(L.running_mean), ptr(L.running_var), ptr(L.mean), ptr(L.rstd), ptr(L.scale),
                            ptr(L.shift), int(train))
-                self._call(lib.dr_cuda_bn_apply, ptr(L.a), B, L.N, L.N, ptr(L.scale), ptr(L.shift), ptr(L.y), L.N)
-                x, ldx = L.y, L.N
+                y, ldy = (self.xs[0], self.inter_dim) if self.dcn else (L.y, L.N)
+                self._call(lib.dr_cuda_bn_apply, ptr(L.a), B, L.N, L.N, ptr(L.scale), ptr(L.shift), ptr(y), ldy)
+                x, ldx = y, ldy
         self._tick("f_bot")
         return x, ldx
 
@@ -393,7 +441,10 @@ class DLRMEngine:
         lib, B, cfg = self.lib, self.B, self.cfg
         # ---- interaction + top MLP
         fused0 = self.uf and cfg.fuse_interaction_gemm and self.D == 16 and self.top[0].N <= 512 and self.inter_dim <= 384 and not self.emu
-        if fused0:    # gather + Gram + lower-triangle pack + Linear(512) + ReLU in one kernel; Z only leaves the SM as a TMA store for the backward
+        if self.dcn:  # the gathered rows complete x0 (the kernel waits for every owner's ROWS flag), then the cross layers
+            self.sp.gather_pitched(self.xs[0][:, self.D:])
+            self._cross_forward(train)
+        elif fused0:    # gather + Gram + lower-triangle pack + Linear(512) + ReLU in one kernel; Z only leaves the SM as a TMA store for the backward
             L0 = self.top[0]
             self._call(lib.dr_cuda_dlrm_inter_gemm, ptr(x), ldx, ptr(self.sp.urow), ptr(self.sp.inv), self.sp.ldinv, self.T, self.D, B, ptr(L0.w_bf16), L0.Kp,
                        L0.N, ptr(self.p(L0.name + "/bias")), ptr(L0.a), L0.N, ptr(self.Z) if train else None, self.Zp, self.sp.sync_ref())
@@ -417,6 +468,33 @@ class DLRMEngine:
                 self._gemm(x, ldx, L.w_bf16, L.Kp, B, L.N, L.Kp, self.p(L.name + "/bias"), True, None, 0, L.a, L.N)
             x, ldx = L.a, L.N
         self._tick("f_top")
+
+    def _cross_forward(self, train: bool) -> None:
+        """x_{l+1} = x0 * (t_l W_l^T + b_l) + x_l with t_l = x_l V_l^T: a plain GEMM, then a GEMM whose epilogue applies the cross (and keeps u_l)."""
+        B, N, x0 = self.B, self.inter_dim, self.xs[0]
+        for l, (V, W) in enumerate(self.cross):
+            self._gemm(self.xs[l], N, V.w_bf16, V.Kp, B, V.N, V.Kp, None, False, None, 0, self.ts[l], V.N)
+            self._call(self.lib.dr_cuda_gemm_tn_cross, ptr(self.ts[l]), V.N, ptr(W.w_bf16), W.Kp, B, N, W.Kp, ptr(self.p(W.name + "/bias")), 1,
+                       ptr(x0), N, ptr(self.xs[l]), N, ptr(self.xs[l + 1]), N, ptr(self.us[l]) if train else None, N, self._ctas)
+
+    def _cross_backward(self) -> None:
+        """dL/dx_L (dZ) back through the cross layers -> dy of the last bottom layer and the feature-major demb."""
+        lib, B, N, x0 = self.lib, self.B, self.inter_dim, self.xs[0]
+        g, nl = self.dZ, len(self.cross)
+        for l in range(nl - 1, -1, -1):
+            V, W = self.cross[l]
+            # du = g * x0, dx0 (+)= g * u_l, db_l += column sums of du
+            self._call(lib.dr_cuda_cross_bwd, ptr(g), N, ptr(x0), N, ptr(self.us[l]), N, B, N, ptr(self.du), N, ptr(self.dx0), N, int(l == nl - 1),
+                       ptr(self.g(W.name + "/bias")))
+            self._gemm_dw(self.du, N, self.ts[l], V.N, W.N, W.Kp, self.g(W.name + "/kernel"), W.Kp)          # dW_l += du^T t_l
+            self._gemm(self.du, N, W.wt_bf16, W.Np, B, V.N, N, None, False, None, 0, self.dt, V.N)            # dt = du W_l
+            self._gemm_dw(self.dt, V.N, self.xs[l], N, V.N, V.Kp, self.g(V.name + "/kernel"), V.Kp)         # dV_l += dt^T x_l
+            gn = self.gbuf[l % 2]                                                                             # dx_l = g + dt V_l
+            self._call(lib.dr_cuda_gemm_tn_cross, ptr(self.dt), V.N, ptr(V.wt_bf16), V.Np, B, N, V.N, None, 2, None, 0, ptr(g), N, ptr(gn), N, None, 0,
+                       self._ctas)
+            g = gn
+        last = self.bot[-1]
+        self._call(lib.dr_cuda_cross_split, ptr(self.dx0), N, ptr(g), N, B, self.T, self.D, ptr(last.dy), last.N, ptr(self.demb))
 
     def _head(self, train: bool) -> None:
         h = self.top[-1]
@@ -445,7 +523,9 @@ class DLRMEngine:
         self._tick("b_top")
         # ---- interaction backward -> dy of the last bottom layer, demb (feature-major)
         last = self.bot[-1]
-        if self.uf and self.emu:
+        if self.dcn:
+            self._cross_backward()
+        elif self.uf and self.emu:
             self._call(lib.dr_cuda_dot_interaction_bwd, ptr(self.dZ), self.Zp, ptr(last.y), last.N, ptr(self._emb_g), self.D, self.T * self.D, self.T, self.D, B,
                        ptr(last.dy), last.N, ptr(self.demb), B * self.D, self.D)
         elif self.uf:   # features gathered through inv; per-sample gradient rows -> demb (pre-reduced per key by k_sp_segsum on the side stream)

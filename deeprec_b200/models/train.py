@@ -52,6 +52,9 @@ def get_arg_parser():
     p.add_argument("--timeline", type=int, default=0)
     p.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
     p.add_argument("--engine", action="store_true", help="fused sm_90a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / DIN / DIEN / BST, and DSSM / ESMM / MMoE / DBMTL / PLE / SimpleMultiTask over pooled history bags, through FusedRecEngine (models/rec_engine.py)")
+    p.add_argument("--interaction_op", default="dot", choices=["dot", "dcnv2"],
+                   help="--model dlrm: the dot interaction, or DLRM-DCNv2 (a low-rank cross net; with --engine the MLPerf shapes: D = 128, "
+                        "bottom 512-256-128, top 1024-1024-512-256, 3 cross layers of rank 512)")
     p.add_argument("--log_every", type=int, default=20)
     p.add_argument("--watchdog", type=float, default=0, help="seconds without a finished step before the job dumps stacks and exits 86")
     return p
@@ -69,8 +72,10 @@ def main(argv=None) -> int:
     dev = torch.device(a.device)
     name = a.model.lower()
     if a.engine and name == "dlrm":
-        from deeprec_b200.models.dlrm_engine import CRITEO_KAGGLE_CARDINALITIES, DLRMConfig, DLRMEngine
-        eng = DLRMEngine(DLRMConfig(batch_size=a.batch_size, cardinalities=CRITEO_KAGGLE_CARDINALITIES, optimizer=a.optimizer, learning_rate=a.learning_rate))
+        from deeprec_b200.models.dlrm_engine import CRITEO_KAGGLE_CARDINALITIES, MLPERF_DCNV2, DLRMConfig, DLRMEngine
+        shapes = MLPERF_DCNV2 if a.interaction_op == "dcnv2" else {}
+        eng = DLRMEngine(DLRMConfig(batch_size=a.batch_size, cardinalities=CRITEO_KAGGLE_CARDINALITIES, optimizer=a.optimizer, learning_rate=a.learning_rate,
+                                    **shapes))
         t0 = time.time()
         for s in range(a.steps):
             d, ids, y = criteo_batch(a.batch_size, 13, CRITEO_KAGGLE_CARDINALITIES, seed=s)
@@ -150,7 +155,12 @@ def main(argv=None) -> int:
     from deeprec_b200.models import zoo
     zoo.table_variant("multihash" if a.multihash else "adaptive" if a.adaptive_emb else "ev")
     try:
-        model = build_model(name, ev_option_from_args(a), dev, a.group_embedding or a.emb_fusion, cardinalities=cards)
+        if name == "dlrm" and a.interaction_op == "dcnv2":
+            from deeprec_b200.models.dlrm import DLRM
+            from deeprec_b200.models.dlrm_engine import MLPERF_DCNV2
+            model = DLRM(13, cards, ev_option=ev_option_from_args(a), device=dev, **MLPERF_DCNV2)
+        else:
+            model = build_model(name, ev_option_from_args(a), dev, a.group_embedding or a.emb_fusion, cardinalities=cards)
     finally:
         zoo.table_variant("ev")
     if a.op_fusion:                       # auto graph fusion (do_op_fusion)

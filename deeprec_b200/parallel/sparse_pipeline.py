@@ -186,6 +186,14 @@ class SparsePipeline:
         check(self.lib.dr_sp_gather(ptr(self.urow), ptr(self.inv), self.geom_ref(), ptr(out), self.sync_ref(), stream_ptr(self.dev)), "gather")
         self.launches += 1
 
+    def gather_pitched(self, out: torch.Tensor) -> None:
+        """gather into the first C * dim columns of a wider row: out[b, c * dim: (c + 1) * dim] = urow[inv[b, c]] (out: a bf16 [B, >= C * dim]
+        view whose rows may be longer, e.g. the embedding columns of DLRM-DCNv2's x0)."""
+        assert out.dim() == 2 and out.shape[0] == self.B and out.shape[1] >= self.C * self.dim and out.dtype == torch.bfloat16 and out.stride(1) == 1
+        check(self.lib.dr_sp_gather_pitched(ptr(self.urow), ptr(self.inv), self.geom_ref(), C.c_void_p(out.data_ptr()), out.stride(0),
+                                            self.sync_ref(), stream_ptr(self.dev)), "gather_pitched")
+        self.launches += 1
+
     def segsum(self, demb: torch.Tensor) -> None:
         """Requester side: pre-reduce the per-sample gradient rows (bf16 [C, B, dim]) per distinct key into ugrad; raises GRAD."""
         assert demb.shape == (self.C, self.B, self.dim) and demb.dtype == torch.bfloat16

@@ -32,8 +32,16 @@ def _write_versions(root: str, full: Optional[dict] = None, delta: Optional[dict
     os.replace(tmp, p)
 
 
+def _check_exportable(engine) -> None:
+    # the "dlrm" saved-model format and the Processors know the dot interaction only: a DLRM-DCNv2 export would be served without its
+    # cross layers, i.e. as a different model
+    if getattr(engine.cfg, "interaction_op", "dot") != "dot":
+        raise ValueError(f"serving export of a DLRMEngine with interaction_op={engine.cfg.interaction_op!r} is not supported")
+
+
 def export_saved_model(engine, export_dir: str, version: Optional[int] = None, root: Optional[str] = None) -> str:
     """Full export of a :class:`DLRMEngine` (rank-local tables; rank 0 also writes the dense block)."""
+    _check_exportable(engine)
     cfg = engine.cfg
     version = int(version if version is not None else engine.global_step())
     os.makedirs(os.path.join(export_dir, "variables"), exist_ok=True)
@@ -61,6 +69,7 @@ def export_saved_model(engine, export_dir: str, version: Optional[int] = None, r
 
 def export_delta(engine, root: str, base_version: int, version: Optional[int] = None) -> str:
     """Incremental export: rows touched since the last export + the (small) dense block."""
+    _check_exportable(engine)
     version = int(version if version is not None else engine.global_step())
     d = os.path.join(root, ".incr")
     os.makedirs(d, exist_ok=True)
