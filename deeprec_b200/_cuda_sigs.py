@@ -165,6 +165,7 @@ _sig("dr_ag_sizeof_geom", [])
 _sig("dr_cuda_set_device", [INT])
 _sig("dr_cuda_get_device", [])
 _sig("dr_cuda_set_sparse_blocks_per_sm", [INT])
+_sig("dr_cuda_set_sparse_sms", [INT])
 _sig("dr_cuda_sm_partition", [INT, INT, C.POINTER(INT), C.POINTER(vp)])
 _sig("dr_cuda_graph_kernel_contexts", [P, C.POINTER(vp), INT])
 _sig("dr_comm_alloc", [i64, C.POINTER(vp)])

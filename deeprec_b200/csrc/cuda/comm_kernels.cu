@@ -83,6 +83,7 @@ extern "C" {
 // ---- device / IPC plumbing (this library links its own static cudart: make its current device explicit) ----------
 int dr_cuda_set_device(int dev) { DR_CUDA_CHECK(cudaSetDevice(dev)); return 0; }
 int dr_cuda_set_sparse_blocks_per_sm(int n) { sparse_blocks_per_sm() = n < 1 ? 1 : n; return 0; }
+int dr_cuda_set_sparse_sms(int n) { sparse_grid_sms() = n < 0 ? 0 : n; return 0; }
 int dr_cuda_get_device() { int d = -1; cudaGetDevice(&d); return d; }
 
 int dr_comm_alloc(int64_t bytes, void** out) {

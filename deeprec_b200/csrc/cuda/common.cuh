@@ -87,6 +87,10 @@ struct DrPerDeviceOnce {
 // sparse blocks cannot also take a wgmma GEMM CTA (384 threads, up to 168 registers each, ~200 KB smem), so next to the GEMMs the two
 // streams share SMs only one at a time; DLRMConfig.sparse_sms gives the sparse kernels SMs of their own instead (sm_partition.cu).
 inline int& sparse_blocks_per_sm() { static int v = 16; return v; }
+// SMs the sparse-path grids are sized for (0 = every SM of the device).  DLRMEngine sets its sparse partition's SM count while it enqueues
+// the side stream of an overlap window: a grid sized to the whole GPU would end in a partial wave on the partition's SMs.
+inline int& sparse_grid_sms() { static int v = 0; return v; }
+inline int sparse_sm_count() { return sparse_grid_sms() > 0 ? sparse_grid_sms() : num_sms(); }
 constexpr int64_t kEmptyKey = INT64_MIN;
 constexpr int64_t kTombKey = INT64_MIN + 1;
 

@@ -238,7 +238,7 @@ __global__ void __launch_bounds__(256) k_dense_apply(float* __restrict__ w, cons
 }
 
 inline int grid_for(int64_t n, int block, int max_blocks = 0) {
-  if (max_blocks <= 0) max_blocks = num_sms() * sparse_blocks_per_sm();
+  if (max_blocks <= 0) max_blocks = sparse_sm_count() * sparse_blocks_per_sm();
   int64_t b = (n + block - 1) / block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -275,7 +275,7 @@ int dr_cuda_sparse_accumulate(const DrDeviceTable* tables_dev, const int32_t* ta
 int dr_cuda_sparse_apply(const DrDeviceTable* tables_dev, const int64_t* ulist, int32_t* n_unique_dev, int64_t ulist_cap,
                          float* gsum, int dim, const DrOptHyper* hp_dev, int64_t max_unique, int reset_counter, cudaStream_t s) {
   int lpr = lanes_for(dim);
-  int grid = grid_for(max_unique * lpr, 256, num_sms() * (sparse_blocks_per_sm() < 8 ? sparse_blocks_per_sm() : 8));
+  int grid = grid_for(max_unique * lpr, 256, sparse_sm_count() * (sparse_blocks_per_sm() < 8 ? sparse_blocks_per_sm() : 8));
   switch (lpr) {
     case 1: DR_PDL_LAUNCH((k_apply<1>), grid, 256, 0, s, tables_dev, ulist, n_unique_dev, ulist_cap, gsum, dim, hp_dev); break;
     case 2: DR_PDL_LAUNCH((k_apply<2>), grid, 256, 0, s, tables_dev, ulist, n_unique_dev, ulist_cap, gsum, dim, hp_dev); break;

@@ -323,21 +323,28 @@ __global__ void __launch_bounds__(256) k_sp_lookup(const DrDeviceTable* __restri
 // k_sp_segsum (requester): ugrad[gs] += per-sample gradient rows, pre-reduced per distinct key BEFORE anything crosses NVLink
 // (the reference sums duplicates with unique + unsorted_segment_sum on the OWNER after shipping every row:
 // all2all_output_dispatcher.cu:233-246, kit_cc/framework/compat/kernels/unsorted_segment_sum.cu).
-// One warp = 32 consecutive samples of one id column (coalesced 32 B bf16 rows of the feature-major demb buffer).  Lanes holding
-// the same key are found with match.any; every group's leader sums its members' rows out of a 1 KB shared-memory tile and issues
-// ONE vectorised L2 reduction per 16 B chunk -- no shared-memory atomics (fp32 ATOMS are CAS loops), no sort.
+// One warp = 32 consecutive samples of one id column (coalesced bf16 rows of the feature-major demb buffer, staged in shared memory).
+// Lanes holding the same key are found with match.any.  The tile's key groups are then summed with the lanes on consecutive elements of
+// a row: a lane adds one element of its group's members in ascending lane order (an fp32 sum from 0, so the bits do not depend on how
+// lanes are assigned), converts it to fixed point and reduces it into ugrad.  One reduction instruction covers whole rows (two 128 B rows
+// at dim 16) instead of 32 scattered 8-byte ones; no shared-memory atomics (fp32 ATOMS are CAS loops), no sort.
+// Rows wider than 64 (dim 128) are staged and summed in 64-wide passes: a whole tile would need 64 KB of shared memory.
 // -----------------------------------------------------------------------------------------------------------------
-// Rows wider than 64 (dim 128): the tile of a whole row would need 64 KB of shared memory and the leader 128 accumulators, so the row is
-// summed in 64-wide passes over the same key groups.  The 64-bit fixed-point L2 reductions make the result independent of the split.
-template <int LPR>
-__device__ __forceinline__ void sp_segsum_passes(const __nv_bfloat16* __restrict__ demb, const int32_t* __restrict__ invT, const DrSpGeom& g,
-                                                 unsigned long long* __restrict__ ugrad) {
+template <int LPR /* dim / 4 */>
+__global__ void __launch_bounds__(256) k_sp_segsum(const __nv_bfloat16* __restrict__ demb /* [C][B][dim] */, const int32_t* __restrict__ invT /* [C][B] */,
+                                                   DrSpGeom g, unsigned long long* __restrict__ ugrad, DrSpSync sync) {
+  pdl_sync();
   constexpr int dim = 4 * LPR;
-  constexpr int PD = 64;                                       // columns per pass
-  constexpr int V = PD / 8;
+  constexpr int PD = dim < 64 ? dim : 64;                      // row elements per pass
+  constexpr int V = PD / 8;                                    // int4 (8 bf16) chunks per row and pass
+  constexpr int EL = PD < 32 ? PD : 32;                        // lanes per row
+  constexpr int EPL = PD / EL;                                 // elements per lane
+  constexpr int RPI = 32 / EL;                                 // rows per reduction instruction
   static_assert(dim % PD == 0, "dim: a multiple of the pass width");
   __shared__ __align__(16) int4 s_row[8][32][V];
+  __shared__ int32_t s_lead[8][32];                            // lane of the j-th key group's leader (groups in ascending leader lane)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int sub = lane / EL, e0 = lane % EL;
   const int64_t tiles = (g.B + 31) / 32;
   const int64_t units = tiles * g.C;
   for (int64_t u = (int64_t)blockIdx.x * 8 + warp; u < units; u += (int64_t)gridDim.x * 8) {
@@ -349,7 +356,10 @@ __device__ __forceinline__ void sp_segsum_passes(const __nv_bfloat16* __restrict
     const unsigned lm = __ballot_sync(0xffffffffu, live);
     unsigned same = 0;
     if (live) same = __match_any_sync(lm, gs);
-    const bool leader = live && lane == __ffs(same) - 1;       // leader of this key inside the tile
+    const bool leader = live && lane == __ffs(same) - 1;
+    const unsigned lead = __ballot_sync(0xffffffffu, leader);
+    if (leader) s_lead[warp][__popc(lead & ((1u << lane) - 1u))] = lane;
+    const int ngroups = __popc(lead);
     for (int p = 0; p < dim / PD; ++p) {
       if (live) {
         const int4* src = reinterpret_cast<const int4*>(demb + ((int64_t)c * g.B + b) * dim + p * PD);
@@ -357,78 +367,27 @@ __device__ __forceinline__ void sp_segsum_passes(const __nv_bfloat16* __restrict
         for (int v = 0; v < V; ++v) s_row[warp][lane][v] = ld_nc_v4(src + v);
       }
       __syncwarp();
-      if (leader) {
-        float acc[PD];
+      for (int j0 = 0; j0 < ngroups; j0 += RPI) {
+        const int j = j0 + sub;
+        const int ll = s_lead[warp][j < ngroups ? j : j0];
+        const unsigned members = __shfl_sync(0xffffffffu, same, ll);
+        const int32_t key = __shfl_sync(0xffffffffu, gs, ll);
+        if (j < ngroups) {
+          float acc[EPL];
 #pragma unroll
-        for (int d = 0; d < PD; ++d) acc[d] = 0.f;
-        for (unsigned m = same; m; m &= m - 1) {
-          const int src_lane = __ffs(m) - 1;
+          for (int k = 0; k < EPL; ++k) acc[k] = 0.f;
+          for (unsigned m = members; m; m &= m - 1) {
+            const uint16_t* r = reinterpret_cast<const uint16_t*>(s_row[warp][__ffs(m) - 1]);
 #pragma unroll
-          for (int v = 0; v < V; ++v) {
-            const int4 raw = s_row[warp][src_lane][v];
-            const uint32_t w[4] = {(uint32_t)raw.x, (uint32_t)raw.y, (uint32_t)raw.z, (uint32_t)raw.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) { const float2 f = unpack_bf16x2(w[e]); acc[8 * v + 2 * e] += f.x; acc[8 * v + 2 * e + 1] += f.y; }
+            for (int k = 0; k < EPL; ++k) acc[k] += __uint_as_float((uint32_t)r[e0 + EL * k] << 16);      // bf16 -> fp32 is exact
           }
-        }
-        unsigned long long* dst = ugrad + (int64_t)gs * dim + p * PD;
+          unsigned long long* dst = ugrad + (int64_t)key * dim + p * PD + e0;
 #pragma unroll
-        for (int d = 0; d < PD; ++d) atomicAdd(dst + d, ugrad_fix(acc[d]));
+          for (int k = 0; k < EPL; ++k) atomicAdd(dst + EL * k, ugrad_fix(acc[k]));
+        }
       }
       __syncwarp();
     }
-  }
-}
-
-template <int LPR /* dim / 4 */>
-__global__ void __launch_bounds__(256) k_sp_segsum(const __nv_bfloat16* __restrict__ demb /* [C][B][dim] */, const int32_t* __restrict__ invT /* [C][B] */,
-                                                   DrSpGeom g, unsigned long long* __restrict__ ugrad, DrSpSync sync) {
-  pdl_sync();
-  constexpr int dim = 4 * LPR;
-  if constexpr (dim > 64) {
-    sp_segsum_passes<LPR>(demb, invT, g, ugrad);
-  } else {
-  constexpr int V = dim / 8;                                   // int4 (8 bf16) chunks per row
-  __shared__ __align__(16) int4 s_row[8][32][V];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t tiles = (g.B + 31) / 32;
-  const int64_t units = tiles * g.C;
-  for (int64_t u = (int64_t)blockIdx.x * 8 + warp; u < units; u += (int64_t)gridDim.x * 8) {
-    const int c = (int)(u / tiles);
-    const int64_t b = (u % tiles) * 32 + lane;
-    int32_t gs = -1;
-    if (b < g.B) gs = invT[(int64_t)c * g.B + b];
-    const bool live = gs >= 0;
-    const unsigned lm = __ballot_sync(0xffffffffu, live);
-    if (live) {
-      const int4* src = reinterpret_cast<const int4*>(demb + ((int64_t)c * g.B + b) * dim);
-#pragma unroll
-      for (int v = 0; v < V; ++v) s_row[warp][lane][v] = ld_nc_v4(src + v);
-    }
-    __syncwarp();
-    if (live) {
-      const unsigned same = __match_any_sync(lm, gs);
-      if (lane == __ffs(same) - 1) {                            // leader of this key inside the tile
-        float acc[dim];
-#pragma unroll
-        for (int d = 0; d < dim; ++d) acc[d] = 0.f;
-        for (unsigned m = same; m; m &= m - 1) {
-          const int src_lane = __ffs(m) - 1;
-#pragma unroll
-          for (int v = 0; v < V; ++v) {
-            const int4 raw = s_row[warp][src_lane][v];
-            const uint32_t w[4] = {(uint32_t)raw.x, (uint32_t)raw.y, (uint32_t)raw.z, (uint32_t)raw.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) { const float2 f = unpack_bf16x2(w[e]); acc[8 * v + 2 * e] += f.x; acc[8 * v + 2 * e + 1] += f.y; }
-          }
-        }
-        unsigned long long* dst = ugrad + (int64_t)gs * dim;
-#pragma unroll
-        for (int d = 0; d < dim; ++d) atomicAdd(dst + d, ugrad_fix(acc[d]));
-      }
-    }
-    __syncwarp();
-  }
   }
   sp_signal_last_block(sync, SP_CH_GRAD);
 }
@@ -711,7 +670,7 @@ __global__ void k_sp_stats(DrSpGeom g, const int32_t* __restrict__ bcnt, int64_t
 }
 
 inline int sp_grid(int64_t blocks) {
-  const int64_t cap = (int64_t)num_sms() * sparse_blocks_per_sm();
+  const int64_t cap = (int64_t)sparse_sm_count() * sparse_blocks_per_sm();
   if (blocks < 1) blocks = 1;
   return (int)(blocks > cap ? cap : blocks);
 }

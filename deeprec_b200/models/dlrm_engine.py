@@ -70,7 +70,8 @@ class DLRMConfig:
     sparse_blocks_per_sm: int = 4               # resident-block budget of the side-stream sparse kernels
     # SMs of the green context the embedding branch runs in during the two overlap windows; the bottom MLP gets the rest (csrc/cuda/
     # sm_partition.cu).  Rounded by the driver (multiples of 8 on Hopper).  0 = both branches share every SM as two streams of one context.
-    sparse_sms: int = 48
+    # 40 balances both windows at the bench shapes on an H100 SXM (DESIGN.md: SM partition).
+    sparse_sms: int = 40
     gemm_v1: bool = False                       # A/B switch: separate statistics passes instead of the statistics fused into the GEMM epilogue
     # combine + dot interaction + top-MLP layer 0 in ONE tensor-core kernel (csrc/cuda/fused_interaction_gemm.cu).  Opt-in: the builder
     # phase and the GEMM phase of a tile share one 96 KB Z tile in shared memory and run one after the other, so the default step keeps
@@ -378,6 +379,7 @@ class DLRMEngine:
         self._side.wait_stream(main)
         if self._dense is not None:
             self._dense.wait_stream(main)
+            self.lib.dr_cuda_set_sparse_sms(self.partition_sms[0])     # side-stream grids: one wave on the sparse partition
 
     def _dense_window(self):
         if self._dense is None:
@@ -390,6 +392,7 @@ class DLRMEngine:
         if self._dense is not None:
             main.wait_stream(self._dense)
             self._ctas = 0
+            self.lib.dr_cuda_set_sparse_sms(0)
 
     def _forward(self, train: bool) -> None:
         cfg = self.cfg
