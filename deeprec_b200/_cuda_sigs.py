@@ -76,6 +76,7 @@ _sig("dr_cuda_table_rehash", [TP, TP, S])
 _sig("dr_cuda_table_shrink", [TP, INT, P, S])
 _sig("dr_cuda_table_remove", [TP, P, i64, P, S])
 _sig("dr_cuda_table_snapshot", [TP, INT, INT, INT, P, P, P, P, P, P, P, P, S])
+_sig("dr_cuda_table_snapshot_since", [TP, i64, P, P, P, P, P, S])
 _sig("dr_cuda_table_export_keys", [TP, P, i64, P, P, P, P, S])
 _sig("dr_cuda_table_clear_dirty", [TP, S])
 _sig("dr_cuda_table_import", [TP, P, P, INT, P, P, i64, INT, INT, INT, P, S])

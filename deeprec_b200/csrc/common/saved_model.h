@@ -28,12 +28,13 @@ inline int pad8(int n) { return (n + 7) / 8 * 8; }
 // Op program (saved_model.json "arch": "program", serving/export.py::export_saved_model_program): the inference graph of a model other than
 // DLRM as a list of ops over [B, width] buffers; buffer 0 = dense inputs, buffer 1 = embeddings [B, C * D].
 enum POpKind { P_CONCAT, P_LINEAR, P_AFFINE, P_FM, P_CROSS, P_MUL_ADD, P_ADD, P_LAYERNORM, P_MUL, P_SLICE,
-               P_VALID_MASK, P_SEQ_ZIP, P_SEQ_MASK, P_SEQ_SUM, P_DIN_ATT, P_PRELU, P_SOFTMAX, P_COSINE, P_TILE, P_GRU, P_SEQ_LAST, P_MHA, P_SEQ_MEAN, P_NUM_OPS };
+               P_VALID_MASK, P_SEQ_ZIP, P_SEQ_MASK, P_SEQ_SUM, P_DIN_ATT, P_PRELU, P_SOFTMAX, P_COSINE, P_TILE, P_GRU, P_SEQ_LAST, P_MHA, P_SEQ_MEAN,
+               P_CROSS_LINEAR, P_NUM_OPS };
 // rows1: sample-aware graph compression (serving/export.py::compress_sample_aware) -- the op depends on user-side features only, which are
 // identical for every candidate row of a ranking request: it runs at batch 1 on row 0 of its inputs; a TILE op broadcasts row 0 to the batch
 // where a per-candidate op consumes the result (reference: python/graph_optimizer/sample_awared_graph_compression.py:26).
 // len on LINEAR / LAYERNORM: the op is applied at each of `len` positions of a [B, len * w] sequence buffer (DIEN / BST); mode: din_attention output
-// (0 = weighted sum of the keys, 1 = the softmax weights); heads: mha
+// (0 = weighted sum of the keys, 1 = the softmax weights), seq_mean divisor (0 = count, 1 = sqrt(count): the sqrtn combiner); heads: mha
 struct POp { int kind = 0, out = 0; std::vector<int> in; bool relu = false, rows1 = false; float eps = 1e-5f; int start = 0, len = 0, mode = 0, heads = 1; std::string name; };
 struct Arch {
   int num_dense = 13, T = 0, D = 16; std::vector<int> bot, top; float bn_eps = 1e-3f; int inter = 0, Zp = 0;     // Zp: interaction width padded to 8
@@ -93,8 +94,9 @@ inline bool ParseArch(const std::string& dir, Arch* a, int64_t* version, std::st
   std::vector<std::string> names = {"dense", "emb"};
   auto id_of = [&](const std::string& n) { for (size_t i = 0; i < names.size(); ++i) if (names[i] == n) return (int)i; return -1; };
   static const char* kNames[] = {"concat", "linear", "affine", "fm", "cross", "mul_add", "add", "layernorm", "mul", "slice",
-                                 "valid_mask", "seq_zip", "seq_mask", "seq_sum", "din_attention", "prelu", "softmax", "cosine", "tile", "gru", "seq_last", "mha", "seq_mean"};
-  static const int kArity[] = {-1, 1, 1, 1, 2, 3, 2, 1, 2, 1, 1, 2, 2, 1, 3, 1, 1, 2, 1, 1, 2, 2, 2};
+                                 "valid_mask", "seq_zip", "seq_mask", "seq_sum", "din_attention", "prelu", "softmax", "cosine", "tile", "gru", "seq_last", "mha", "seq_mean",
+                                 "cross_linear"};
+  static const int kArity[] = {-1, 1, 1, 1, 2, 3, 2, 1, 2, 1, 1, 2, 2, 1, 3, 1, 1, 2, 1, 1, 2, 2, 2, 3};
   const JVal* pr = j.get("program");
   if (!pr || pr->t != JVal::ARR) return false;
   std::vector<bool> rows1_buf(2, false);
@@ -124,8 +126,8 @@ inline bool ParseArch(const std::string& dir, Arch* a, int64_t* version, std::st
 
 // fp32 tensors of one program op, row-major as exported
 struct OpTensors {
-  int N = 0, K = 0;                       // linear: kernel [N, K], K per position of a sequence | gru: w_ih [3H, I] (N = 3H, K = I)
-  std::vector<float> W, b;                // linear: kernel, bias | gru: w_ih, b_ih
+  int N = 0, K = 0;                       // linear: kernel [N, K], K per position of a sequence | gru: w_ih [3H, I] (N = 3H, K = I) | cross_linear: kernel [N, r] (K = r)
+  std::vector<float> W, b;                // linear, cross_linear: kernel, bias | gru: w_ih, b_ih
   std::vector<float> v0, v1;              // affine, layernorm: scale, shift | cross: w, b | prelu: alpha | gru: w_hh [3H, H], b_hh
   std::vector<std::vector<float>> att;    // din_attention: w1 [H1, 4W] b1 w2 [H2, H1] b2 w3 [H2] b3 [1]
   int H1 = 0, H2 = 0;                     // gru: H1 = H | din_attention: hidden widths
@@ -179,8 +181,16 @@ inline bool ReadProgram(dr::BundleReader& r, const Arch& a, ProgramData* out) {
         t.N = H3; t.K = I; t.H1 = H;
         w = op.len * H; break;
       }
+      case P_SEQ_MEAN: if (op.mode < 0 || op.mode > 1) return false; [[fallthrough]];                            // mean (mode 1: sum / sqrt(count))
       case P_SEQ_LAST:                                               // the state at the last valid position
-      case P_SEQ_MEAN: if (op.len <= 0 || w0 % op.len || w1 != op.len) return false; w = w0 / op.len; break;     // mean over the valid positions
+        if (op.len <= 0 || w0 % op.len || w1 != op.len) return false;
+        w = w0 / op.len; break;
+      case P_CROSS_LINEAR: {                                         // x0 [B, N], x_l [B, N], t [B, r]: x0 * (t kernel^T + bias) + x_l, kernel [N, r]
+        const int rank = width[(size_t)op.in[2]];
+        if (w1 != w0 || !ReadVec(r, base + "kernel", &t.W) || !ReadVec(r, base + "bias", &t.b) || (int)t.b.size() != w0 || t.W.size() != (size_t)w0 * rank) return false;
+        t.N = w0; t.K = rank;
+        break;
+      }
       case P_MHA: {                                                  // qkv [B, S * 3E] (per position [q | k | v]), valid [B, S] -> [B, S * E]
         if (op.len <= 0 || w0 % (3 * op.len) || w1 != op.len) return false;
         const int E = w0 / (3 * op.len);

@@ -277,6 +277,17 @@ __global__ void __launch_bounds__(256) k_prog_seq_mean(const __nv_bfloat16* __re
     stb(y + b * ldy + k, acc / (float)(cnt > 1 ? cnt : 1));
   }
 }
+// y[b, :] = sum over the valid positions of x[b, l, :] / sqrt(count) -- the sqrtn combiner of k_sp_pool; no valid position gives 0
+__global__ void __launch_bounds__(256) k_prog_seq_sqrtn(const __nv_bfloat16* __restrict__ x, int64_t ldx, const __nv_bfloat16* __restrict__ m, int64_t ldm, int L, int w,
+                                                        __nv_bfloat16* __restrict__ y, int64_t ldy, int64_t B) {
+  const int64_t n = B * (int64_t)w;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / w; const int k = (int)(i - b * w);
+    float acc = 0.f; int cnt = 0;
+    for (int l = 0; l < L; ++l) if (ldb(m + b * ldm + l) > 0.f) { acc += ldb(x + b * ldx + (int64_t)l * w + k); ++cnt; }
+    stb(y + b * ldy + k, cnt > 0 ? acc / sqrtf((float)cnt) : 0.f);
+  }
+}
 // multi-head self-attention core: qkv [B, S * 3E] (per position [q | k | v]), valid [B, S] -> [B, S * E].  One block per sample, the sample's qkv
 // staged in shared memory as fp32; one thread per (head, query position) runs an online softmax over the valid keys (dh <= 64).
 constexpr int kMhaMaxDh = 64;
@@ -435,6 +446,12 @@ int dr_prog_seq_last(const void* x, int64_t ldx, const void* m, int64_t ldm, int
 int dr_prog_seq_mean(const void* x, int64_t ldx, const void* m, int64_t ldm, int L, int w, void* y, int64_t ldy, int64_t B, cudaStream_t s) {
   if (B <= 0 || L <= 0 || w <= 0) return 0;
   k_prog_seq_mean<<<grid_el(B * w), 256, 0, s>>>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)m, ldm, L, w, (__nv_bfloat16*)y, ldy, B);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+int dr_prog_seq_sqrtn(const void* x, int64_t ldx, const void* m, int64_t ldm, int L, int w, void* y, int64_t ldy, int64_t B, cudaStream_t s) {
+  if (B <= 0 || L <= 0 || w <= 0) return 0;
+  k_prog_seq_sqrtn<<<grid_el(B * w), 256, 0, s>>>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)m, ldm, L, w, (__nv_bfloat16*)y, ldy, B);
   DR_LAUNCH_CHECK();
   return 0;
 }

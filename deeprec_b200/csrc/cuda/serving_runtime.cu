@@ -78,6 +78,10 @@ int dr_prog_emb_feature_major(const float* x, int T, int D, int64_t B, void* y, 
 int dr_prog_gru(const void* gi, int64_t ldg, const float* whh, const float* bhh, int L, int H, void* y, int64_t ldy, int64_t B, cudaStream_t s);
 int dr_prog_seq_last(const void* x, int64_t ldx, const void* m, int64_t ldm, int L, int w, void* y, int64_t ldy, int64_t B, cudaStream_t s);
 int dr_prog_seq_mean(const void* x, int64_t ldx, const void* m, int64_t ldm, int L, int w, void* y, int64_t ldy, int64_t B, cudaStream_t s);
+int dr_prog_seq_sqrtn(const void* x, int64_t ldx, const void* m, int64_t ldm, int L, int w, void* y, int64_t ldy, int64_t B, cudaStream_t s);
+int dr_cuda_gemm_tn_cross(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* bias, int kind,
+                          const void* x0, int64_t ld_x0, const void* xl, int64_t ld_xl, void* out, int64_t ldc, void* u_out, int64_t ld_u,
+                          int max_ctas, cudaStream_t s);
 int dr_prog_mha(const void* qkv, int64_t ldq, const void* valid, int64_t ldv, int S, int E, int heads, void* y, int64_t ldy, int64_t B, cudaStream_t s);
 int dr_cuda_din_attention_fwd_w(const float* q, const float* k, const uint8_t* mask, int64_t B, int L, int D, const float* W1, const float* b1, int H1,
                                 const float* W2, const float* b2, int H2, const float* w3, float b3, float* out, float* weights_out, cudaStream_t s);
@@ -240,6 +244,20 @@ static bool BuildProgram(dr::BundleReader& r, const Arch& a, std::shared_ptr<Den
         break;
       }
       case P_MHA: if (w0 / (3 * op.len) / op.heads > 64) return false; break;
+      case P_CROSS_LINEAR: {                                         // dr_cuda_gemm_tn_cross over the padded widths: A = t [B, Kp], kernel [Np, Kp], x0 / x_l / out [B, Np]
+        const int N = t.N, K = t.K, Np = prog_npad(N), Kp = prog_ld(a, p.width, op.in[2]);
+        const int64_t ld_x0 = prog_ld(a, p.width, op.in[0]), ld_xl = prog_ld(a, p.width, op.in[1]);
+        if (Kp % 8 || Np % 8 || ld_x0 % 8 || ld_xl % 8 || ld_x0 < Np || ld_xl < Np || Kp < K) {
+          fprintf(stderr, "[deeprec_serving] cross_linear op %s: the cross GEMM needs pitches that are multiples of 8 and at least the padded width "
+                          "(N %d padded to %d, rank %d, pitches x0 %lld, x_l %lld, t %d)\n", op.name.c_str(), N, Np, K, (long long)ld_x0, (long long)ld_xl, Kp);
+          return false;
+        }
+        std::vector<uint16_t> wb((size_t)Np * Kp, 0); std::vector<float> bias((size_t)Np, 0.f);     // zero pad rows / bias: pad outputs stay x_l's zeros
+        for (int n = 0; n < N; ++n) { bias[(size_t)n] = t.b[(size_t)n]; for (int k = 0; k < K; ++k) wb[(size_t)n * Kp + k] = f2bf(t.W[(size_t)n * K + k]); }
+        d.L.N = N; d.L.K = K; d.L.Kp = Kp; d.L.Np = Np;
+        if (!Upload(d.L.w_bf16, wb) || !Upload(d.L.bias, bias)) return false;
+        break;
+      }
       case P_DIN_ATT:
         d.b3 = t.att[5][0]; d.att.resize(5);
         for (int k = 0; k < 5; ++k) if (!Upload(d.att[(size_t)k], t.att[(size_t)k])) return false;
@@ -455,7 +473,14 @@ struct Session {
           break;
         }
         case P_SEQ_LAST: rc |= dr_prog_seq_last(a0, ld0, buf(op.in[1]), ld(op.in[1]), op.len, W, out, ldo, B, s); break;
-        case P_SEQ_MEAN: rc |= dr_prog_seq_mean(a0, ld0, buf(op.in[1]), ld(op.in[1]), op.len, W, out, ldo, B, s); break;
+        case P_SEQ_MEAN:
+          if (op.mode == 1) rc |= dr_prog_seq_sqrtn(a0, ld0, buf(op.in[1]), ld(op.in[1]), op.len, W, out, ldo, B, s);
+          else rc |= dr_prog_seq_mean(a0, ld0, buf(op.in[1]), ld(op.in[1]), op.len, W, out, ldo, B, s);
+          break;
+        case P_CROSS_LINEAR:                                         // x0 * (t W^T + b) + x_l in the GEMM epilogue (the DCNv2 training forward)
+          rc |= dr_cuda_gemm_tn_cross(buf(op.in[2]), ld(op.in[2]), pd.L.w_bf16.p, pd.L.Kp, B, pd.L.Np, pd.L.Kp, pd.L.bias.as<float>(), 1, a0, ld0,
+                                      buf(op.in[1]), ld(op.in[1]), out, ldo, nullptr, 0, 0, s);
+          break;
         case P_MHA: rc |= dr_prog_mha(a0, ld0, buf(op.in[1]), ld(op.in[1]), op.len, W / op.len, op.heads, out, ldo, B, s); break;
         case P_CONCAT: {
           int off = 0;

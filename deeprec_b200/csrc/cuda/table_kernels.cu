@@ -249,6 +249,24 @@ __global__ void k_snapshot(DrDeviceTable TB, int dirty_only, int part_id, int pa
   }
 }
 
+// Snapshot of the admitted keys whose version (the global step of their last update, written by k_apply) is >= min_version: the rows a
+// serving delta needs, selected without reading or clearing the dirty bits that incremental checkpoints consume.  counts[0] = rows.
+__global__ void k_snapshot_since(DrDeviceTable TB, int64_t min_version, int32_t* __restrict__ counts, int64_t* __restrict__ keys, float* __restrict__ rows,
+                                 int64_t* __restrict__ freqs, int64_t* __restrict__ versions) {
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < TB.capacity; p += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t key = TB.slots[p].key;
+    if (key == kEmptyKey || key == kTombKey) continue;
+    const int32_t r = TB.slots[p].row_of, v = TB.slots[p].version;
+    if (r < 0 || (int64_t)v < min_version) continue;
+    const int32_t o = atomicAdd(&counts[0], 1);
+    if (keys) {
+      keys[o] = key; freqs[o] = TB.slots[p].freq; versions[o] = v;
+      const float* src = TB.rows + (int64_t)r * TB.stride; float* dst = rows + (int64_t)o * TB.stride;
+      for (int d = 0; d < TB.stride; ++d) dst[d] = src[d];
+    }
+  }
+}
+
 // rows (full stride) + metadata of specific keys (multi-tier demotion / promotion); found[i] = key owns a row
 __global__ void k_export_keys(DrDeviceTable TB, const int64_t* __restrict__ keys, int64_t n, float* __restrict__ rows, int64_t* __restrict__ freqs,
                               int64_t* __restrict__ versions, uint8_t* __restrict__ found) {
@@ -405,6 +423,14 @@ int dr_cuda_table_snapshot(const DrDeviceTable* t_host, int dirty_only, int part
                            int64_t* fversions, cudaStream_t s) {
   k_snapshot<<<grid_for(t_host->capacity, 256), 256, 0, s>>>(*t_host, dirty_only, part_id, part_num, counts, keys, rows, freqs,
                                                             versions, fkeys, ffreqs, fversions);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// Pass null outputs to only count (counts[0]), then allocate and call again with counts zeroed -- as dr_cuda_table_snapshot.
+int dr_cuda_table_snapshot_since(const DrDeviceTable* t_host, int64_t min_version, int32_t* counts, int64_t* keys, float* rows, int64_t* freqs,
+                                 int64_t* versions, cudaStream_t s) {
+  k_snapshot_since<<<grid_for(t_host->capacity, 256), 256, 0, s>>>(*t_host, min_version, counts, keys, rows, freqs, versions);
   DR_LAUNCH_CHECK();
   return 0;
 }

@@ -179,7 +179,8 @@ static bool BuildProgram(dr::BundleReader& r, const Arch& a, std::shared_ptr<Den
   for (size_t i = 0; i < a.ops.size(); ++i) {
     OpTensors& t = p.ops[i]; PData& d = dp->pdata[i];
     switch (a.ops[i].kind) {
-      case P_LINEAR: d.L = Transposed(t.N, t.K, t.W.data(), (size_t)t.K, t.b); break;
+      case P_LINEAR:
+      case P_CROSS_LINEAR: d.L = Transposed(t.N, t.K, t.W.data(), (size_t)t.K, t.b); break;
       case P_GRU: d.Gih = Transposed(t.N, t.K, t.W.data(), (size_t)t.K, t.b); d.Ghh = Transposed(t.N, t.H1, t.v0.data(), (size_t)t.H1, t.v1); break;
       case P_DIN_ATT: {
         // first layer split (the algebra of csrc/cuda/attention_kernels.cu): W1 [q | k | q - k | q * k] = (Wa + Wc) q + (Wb - Wc) k + Wd (q * k);
@@ -499,6 +500,16 @@ struct Session {
           }
           break;
         }
+        case P_CROSS_LINEAR: {                                   // x0 * (t kernel^T + bias) + x_l: the product lands in `out` first
+          const float* xl = Buf(op.in[1]); const float* tt = Buf(op.in[2]);
+          Linear(tt, d.width[(size_t)op.in[2]], B, pd.L, out, false, threads);
+#pragma omp parallel for schedule(static) num_threads(threads) if (par)
+          for (int i = 0; i < B; ++i) {
+            const float* x0 = a0 + (size_t)i * W; const float* x = xl + (size_t)i * W; float* y = out + (size_t)i * W;
+            for (int k = 0; k < W; ++k) y[k] = x0[k] * y[k] + x[k];
+          }
+          break;
+        }
         case P_MUL_ADD: case P_ADD: case P_MUL: {
           const float* b1 = Buf(op.in[1]); const float* c1 = op.kind == P_MUL_ADD ? Buf(op.in[2]) : nullptr;
           const size_t n = (size_t)B * W;
@@ -543,14 +554,14 @@ struct Session {
           }
           break;
         }
-        case P_SEQ_MEAN: {                                       // mean over the valid positions
+        case P_SEQ_MEAN: {                                       // mean over the valid positions (mode 1: sum / sqrt(count))
           const float* mk = Buf(op.in[1]); const int L = op.len;
 #pragma omp parallel for schedule(static) num_threads(threads) if (par)
           for (int i = 0; i < B; ++i) {
             float* y = out + (size_t)i * W; for (int k = 0; k < W; ++k) y[k] = 0.f;
             int cnt = 0;
             for (int l = 0; l < L; ++l) if (mk[(size_t)i * L + l] > 0.f) { ++cnt; const float* x = a0 + (size_t)i * w0 + (size_t)l * W; for (int k = 0; k < W; ++k) y[k] += x[k]; }
-            const float inv = 1.f / (float)std::max(cnt, 1);
+            const float inv = op.mode == 1 ? 1.f / std::sqrt((float)std::max(cnt, 1)) : 1.f / (float)std::max(cnt, 1);
             for (int k = 0; k < W; ++k) y[k] *= inv;
           }
           break;

@@ -321,6 +321,15 @@ class DeviceTable:
         check(self.lib.dr_cuda_table_get_meta(C.byref(self.struct), ptr(k), k.numel(), None, ptr(out), None, stream_ptr()), "get_meta")
         return out.cpu()
 
+    def has_row(self, keys: torch.Tensor) -> torch.Tensor:
+        """bool [n]: the key owns a row in this table (metadata probe only, no row is copied)."""
+        k = self._keys(keys)
+        if k.numel() == 0:
+            return torch.zeros(0, dtype=torch.bool)
+        out = torch.empty(k.numel(), dtype=torch.int32, device=self.device)
+        check(self.lib.dr_cuda_table_get_meta(C.byref(self.struct), ptr(k), k.numel(), None, None, ptr(out), stream_ptr()), "get_meta")
+        return out.cpu() >= 0
+
     def lookup_slot(self, keys: torch.Tensor, slot: int) -> torch.Tensor:
         k = self._keys(keys)
         out = torch.empty(k.numel(), self.dim, dtype=torch.float32, device=self.device)
@@ -387,6 +396,20 @@ class DeviceTable:
         return dict(keys=keys[oa].cpu(), rows=rows[oa].cpu(), freqs=freqs[oa].cpu(), versions=vers[oa].cpu(), partition_offset=offa,
                     keys_filtered=fkeys[of].cpu(), freqs_filtered=ffreqs[of].cpu(), versions_filtered=fvers[of].cpu(),
                     partition_filter_offset=offf)
+
+    def snapshot_since(self, min_version: int) -> Dict[str, torch.Tensor]:
+        """Admitted keys whose version (global step of their last update) is >= ``min_version``, with their full-stride rows, frequencies
+        and versions (host tensors, in no particular order).  Dirty bits are neither read nor cleared."""
+        d, s = self.device, stream_ptr()
+        counts = torch.zeros(1, dtype=torch.int32, device=d)
+        check(self.lib.dr_cuda_table_snapshot_since(C.byref(self.struct), int(min_version), ptr(counts), None, None, None, None, s), "snapshot_since(count)")
+        n = int(counts.item())
+        keys = torch.empty(n, dtype=torch.int64, device=d); rows = torch.empty(n, self.stride, dtype=torch.float32, device=d)
+        freqs = torch.empty(n, dtype=torch.int64, device=d); vers = torch.empty(n, dtype=torch.int64, device=d)
+        counts.zero_()
+        check(self.lib.dr_cuda_table_snapshot_since(C.byref(self.struct), int(min_version), ptr(counts), ptr(keys), ptr(rows), ptr(freqs), ptr(vers), s),
+              "snapshot_since(fill)")
+        return dict(keys=keys.cpu(), rows=rows.cpu(), freqs=freqs.cpu(), versions=vers.cpu())
 
     def import_(self, keys, rows, freqs, versions, part_id=0, part_num=1, reset_version=False) -> int:
         k = self._keys(keys)

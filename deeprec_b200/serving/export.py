@@ -33,10 +33,11 @@ def _write_versions(root: str, full: Optional[dict] = None, delta: Optional[dict
 
 
 def _check_exportable(engine) -> None:
-    # the "dlrm" saved-model format and the Processors know the dot interaction only: a DLRM-DCNv2 export would be served without its
-    # cross layers, i.e. as a different model
+    # the "dlrm" saved-model format knows the dot interaction only: a DLRM-DCNv2 export would be served without its cross layers, i.e. as
+    # a different model.  The op-program format describes them.
     if getattr(engine.cfg, "interaction_op", "dot") != "dot":
-        raise ValueError(f"serving export of a DLRMEngine with interaction_op={engine.cfg.interaction_op!r} is not supported")
+        raise ValueError(f"export_saved_model / export_delta take a DLRMEngine with the dot interaction; interaction_op="
+                         f"{engine.cfg.interaction_op!r} exports with export_engine_program / export_engine_delta")
 
 
 def export_saved_model(engine, export_dir: str, version: Optional[int] = None, root: Optional[str] = None) -> str:
@@ -309,9 +310,16 @@ class _ProgramBuilder:
         """Multi-head self-attention core over ``qkv [B, S * 3E]`` (per position ``[q | k | v]``), keys with ``valid [B, S] == 0`` masked -> ``[B, S * E]``."""
         out = self._name("mha"); self.ops.append({"op": "mha", "out": out, "in": [qkv, valid], "len": int(S), "heads": int(heads)}); return out
 
-    def seq_mean(self, x, valid, S):
-        """Mean of ``x [B, S * W]`` over the valid positions -> ``[B, W]``."""
-        out = self._name("smean"); self.ops.append({"op": "seq_mean", "out": out, "in": [x, valid], "len": int(S)}); return out
+    def seq_mean(self, x, valid, S, sqrtn=False):
+        """Mean of ``x [B, S * W]`` over the valid positions -> ``[B, W]``; ``sqrtn``: the sum over them divided by sqrt(count) (0 when none)."""
+        out = self._name("smean"); self.ops.append({"op": "seq_mean", "out": out, "in": [x, valid], "len": int(S), **({"mode": 1} if sqrtn else {})}); return out
+
+    def cross_linear(self, x0, x, t, kernel, bias):
+        """Low-rank cross layer output ``x0 * (t kernel^T + bias) + x`` (``kernel [N, r]``, ``t [B, r]``, ``x0`` and ``x`` ``[B, N]``)."""
+        out = self._name("xlin")
+        self.tensors[f"prog/{out}/kernel"] = kernel.detach().float().cpu().contiguous()
+        self.tensors[f"prog/{out}/bias"] = bias.detach().float().cpu().contiguous()
+        self.ops.append({"op": "cross_linear", "out": out, "in": [x0, x, t]}); return out
 
     def din_attention(self, q, k, mask, att, weights=False):
         """Linear(4W, H1)-Sigmoid-Linear(H1, H2)-Sigmoid-Linear(H2, 1) attention unit, masked softmax, weighted sum of the keys
@@ -344,12 +352,20 @@ class _ProgramBuilder:
         """nn.Sequential of Linear / ReLU / BatchNorm1d (what ``models.zoo.mlp`` builds on CPU): a BatchNorm folds into the next Linear
         (W' = W diag(s), b' = b + W t); one left over at the end becomes an explicit affine op."""
         import torch.nn as nn
+        from ..nn import FusedMLP
         pending = None
 
         def flat(m):
             if isinstance(m, nn.Sequential):
                 for c in m:
                     yield from flat(c)
+            elif isinstance(m, FusedMLP):                   # the wgmma Linear(-ReLU) chain of models.zoo.mlp on CUDA (FusedLinear included)
+                for i, w in enumerate(m.weights):
+                    lin = nn.Linear(w.shape[1], w.shape[0], bias=False)
+                    lin.weight, lin.bias = w, (m.biases[i] if m.biases is not None else None)
+                    yield lin
+                    if i + 1 < len(m.weights) or m.last_act:
+                        yield nn.ReLU()
             else:
                 yield m
         mods = list(flat(seq))
@@ -384,9 +400,13 @@ class _ProgramBuilder:
         return src
 
 
-def _build_program(model, max_len: int = 50) -> _ProgramBuilder:
+def _build_program(model, max_len: int = 50, tables: Optional[list] = None, pool: Optional[tuple] = None) -> _ProgramBuilder:
+    """``tables``: the table sources in the program's table order (``_EvTable`` / ``_EngineTable``); None: the module's EmbeddingVariables.
+    ``pool``: the combiners (``sum | mean | sqrtn``) of the two history bags of a pooled Taobao model, each bag counting its own valid ids
+    (``FusedRecEngine(bags=...)``); None: the history summed over the positions valid in the item column (``_embed_pooled``)."""
     from ..models import zoo
     p = _ProgramBuilder()
+    p.tables = tables
     if isinstance(model, zoo.DeepFM):
         x0 = p.concat(["dense", "emb"])
         dnn = p.sequential(x0, model.dnn)
@@ -400,7 +420,8 @@ def _build_program(model, max_len: int = 50) -> _ProgramBuilder:
         sel = torch.zeros(1, T * D); sel[0, ::D] = 1.0                     # sum over tables of component 0 of the wide embedding
         wide = p.add(p.linear(p.slice("emb", T * D, T * D), sel, None), p.linear("dense", model.wide_dense.weight, model.wide_dense.bias))
         p.out = p.add(wide, deep)
-        p.tables = [(ev, ev.embedding_dim) for ev in _evs_of(model.emb)] + [(ev, ev.embedding_dim) for ev in _evs_of(model.wide)]
+        if p.tables is None:
+            p.tables = [_EvTable(ev) for ev in _evs_of(model.emb)] + [_EvTable(ev) for ev in _evs_of(model.wide)]
         p.id_map = list(range(T)) + list(range(T))
     elif isinstance(model, zoo.MaskNet):                                 # serial MaskBlocks: h = ReLU(LN(W (h * mask(v))))
         h = p.layernorm("emb", model.ln_emb)
@@ -422,12 +443,23 @@ def _build_program(model, max_len: int = 50) -> _ProgramBuilder:
     elif isinstance(model, (zoo._MultiTask, zoo.DSSM)):
         # Taobao-shaped models on the pooled behaviour history: lookup columns as for DIN, features = [user | target | sum of the valid history]
         L, D = int(max_len), model.emb_dim
-        p.tables = [(model.user, D), (model.item, D), (model.cat, D)]
+        if p.tables is None:
+            p.tables = [_EvTable(model.user), _EvTable(model.item), _EvTable(model.cat)]
         p.col_table = [0, 1, 2] + [1] * L + [2] * L
         p.num_dense = 1
         u, q = p.slice("emb", 0, D), p.slice("emb", D, 2 * D)
-        mask = p.valid_mask(3, L)
-        pooled = p.seq_sum(p.seq_mask(p.seq_zip(p.slice("emb", 3 * D, L * D), p.slice("emb", (3 + L) * D, L * D), L), mask, L), L)      # [B, 2D]
+        if pool is None:
+            mask = p.valid_mask(3, L)
+            pooled = p.seq_sum(p.seq_mask(p.seq_zip(p.slice("emb", 3 * D, L * D), p.slice("emb", (3 + L) * D, L * D), L), mask, L), L)      # [B, 2D]
+        else:
+            def bag(col, comb):                                           # columns col .. col + L - 1, their own padding mask
+                x, m = p.slice("emb", col * D, L * D), p.valid_mask(col, L)
+                if comb == "sum":
+                    return p.seq_sum(p.seq_mask(x, m, L), L)
+                if comb not in ("mean", "sqrtn"):
+                    raise ValueError(f"op-program export: unknown combiner {comb!r}")
+                return p.seq_mean(x, m, L, sqrtn=comb == "sqrtn")
+            pooled = p.concat([bag(3, pool[0]), bag(3 + L, pool[1])])
         if isinstance(model, zoo.DSSM):
             ue, ie = p.sequential(p.concat([u, pooled]), model.user_tower), p.sequential(q, model.item_tower)
             p.out = p.affine(p.cosine(ue, ie), model.scale.detach().reshape(1), torch.zeros(1))
@@ -440,8 +472,7 @@ def _build_program(model, max_len: int = 50) -> _ProgramBuilder:
                 outs = [p.sequential(f, model.towers[t]) for t in tasks]
             elif isinstance(model, zoo.MMoE):
                 ex = [p.sequential(f, e) for e in model.experts]
-                w = model.experts[0][-2].out_features if isinstance(model.experts[0][-1], torch.nn.ReLU) else model.experts[0][-1].out_features
-                outs = [p.sequential(p.mixture(p.softmax(p.linear(f, model.gates[t].weight, model.gates[t].bias)), ex, w), model.towers[t]) for t in tasks]
+                outs = [p.sequential(p.mixture(p.softmax(p.linear(f, model.gates[t].weight, model.gates[t].bias)), ex, 0), model.towers[t]) for t in tasks]
             elif isinstance(model, zoo.DBMTL):
                 sh = p.sequential(f, model.bottom)
                 a_, c_ = p.sequential(sh, model.t_ctr), p.sequential(sh, model.t_cvr)
@@ -466,7 +497,8 @@ def _build_program(model, max_len: int = 50) -> _ProgramBuilder:
         # padding ids (-1) give masked (zeroed) history positions
         import torch.nn as nn
         L, D = int(max_len), model.emb_dim
-        p.tables = [(model.user, D), (model.item, D), (model.cat, D)]
+        if p.tables is None:
+            p.tables = [_EvTable(model.user), _EvTable(model.item), _EvTable(model.cat)]
         p.col_table = [0, 1, 2] + [1] * L + [2] * L
         p.num_dense = 1                                                   # a dummy dense column keeps the request format uniform
         u, q = p.slice("emb", 0, D), p.slice("emb", D, 2 * D)
@@ -477,7 +509,8 @@ def _build_program(model, max_len: int = 50) -> _ProgramBuilder:
     elif isinstance(model, (zoo.DIEN, zoo.BST)):
         L, D = int(max_len), model.emb_dim
         E = 2 * D
-        p.tables = [(model.user, D), (model.item, D), (model.cat, D)]
+        if p.tables is None:
+            p.tables = [_EvTable(model.user), _EvTable(model.item), _EvTable(model.cat)]
         p.col_table = [0, 1, 2] + [1] * L + [2] * L
         p.num_dense = 1
         u, q = p.slice("emb", 0, D), p.slice("emb", D, 2 * D)
@@ -507,14 +540,20 @@ def _build_program(model, max_len: int = 50) -> _ProgramBuilder:
             f_ = p.seq_linear(p.seq_linear(x1, enc.linear1.weight, enc.linear1.bias, S, relu=True), enc.linear2.weight, enc.linear2.bias, S)
             x2 = p.seq_layernorm(p.add(x1, f_), enc.norm2, S)
             p.out = p.linear(p.sequential(p.concat([u, q, p.seq_mean(x2, valid, S)]), model.final), model.out.weight, model.out.bias)
+    elif isinstance(model, zoo.DLRMDCN):                                 # x0 = [bottom | emb], x_{l+1} = x0 * ((x_l U) V + b) + x_l
+        x0 = p.concat([p.sequential("dense", model.bot), "emb"])
+        x = x0
+        for U, V, b in zip(model.U, model.V, model.cb):
+            x = p.cross_linear(x0, x, p.linear(x, U.detach().t(), None), V.detach().t(), b)
+        p.out = p.linear(p.sequential(x, model.top), model.out.weight, model.out.bias)
     else:
-        raise TypeError(f"op-program export: no builder for {type(model).__name__} (WDL, DeepFM, DCN, DCNv2, MaskNet, DIN, DIEN, BST, DSSM, ESMM, MMoE, DBMTL, PLE, SimpleMultiTask; DLRM has export_saved_model_module)")
+        raise TypeError(f"op-program export: no builder for {type(model).__name__} (WDL, DeepFM, DCN, DCNv2, MaskNet, DLRMDCN, DIN, DIEN, BST, DSSM, ESMM, MMoE, DBMTL, PLE, SimpleMultiTask; DLRM has export_saved_model_module)")
     return p
 
 
 # ---- sample-aware graph compression as a pass over the op program ---------------------------------------------------------------------------
 _ROW_WISE = {"concat", "linear", "affine", "cross", "mul_add", "add", "mul", "layernorm", "slice", "seq_zip", "seq_mask", "seq_sum", "prelu", "softmax",
-             "cosine", "din_attention", "valid_mask", "gru", "seq_last", "mha", "seq_mean"}
+             "cosine", "din_attention", "valid_mask", "gru", "seq_last", "mha", "seq_mean", "cross_linear"}
 
 
 def compress_sample_aware(ops: list, output: str, user_columns, emb_dim: int, user_dense: bool = False):
@@ -579,10 +618,64 @@ def _evs_of(module):
     return collect_embedding_variables(module)
 
 
+class _EvTable:
+    """An EmbeddingVariable as a table of a program export.  Every export (full or delta) restarts its dirty bits."""
+
+    def __init__(self, ev):
+        self.ev, self.dim = ev, ev.embedding_dim
+
+    def default(self) -> torch.Tensor:
+        return self.ev.default_matrix.detach().float().cpu()
+
+    def full(self) -> dict:
+        s = self.ev.table.snapshot()
+        return {k: s[k].cpu() for k in ("keys", "rows", "freqs", "versions")}
+
+    def delta(self, since) -> dict:
+        return {k: v.cpu() for k, v in self.ev.table.snapshot(dirty_only=True).items() if k in ("keys", "rows")}
+
+    def exported(self) -> None:
+        self.ev.table.clear_dirty()
+
+
+class _EngineTable:
+    """A fused engine's device table (with its DRAM tier when tiered) as a table of a program export.  Keys the admission filter holds
+    back have no row and are not exported.  Deltas select rows by version (the global step of their last update), so the dirty bits stay
+    with the engine's incremental checkpoints."""
+
+    def __init__(self, table, tier=None):
+        self.table, self.mgr, self.dim = table, tier, table.dim
+
+    def default(self) -> torch.Tensor:
+        return self.table.default_matrix.detach().float().cpu()
+
+    def _with_dram(self, s: dict, since: Optional[int]) -> dict:
+        if self.mgr is None:
+            return s
+        self.mgr.drain()                                  # in-flight promotions / demotions land first
+        h = self.mgr.host.snapshot()                      # host memory: the DRAM tier has no version-selected snapshot
+        if since is None:
+            keep = ~torch.isin(h["keys"], s["keys"])      # the HBM copy of a key is the live one
+        else:                                             # delta: only the DRAM rows updated since, minus those resident in HBM
+            keep = h["versions"] >= since
+            keep[keep.clone()] = ~self.table.has_row(h["keys"][keep])
+        return {k: torch.cat([s[k], h[k][keep]]) for k in ("keys", "rows", "freqs", "versions")}
+
+    def full(self) -> dict:
+        s = self.table.snapshot()
+        return self._with_dram({k: s[k] for k in ("keys", "rows", "freqs", "versions")}, None)
+
+    def delta(self, since: int) -> dict:
+        return self._with_dram(self.table.snapshot_since(since), since)
+
+    def exported(self) -> None:
+        pass
+
+
 def _program_tables(model, p):
-    """[(EmbeddingVariable, its dim)] in table order, the common row width D (narrower tables are stored zero-padded), id_map or None."""
-    tables = getattr(p, "tables", None) or [(ev, ev.embedding_dim) for ev in _evs_of(model.emb)]
-    return tables, max(d for _, d in tables), getattr(p, "id_map", None)
+    """[table source] in table order, the common row width D (narrower tables are stored zero-padded), id_map or None."""
+    tables = p.tables if p.tables is not None else [_EvTable(ev) for ev in _evs_of(model.emb)]
+    return tables, max(t.dim for t in tables), getattr(p, "id_map", None)
 
 
 def _padded(rows: torch.Tensor, d: int, D: int) -> torch.Tensor:
@@ -593,34 +686,25 @@ def _padded(rows: torch.Tensor, d: int, D: int) -> torch.Tensor:
     return out
 
 
-def export_saved_model_program(model, export_dir: str, version: int, root: Optional[str] = None, max_len: int = 50,
-                               sample_aware: Optional[dict] = None) -> str:
-    """Full export of a zoo model (Criteo-style ``WDL``, ``DeepFM``, ``DCN``, ``DCNv2``, ``MaskNet``; sequence model ``DIN`` with ``max_len`` history
-    positions -- request ids = the ``[3 + 2 L, B]`` block of ``models.rec_engine.din_ids`` and one dummy dense column) as an op program + EmbeddingVariable tables; loaded by
-    ``Processor(dir, cfg)`` (GPU runtime: wgmma GEMMs + csrc/cuda/program_kernels.cu; ``device="cpu"``: the host interpreter) exactly like a DLRM
-    export (same ModelConfig, update protocol, request formats)."""
-    was_training = model.training
-    model.eval()
-    p = _build_program(model, max_len)
-    tables, D, id_map = _program_tables(model, p)
+def _write_program(p, tables, D, id_map, name: str, num_dense: int, export_dir: str, version: int, root: Optional[str],
+                   sample_aware: Optional[dict], extra: Optional[dict] = None) -> str:
     col_table = getattr(p, "col_table", None)
-    num_dense = getattr(p, "num_dense", None) or model.num_dense
     n_compressed = 0
     if sample_aware:                               # {"user_columns": [...], "user_dense": bool}: user-side sub-graph once per request
         p.ops, p.out, n_compressed = compress_sample_aware(p.ops, p.out, sample_aware["user_columns"], D, bool(sample_aware.get("user_dense", False)))
     os.makedirs(os.path.join(export_dir, "variables"), exist_ok=True)
     w = BundleWriter(os.path.join(export_dir, "variables", "variables"))
-    for name, t in p.tensors.items():
-        w.add(name, t)
-    for t, (ev, d) in enumerate(tables):
-        s = ev.table.snapshot()
-        w.add(f"table/{t}-keys", s["keys"].cpu()); w.add(f"table/{t}-values", _padded(s["rows"], d, D))
-        w.add(f"table/{t}-freqs", s["freqs"].cpu()); w.add(f"table/{t}-versions", s["versions"].cpu())
-        w.add(f"table/{t}-default", _padded(ev.default_matrix.detach(), d, D))
-        ev.table.clear_dirty()
+    for nm, t in p.tensors.items():
+        w.add(nm, t)
+    for t, src in enumerate(tables):
+        s = src.full()
+        w.add(f"table/{t}-keys", s["keys"]); w.add(f"table/{t}-values", _padded(s["rows"], src.dim, D))
+        w.add(f"table/{t}-freqs", s["freqs"]); w.add(f"table/{t}-versions", s["versions"])
+        w.add(f"table/{t}-default", _padded(src.default(), src.dim, D))
+        src.exported()
     w.close()
     rows = (len(col_table) if col_table is not None else len(tables)) if id_map is None else max(id_map) + 1
-    meta = {"model": type(model).__name__.lower(), "arch": "program", "version": int(version), "num_dense": num_dense, "num_tables": len(tables),
+    meta = {"model": name, "arch": "program", "version": int(version), "num_dense": num_dense, "num_tables": len(tables),
             "num_id_rows": rows, "embedding_dim": D, "program": p.ops, "output": p.out, "variables": "variables/variables",
             "signature": {"inputs": {"dense": ["B", num_dense], "ids": [rows, "B"]}, "outputs": {"probabilities": ["B"]}}}
     if id_map is not None:
@@ -633,9 +717,41 @@ def export_saved_model_program(model, export_dir: str, version: int, root: Optio
     if getattr(p, "num_outputs", 1) > 1:                                 # multi-task: probabilities [B, num_outputs], one column per task
         meta["num_outputs"], meta["output_names"] = p.num_outputs, list(p.output_names)
         meta["signature"]["outputs"] = {"probabilities": ["B", p.num_outputs]}
+    meta.update(extra or {})
     with open(os.path.join(export_dir, "saved_model.json"), "w") as f:
         json.dump(meta, f)
     _write_versions(root or export_dir, full={"version": int(version), "dir": os.path.abspath(export_dir)})
+    return export_dir
+
+
+def _write_program_delta(p, tables, D, root: str, base_version: int, version: int, since: Optional[int] = None) -> str:
+    d = os.path.join(root, ".incr")
+    os.makedirs(d, exist_ok=True)
+    prefix = os.path.join(d, f"delta-{int(version)}")
+    w = BundleWriter(prefix)
+    for nm, t in p.tensors.items():
+        w.add(nm, t)
+    for t, src in enumerate(tables):
+        s = src.delta(since)
+        w.add(f"table/{t}-sparse_incr_keys", s["keys"]); w.add(f"table/{t}-sparse_incr_values", _padded(s["rows"], src.dim, D))
+        src.exported()
+    w.close()
+    _write_versions(root, delta={"version": int(version), "base": int(base_version), "prefix": os.path.abspath(prefix)})
+    return prefix
+
+
+def export_saved_model_program(model, export_dir: str, version: int, root: Optional[str] = None, max_len: int = 50,
+                               sample_aware: Optional[dict] = None) -> str:
+    """Full export of a zoo model (Criteo-style ``WDL``, ``DeepFM``, ``DCN``, ``DCNv2``, ``MaskNet``, ``DLRMDCN``; sequence model ``DIN`` with ``max_len`` history
+    positions -- request ids = the ``[3 + 2 L, B]`` block of ``models.rec_engine.din_ids`` and one dummy dense column) as an op program + EmbeddingVariable tables; loaded by
+    ``Processor(dir, cfg)`` (GPU runtime: wgmma GEMMs + csrc/cuda/program_kernels.cu; ``device="cpu"``: the host interpreter) exactly like a DLRM
+    export (same ModelConfig, update protocol, request formats)."""
+    was_training = model.training
+    model.eval()
+    p = _build_program(model, max_len)
+    tables, D, id_map = _program_tables(model, p)
+    num_dense = getattr(p, "num_dense", None) or model.num_dense
+    _write_program(p, tables, D, id_map, type(model).__name__.lower(), num_dense, export_dir, version, root, sample_aware)
     model.train(was_training)
     return export_dir
 
@@ -645,18 +761,113 @@ def export_delta_program(model, root: str, base_version: int, version: int, max_
     was_training = model.training
     model.eval()
     p = _build_program(model, max_len)
-    d = os.path.join(root, ".incr")
-    os.makedirs(d, exist_ok=True)
-    prefix = os.path.join(d, f"delta-{int(version)}")
-    w = BundleWriter(prefix)
-    for name, t in p.tensors.items():
-        w.add(name, t)
     tables, D, _ = _program_tables(model, p)
-    for t, (ev, dd) in enumerate(tables):
-        s = ev.table.snapshot(dirty_only=True)
-        w.add(f"table/{t}-sparse_incr_keys", s["keys"].cpu()); w.add(f"table/{t}-sparse_incr_values", _padded(s["rows"], dd, D))
-        ev.table.clear_dirty()
-    w.close()
-    _write_versions(root, delta={"version": int(version), "base": int(base_version), "prefix": os.path.abspath(prefix)})
+    prefix = _write_program_delta(p, tables, D, root, base_version, version)
     model.train(was_training)
     return prefix
+
+
+# ------------------------------------------------------------------------------------------------------------------------------------
+# Engine exports: a model trained on FusedRecEngine or DLRMEngine(interaction_op="dcnv2") -> the op-program format of the native
+# Processors.  The tables come from the engine (both tiers of a tiered table), the dense weights from its flat parameter buffer.
+# ------------------------------------------------------------------------------------------------------------------------------------
+def _check_engine(engine) -> None:
+    """The refusals of the engine exports, before any work."""
+    from ..models.dlrm_engine import DLRMEngine
+    from ..models.rec_engine import FusedRecEngine
+    if not isinstance(engine, (FusedRecEngine, DLRMEngine)):
+        raise TypeError(f"engine export: expected a FusedRecEngine or a DLRMEngine, got {type(engine).__name__}")
+    if engine.world > 1:
+        raise ValueError(f"engine export at world_size {engine.world}: restore the engine checkpoint into a world_size 1 engine "
+                         "(restore_engine re-shards it) and export from that")
+    if isinstance(engine, DLRMEngine) and getattr(engine.cfg, "interaction_op", "dot") != "dcnv2":
+        raise ValueError("a DLRMEngine with the dot interaction exports with export_saved_model / export_delta")
+    bags = engine.deep.bags if isinstance(engine, FusedRecEngine) else None
+    if bags is not None:                                                 # pooled_seq_engine: [user | item | cat | hist_item x L | hist_cat x L]
+        L = (engine.C - 3) // 2
+        if [n for n, _ in bags.spec] != [1, 1, 1, L, L] or engine.C != 3 + 2 * L:
+            raise ValueError(f"engine export: bags {bags.spec} over {engine.C} id columns are not the pooled Taobao layout of pooled_seq_engine")
+
+
+def _engine_program(engine):
+    """(program, table sources, model name, num_dense) of an engine that passed :func:`_check_engine`."""
+    import copy
+    from ..models.rec_engine import FusedRecEngine
+    if isinstance(engine, FusedRecEngine):                               # the zoo module around the engine's weights
+        model = copy.deepcopy(engine.net.inner).float().cpu().eval()
+        tables = [_EngineTable(engine.tables[t], engine.tiers[t][0] if t in engine.tiers else None) for t in range(engine.T)]
+        if engine.linear:                                                # WDL: the linear group's dim-4 tables are tables T .. 2T-1
+            tables += [_EngineTable(engine.lin_tables[t]) for t in range(engine.T)]
+        bags = engine.deep.bags
+        pool = (bags.spec[3][1], bags.spec[4][1]) if bags is not None else None
+        p = _build_program(model, (engine.C - 3) // 2, tables=tables, pool=pool)
+        return p, tables, type(model).__name__.lower(), getattr(p, "num_dense", None) or model.num_dense
+    return _dlrm_dcn_program(engine), [_EngineTable(engine.tables[t]) for t in range(engine.T)], "dlrm_dcnv2", engine.cfg.num_dense
+
+
+def _dlrm_dcn_program(engine) -> _ProgramBuilder:
+    """DLRMEngine(dcnv2): bottom Linear-ReLU-BatchNorm layers (folded into the next Linear, the last one an affine op), x0 = [bottom | emb],
+    per cross layer t = x_l V_l^T (a zero-bias linear) and x_{l+1} = cross_linear(x0, x_l, t) with W_l, b_l, then the top MLP and the logits."""
+    import torch.nn as nn
+    cfg = engine.cfg
+    w = lambda L: engine.p(L.name + "/kernel").view(L.N, L.Kp)[:, : L.K].float().cpu()
+    b = lambda L: engine.p(L.name + "/bias").float().cpu()
+    bot = []
+    for L in engine.bot:
+        lin, bn = nn.Linear(L.K, L.N), nn.BatchNorm1d(L.N, eps=cfg.bn_eps)
+        with torch.no_grad():
+            lin.weight.copy_(w(L)); lin.bias.copy_(b(L))
+            bn.weight.copy_(engine.p(L.name + "/bn_gamma").cpu()); bn.bias.copy_(engine.p(L.name + "/bn_beta").cpu())
+            bn.running_mean.copy_(L.running_mean.cpu()); bn.running_var.copy_(L.running_var.cpu())
+        bot += [lin, nn.ReLU(), bn]
+    p = _ProgramBuilder()
+    x0 = p.concat([p.sequential("dense", nn.Sequential(*bot).eval()), "emb"])
+    x = x0
+    for V, W in engine.cross:
+        x = p.cross_linear(x0, x, p.linear(x, w(V), None), w(W), b(W))
+    for L in engine.top:
+        x = p.linear(x, w(L), b(L), relu=True)
+    p.out = p.linear(x, engine.p("logits/kernel").float().cpu().view(1, -1), engine.p("logits/bias")[:1].float().cpu())
+    return p
+
+
+def _engine_step(engine) -> int:
+    from ..checkpoint.engine_ckpt import _step_of
+    from .. import _native
+    _native.device_sync(engine.dev)
+    return _step_of(engine)
+
+
+def export_engine_program(engine, export_dir: str, version: Optional[int] = None, root: Optional[str] = None,
+                          sample_aware: Optional[dict] = None) -> str:
+    """Full export of a world-size-1 :class:`models.rec_engine.FusedRecEngine` (any model its zoo adapters accept) or
+    ``DLRMEngine(interaction_op="dcnv2")`` in the ``"arch": "program"`` saved-model format: ``Processor(dir, cfg)`` serves it on the GPU, the
+    emulation and ``device="cpu"``.  ``version`` defaults to the engine's global step.  Request ids are the engine's id columns (Taobao models:
+    :func:`models.rec_engine.din_ids` and one dummy dense column).  Admitted rows of both tiers are exported (embedding only, no optimizer
+    slots); keys the admission filter holds back read the default rows, as unseen keys do."""
+    _check_engine(engine)
+    p, tables, name, num_dense = _engine_program(engine)
+    step = _engine_step(engine)
+    version = step if version is None else int(version)
+    D = max(t.dim for t in tables)
+    return _write_program(p, tables, D, getattr(p, "id_map", None), name, num_dense, export_dir, version, root, sample_aware, extra={"global_step": step})
+
+
+def export_engine_delta(engine, root: str, base_version: int, version: Optional[int] = None) -> str:
+    """Incremental export on top of the full export ``base_version`` of :func:`export_engine_program` under ``root``: every row updated since
+    that export (its version is at least the global step the export recorded) and the whole dense block.  Dirty bits are not touched, so
+    the engine's incremental checkpoints stay complete.  Keys evicted since the base export (``steps_to_live``) stay served until the next
+    full export."""
+    _check_engine(engine)
+    with open(os.path.join(root, "serving_versions.json")) as f:
+        full = json.load(f).get("full") or {}
+    if full.get("version") != int(base_version):
+        raise ValueError(f"export_engine_delta: the full export under {root} is version {full.get('version')}, not {base_version}")
+    with open(os.path.join(full["dir"], "saved_model.json")) as f:
+        since = json.load(f).get("global_step")
+    if since is None:
+        raise ValueError(f"export_engine_delta: {full['dir']} was not written by export_engine_program")
+    p, tables, _, _ = _engine_program(engine)
+    step = _engine_step(engine)
+    version = step if version is None else int(version)
+    return _write_program_delta(p, tables, max(t.dim for t in tables), root, base_version, version, since=int(since))
