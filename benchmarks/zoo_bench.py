@@ -122,7 +122,7 @@ def engine_main(a):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="deepfm")
+    ap.add_argument("--model", default="deepfm", help="a zoo model (models/zoo.py), e.g. deepfm, dcn, masknet_parallel, masknet_serial, din")
     ap.add_argument("--batch", type=int, default=8192)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)

@@ -91,6 +91,7 @@ _sig("dr_cuda_segment_sum", [P, P, i64, INT, P, S])
 _sig("dr_cuda_gemm_tn", [P, i64, P, i64, INT, INT, INT, P, INT, P, i64, P, i64, P, INT, S])
 _sig("dr_cuda_gemm_tn_ex", [P, i64, P, i64, INT, INT, INT, P, INT, P, i64, INT, P, i64, P, P, P, INT, INT, S])
 _sig("dr_cuda_gemm_tn_cross", [P, i64, P, i64, INT, INT, INT, P, INT, P, i64, P, i64, P, i64, P, i64, INT, S])
+_sig("dr_cuda_gemm_tn_ln", [P, i64, P, i64, INT, INT, INT, P, P, P, f32, INT, P, i64, P, i64, P, INT, S])
 _sig("dr_cuda_gemm_fp8_tn", [P, i64, P, i64, INT, INT, INT, P, P, INT, P, i64, INT, f32, S])
 _sig("dr_cuda_quantize_e4m3", [P, INT, i64, INT, i64, P, INT, f32, S])
 _sig("dr_cuda_quantize_weights_e4m3", [P, INT, INT, i64, P, INT, P, S])
@@ -111,6 +112,9 @@ _sig("dr_cuda_det_colsum", [P, INT, i64, INT, P, P, S])
 _sig("dr_cuda_pack_weights", [P, INT, INT, P, P, INT, S])
 _sig("dr_cuda_cross_bwd", [P, i64, P, i64, P, i64, i64, INT, P, i64, P, i64, INT, P, S])
 _sig("dr_cuda_cross_split", [P, i64, P, i64, i64, INT, INT, P, i64, P, S])
+_sig("dr_cuda_ln_relu_bwd", [P, i64, P, i64, P, i64, P, P, i64, INT, P, i64, P, P, S])
+_sig("dr_cuda_bn_apply_mul", [P, i64, P, P, P, i64, i64, INT, P, i64, S])
+_sig("dr_cuda_bn_mul_bwd", [P, i64, P, i64, P, i64, P, P, i64, INT, P, i64, P, i64, P, P, S])
 _sig("dr_cuda_cast_pad", [P, i64, INT, P, INT, S])
 _sig("dr_cuda_l2_flush", [P, i64, f32, S])
 # interactions, GRU, self-attention, DIN attention, fused element-wise ops

@@ -477,6 +477,146 @@ __global__ void __launch_bounds__(256) k_cross_split(const float* __restrict__ d
   }
 }
 
+// -------------------------------------------------------------------------------------------------
+// MaskNet MaskBlock (nn.FusedMaskBlock): backward of y = relu(gamma * x^ + beta), x^ = LayerNorm(h) from the LayerNorm GEMM epilogue.
+//   d = g * [y > 0],  dg = d * gamma,  dh = rstd * (dg - mean_row(dg) - x^ * mean_row(dg * x^))   (bf16)
+//   part[blockIdx.x] = this block's column sums  [ sum d * x^ | sum d ]  (dgamma | dbeta), added in order by k_det_colsum.
+// One warp per row, lane l owns the column pairs 2 l and 64 + 2 l (N <= 128); the warps' partials are added in warp order.
+// -------------------------------------------------------------------------------------------------
+constexpr int kLnBwdThreads = 256;
+__global__ void __launch_bounds__(kLnBwdThreads) k_ln_relu_bwd(const __nv_bfloat16* __restrict__ g, int64_t ldg, const __nv_bfloat16* __restrict__ y,
+                                                               int64_t ldy, const __nv_bfloat16* __restrict__ xh, int64_t ldx,
+                                                               const float* __restrict__ rstd, const float* __restrict__ gamma, int64_t M, int N,
+                                                               __nv_bfloat16* __restrict__ dh, int64_t ldh, float* __restrict__ part) {
+  pdl_sync();
+  constexpr int kWarps = kLnBwdThreads / 32;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const float inv_n = 1.f / (float)N;
+  float ga[2][2], pg[2][2], pb[2][2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int c = 64 * i + 2 * lane;
+#pragma unroll
+    for (int e = 0; e < 2; ++e) { ga[i][e] = c < N ? gamma[c + e] : 0.f; pg[i][e] = 0.f; pb[i][e] = 0.f; }
+  }
+  for (int64_t r = (int64_t)blockIdx.x * kWarps + warp; r < M; r += (int64_t)gridDim.x * kWarps) {
+    float dg[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, xv[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int c = 64 * i + 2 * lane;
+      if (c < N) {
+        const float2 fg = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(g + r * ldg + c));
+        const float2 fy = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(y + r * ldy + c));
+        const float2 fx = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(xh + r * ldx + c));
+        const float d[2] = {fy.x > 0.f ? fg.x : 0.f, fy.y > 0.f ? fg.y : 0.f};
+        xv[i][0] = fx.x; xv[i][1] = fx.y;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          dg[i][e] = d[e] * ga[i][e];
+          s1 += dg[i][e]; s2 += dg[i][e] * xv[i][e];
+          pg[i][e] += d[e] * xv[i][e]; pb[i][e] += d[e];
+        }
+      }
+    }
+    s1 = warp_sum(s1); s2 = warp_sum(s2);
+    const float rs = rstd[r], m1 = s1 * inv_n, m2 = s2 * inv_n;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int c = 64 * i + 2 * lane;
+      if (c < N)
+        *reinterpret_cast<uint32_t*>(dh + r * ldh + c) =
+            pack_bf16x2(rs * (dg[i][0] - m1 - xv[i][0] * m2), rs * (dg[i][1] - m1 - xv[i][1] * m2));
+    }
+  }
+  __shared__ float sh[kWarps * 2 * 128];          // [warp][dgamma N | dbeta N]
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int c = 64 * i + 2 * lane;
+    if (c < N) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) { sh[warp * 2 * N + c + e] = pg[i][e]; sh[warp * 2 * N + N + c + e] = pb[i][e]; }
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < 2 * N; k += blockDim.x) {
+    float sum = 0.f;
+    for (int w = 0; w < kWarps; ++w) sum += sh[w * 2 * N + k];
+    part[(int64_t)blockIdx.x * 2 * N + k] = sum;
+  }
+}
+
+// The mask's last BatchNorm apply fused with the instance-guided product:  p = (a * scale + shift) * v   (bf16, 8 columns per thread)
+__global__ void __launch_bounds__(256) k_bn_apply_mul(const __nv_bfloat16* __restrict__ a, int64_t lda, const float* __restrict__ scale,
+                                                      const float* __restrict__ shift, const __nv_bfloat16* __restrict__ v, int64_t ldv, int64_t B,
+                                                      int N, __nv_bfloat16* __restrict__ p, int64_t ldp) {
+  pdl_sync();
+  const int tpr = N / 8;
+  const int64_t total = B * tpr;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / tpr; const int c = (int)(i % tpr) * 8;
+    const int4 ra = ld_nc_v4(a + b * lda + c), rv = ld_nc_v4(v + b * ldv + c);
+    const uint32_t wa[4] = {(uint32_t)ra.x, (uint32_t)ra.y, (uint32_t)ra.z, (uint32_t)ra.w};
+    const uint32_t wv[4] = {(uint32_t)rv.x, (uint32_t)rv.y, (uint32_t)rv.z, (uint32_t)rv.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 fa = unpack_bf16x2(wa[e]), fv = unpack_bf16x2(wv[e]);
+      o[e] = pack_bf16x2(fmaf(fa.x, scale[c + 2 * e], shift[c + 2 * e]) * fv.x, fmaf(fa.y, scale[c + 2 * e + 1], shift[c + 2 * e + 1]) * fv.y);
+    }
+    *reinterpret_cast<int4*>(p + b * ldp + c) = make_int4((int)o[0], (int)o[1], (int)o[2], (int)o[3]);
+  }
+}
+
+// Backward of k_bn_apply_mul from dp:  dv = dp * (a * scale + shift),  dm = dp * v  (bf16), and part[blockIdx.x] = this block's column sums
+// [ sum dm | sum dm * a ] of the bf16-rounded dm, the sums the BatchNorm backward (k_bn_bwd_finalize) takes.  Layout of k_colstats: a thread
+// owns 8 columns, rows_par rows run side by side and their partials are added in row-group order.
+__global__ void __launch_bounds__(256) k_bn_mul_bwd(const __nv_bfloat16* __restrict__ dp, int64_t ldp, const __nv_bfloat16* __restrict__ a, int64_t lda,
+                                                    const __nv_bfloat16* __restrict__ v, int64_t ldv, const float* __restrict__ scale,
+                                                    const float* __restrict__ shift, int64_t B, int N, __nv_bfloat16* __restrict__ dv, int64_t lddv,
+                                                    __nv_bfloat16* __restrict__ dm, int64_t lddm, float* __restrict__ part) {
+  pdl_sync();
+  const int tpr = N / 8;
+  const int rows_par = blockDim.x / tpr;
+  const int tr = threadIdx.x / tpr, tc = threadIdx.x % tpr, c = tc * 8;
+  float a1[8], a2[8], sc[8], sf[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) { a1[j] = a2[j] = 0.f; sc[j] = sf[j] = 0.f; }
+  if (tr < rows_par) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { sc[j] = scale[c + j]; sf[j] = shift[c + j]; }
+    for (int64_t b = (int64_t)blockIdx.x * rows_par + tr; b < B; b += (int64_t)gridDim.x * rows_par) {
+      const int4 rp = ld_nc_v4(dp + b * ldp + c), ra = ld_nc_v4(a + b * lda + c), rv = ld_nc_v4(v + b * ldv + c);
+      const uint32_t wp[4] = {(uint32_t)rp.x, (uint32_t)rp.y, (uint32_t)rp.z, (uint32_t)rp.w};
+      const uint32_t wa[4] = {(uint32_t)ra.x, (uint32_t)ra.y, (uint32_t)ra.z, (uint32_t)ra.w};
+      const uint32_t wv[4] = {(uint32_t)rv.x, (uint32_t)rv.y, (uint32_t)rv.z, (uint32_t)rv.w};
+      uint32_t ov[4], om[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 fp = unpack_bf16x2(wp[e]), fa = unpack_bf16x2(wa[e]), fv = unpack_bf16x2(wv[e]);
+        ov[e] = pack_bf16x2(fp.x * fmaf(fa.x, sc[2 * e], sf[2 * e]), fp.y * fmaf(fa.y, sc[2 * e + 1], sf[2 * e + 1]));
+        om[e] = pack_bf16x2(fp.x * fv.x, fp.y * fv.y);
+        const float2 fm = unpack_bf16x2(om[e]);
+        a1[2 * e] += fm.x; a1[2 * e + 1] += fm.y;
+        a2[2 * e] += fm.x * fa.x; a2[2 * e + 1] += fm.y * fa.y;
+      }
+      *reinterpret_cast<int4*>(dv + b * lddv + c) = make_int4((int)ov[0], (int)ov[1], (int)ov[2], (int)ov[3]);
+      *reinterpret_cast<int4*>(dm + b * lddm + c) = make_int4((int)om[0], (int)om[1], (int)om[2], (int)om[3]);
+    }
+  }
+  extern __shared__ float sh[];                  // [rows_par][2N]
+  if (tr < rows_par) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { sh[tr * 2 * N + c + j] = a1[j]; sh[tr * 2 * N + N + c + j] = a2[j]; }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < 2 * N; i += blockDim.x) {
+    float sum = 0.f;
+    for (int r = 0; r < rows_par; ++r) sum += sh[r * 2 * N + i];
+    part[(int64_t)blockIdx.x * 2 * N + i] = sum;
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -643,6 +783,60 @@ int dr_cuda_cross_split(const float* dx0, int64_t lddx, const void* dxa, int64_t
   if (lddx < (int64_t)(T + 1) * D || (dxa && ldda < (int64_t)(T + 1) * D) || ldy < D) return -5;
   DR_PDL_LAUNCH((k_cross_split), grid_for(B * ((T + 1) * D / 8), 256), 256, 0, s, dx0, lddx, (const __nv_bfloat16*)dxa, ldda, B, T, D,
                 (__nv_bfloat16*)dy, ldy, (__nv_bfloat16*)demb);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// MaskBlock LayerNorm + ReLU backward (k_ln_relu_bwd): dh (bf16, pitch ldh) from g, the forward output y (its ReLU mask), x^ and rstd of the
+// LayerNorm GEMM epilogue, and gamma; dgamma += sum d * x^ and dbeta += sum d over the rows, summed in block order.  N <= 128; bf16 operands:
+// N and the pitches multiples of 8, 16-byte aligned.  -2 bad N or pitch, -3 misaligned, -5 a pitch < N or no workspace.
+int dr_cuda_ln_relu_bwd(const void* g, int64_t ldg, const void* y, int64_t ldy, const void* xhat, int64_t ldx, const float* rstd, const float* gamma,
+                        int64_t M, int N, void* dh, int64_t ldh, float* dgamma, float* dbeta, cudaStream_t s) {
+  if (M <= 0 || N <= 0) return 0;
+  if ((N % 8) || N > 128 || (ldg % 8) || (ldy % 8) || (ldx % 8) || (ldh % 8)) return -2;
+  if (((uintptr_t)g | (uintptr_t)y | (uintptr_t)xhat | (uintptr_t)dh) & 15) return -3;
+  if (ldg < N || ldy < N || ldx < N || ldh < N) return -5;
+  const int grid = grid_for((M + 7) / 8, 4, num_sms() * 4);             // >= 4 rows per warp
+  float* part = dr_workspace(kWsLnBwd, (size_t)grid * 2 * N, s);
+  if (!part) return -5;
+  DR_PDL_LAUNCH((k_ln_relu_bwd), grid, kLnBwdThreads, 0, s, (const __nv_bfloat16*)g, ldg, (const __nv_bfloat16*)y, ldy, (const __nv_bfloat16*)xhat, ldx,
+                rstd, gamma, M, N, (__nv_bfloat16*)dh, ldh, part);
+  DR_LAUNCH_CHECK();
+  det_colsum(part, grid, 2 * (int64_t)N, {{0, N, dgamma}, {N, N, dbeta}}, s);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// p = (a * scale + shift) * v  (k_bn_apply_mul): scale / shift from dr_cuda_bn_finalize (training or running statistics).  N and the pitches
+// multiples of 8, bf16 operands 16-byte aligned.
+int dr_cuda_bn_apply_mul(const void* a, int64_t lda, const float* scale, const float* shift, const void* v, int64_t ldv, int64_t B, int N, void* p,
+                         int64_t ldp, cudaStream_t s) {
+  if (B <= 0 || N <= 0) return 0;
+  if ((N % 8) || (lda % 8) || (ldv % 8) || (ldp % 8)) return -2;
+  if (((uintptr_t)a | (uintptr_t)v | (uintptr_t)p) & 15) return -3;
+  if (lda < N || ldv < N || ldp < N) return -5;
+  DR_PDL_LAUNCH((k_bn_apply_mul), grid_for(B * (N / 8), 256), 256, 0, s, (const __nv_bfloat16*)a, lda, scale, shift, (const __nv_bfloat16*)v, ldv, B, N,
+                (__nv_bfloat16*)p, ldp);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+// Backward of dr_cuda_bn_apply_mul (k_bn_mul_bwd): dv = dp * (a * scale + shift), dm = dp * v (bf16), S1 += sum dm, S2 += sum dm * a over
+// the rows (of the bf16 dm), summed in block order; then dr_cuda_bn_bwd_finalize and dr_cuda_bn_bwd_apply(_v2) give da.  N / 8 <= 256.
+int dr_cuda_bn_mul_bwd(const void* dp, int64_t ldp, const void* a, int64_t lda, const void* v, int64_t ldv, const float* scale, const float* shift,
+                       int64_t B, int N, void* dv, int64_t lddv, void* dm, int64_t lddm, float* S1, float* S2, cudaStream_t s) {
+  if (B <= 0 || N <= 0) return 0;
+  if ((N % 8) || N / 8 > 256 || (ldp % 8) || (lda % 8) || (ldv % 8) || (lddv % 8) || (lddm % 8)) return -2;
+  if (((uintptr_t)dp | (uintptr_t)a | (uintptr_t)v | (uintptr_t)dv | (uintptr_t)dm) & 15) return -3;
+  if (ldp < N || lda < N || ldv < N || lddv < N || lddm < N) return -5;
+  const int rows_par = 256 / (N / 8);
+  const int grid = grid_for((B + rows_par - 1) / rows_par, 2, num_sms() * 4);
+  float* part = dr_workspace(kWsBnMul, (size_t)grid * 2 * N, s);
+  if (!part) return -5;
+  DR_PDL_LAUNCH((k_bn_mul_bwd), grid, 256, rows_par * 2 * N * sizeof(float), s, (const __nv_bfloat16*)dp, ldp, (const __nv_bfloat16*)a, lda,
+                (const __nv_bfloat16*)v, ldv, scale, shift, B, N, (__nv_bfloat16*)dv, lddv, (__nv_bfloat16*)dm, lddm, part);
+  DR_LAUNCH_CHECK();
+  det_colsum(part, grid, 2 * (int64_t)N, {{0, N, S1}, {N, N, S2}}, s);
   DR_LAUNCH_CHECK();
   return 0;
 }

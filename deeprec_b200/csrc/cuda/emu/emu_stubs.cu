@@ -75,6 +75,43 @@ int dr_cuda_gemm_tn_cross(const void* A, int64_t lda, const void* B, int64_t ldb
   return 0;
 }
 
+// gemm_wgmma.cu::dr_cuda_gemm_tn_ln: h = acc (+ bias), out = relu?(gamma * x^ + beta), x^ = (h - mean) * rstd over each row's N columns
+// (two-pass variance), x^ (bf16) and rstd (fp32) optional; same return codes.
+int dr_cuda_gemm_tn_ln(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* bias, const float* gamma,
+                       const float* beta, float eps, int relu, void* out, int64_t ldc, void* xhat, int64_t ld_xhat, float* rstd, int max_ctas,
+                       cudaStream_t) {
+  (void)max_ctas;
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  if (!gamma || !beta) return -4;
+  if ((lda % 8) || (ldb % 8) || (ldc % 8) || (N % 8) || N > 128 || (xhat && ld_xhat % 8)) return -2;
+  if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)out | (uintptr_t)xhat) & 15) return -3;
+  if (lda < K || ldb < K || ldc < N || (xhat && ld_xhat < N)) return -5;
+  const __nv_bfloat16* a = (const __nv_bfloat16*)A; const __nv_bfloat16* b = (const __nv_bfloat16*)B;
+  __nv_bfloat16* o = (__nv_bfloat16*)out; __nv_bfloat16* xo = (__nv_bfloat16*)xhat;
+  float h[128];
+  for (int m = 0; m < M; ++m) {
+    float sum = 0.f, sq = 0.f;
+    for (int n = 0; n < N; ++n) {
+      float acc = 0.f;
+      for (int k = 0; k < K; ++k) acc += bf(a + (int64_t)m * lda + k) * bf(b + (int64_t)n * ldb + k);
+      h[n] = acc + (bias ? bias[n] : 0.f);
+      sum += h[n];
+    }
+    const float mu = sum / (float)N;
+    for (int n = 0; n < N; ++n) sq += (h[n] - mu) * (h[n] - mu);
+    const float rs = 1.f / sqrtf(sq / (float)N + eps);
+    if (rstd) rstd[m] = rs;
+    for (int n = 0; n < N; ++n) {
+      const float x = (h[n] - mu) * rs;
+      float y = gamma[n] * x + beta[n];
+      if (relu && y < 0.f) y = 0.f;
+      o[(int64_t)m * ldc + n] = __float2bfloat16(y);
+      if (xo) xo[(int64_t)m * ld_xhat + n] = __float2bfloat16(x);
+    }
+  }
+  return 0;
+}
+
 // gemm_wgmma.cu::dr_cuda_gemm_dw: dW[N_out,K_in](ldw, fp32, accumulated into) += dY[batch,N_out](ldy)^T * X[batch,K_in](ldx)
 int dr_cuda_gemm_dw(const void* dY, int64_t ldy, const void* X, int64_t ldx, int batch, int N_out, int K_in, float* dW, int64_t ldw, int splits, cudaStream_t) {
   (void)splits;

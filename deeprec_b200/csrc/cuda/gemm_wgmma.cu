@@ -91,13 +91,23 @@ struct Epilogue {
 // Epilogue kinds beyond the bias / ReLU / mask / statistics of kind 0.  The kind is a template parameter and only the new kinds take the
 // wider parameter block, so the kind-0 instantiations compile exactly as before.  The aux operand (mask_src, ld_mask) is x_l for kEpiCross
 // and the addend for kEpiResidual; both run with relu = 0 and aux_mode = 0.
-enum { kEpiPlain = 0, kEpiCross = 1, kEpiResidual = 2 };
+enum { kEpiPlain = 0, kEpiCross = 1, kEpiResidual = 2, kEpiLayerNorm = 3 };
 struct EpilogueX : Epilogue {
   const __nv_bfloat16* x0;        // kEpiCross: the x0 factor [M, ld_x0]
   __nv_bfloat16* u_out;           // kEpiCross: optional u = acc + bias [M, ld_u] (bf16), kept for the backward
   int64_t ld_x0, ld_u;
 };
-template <int EPI> using EpiT = std::conditional_t<EPI == kEpiPlain, Epilogue, EpilogueX>;
+// kEpiLayerNorm: a row's N <= BLOCK_N columns sit in one tile, so its LayerNorm runs on the fp32 accumulators; relu applies after the norm.
+struct EpilogueLN : Epilogue {
+  const float* gamma;             // [N]
+  const float* beta;              // [N]
+  __nv_bfloat16* xhat;            // optional x^ = (h - mean) * rstd [M, ld_xhat] (bf16), kept for the backward
+  float* rstd;                    // optional [M]
+  int64_t ld_xhat;
+  float eps;
+};
+template <int EPI>
+using EpiT = std::conditional_t<EPI == kEpiPlain, Epilogue, std::conditional_t<EPI == kEpiLayerNorm, EpilogueLN, EpilogueX>>;
 
 // UE8M0 scale byte -> 2^(b - 127)  (b = 0 is the denormal 2^-127)
 __device__ __forceinline__ float ue8m0(uint32_t b) { return b ? __uint_as_float(b << 23) : 5.877471754111438e-39f; }
@@ -173,7 +183,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
           const __grid_constant__ CUtensorMap tmAux, int M, int N, int K, EpiT<EPI> ep) {
   static_assert(!PP || (!BRES && !CL2 && !FP8), "ping-pong consumers: bf16 streaming kernel only");
-  static_assert(EPI == kEpiPlain || (!PP && !BRES && !CL2 && !FP8), "cross / residual epilogues: bf16 cooperative streaming kernel only");
+  static_assert(EPI == kEpiPlain || (!PP && !BRES && !CL2 && !FP8), "cross / residual / LayerNorm epilogues: bf16 cooperative streaming kernel only");
   using L = SmemLayoutTN<BLOCK_N, BRES, PP>;
   constexpr int kSt = L::kSt;
   constexpr int kAcc = BLOCK_N / 2;
@@ -465,6 +475,69 @@ k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 
       // ---- fused epilogue straight from the accumulator registers
       const int row0 = m_blk * BLOCK_M + wg * 64 + wl * 16 + (lane >> 2);
+      if constexpr (EPI == kEpiLayerNorm) {
+        // rows row0 and row0 + 8 of this thread: the 4 lanes of a quad hold all BLOCK_N columns of both.  h = acc + bias; the mean and the
+        // two-pass variance over the N real columns are in-thread sums plus two shuffles inside the quad.
+        const float inv_n = 1.f / (float)N;
+        float sum[2] = {0.f, 0.f};
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int col = 8 * j + 2 * (lane & 3);
+          if (col < N) {
+            const float b0 = ep.bias ? __ldg(ep.bias + col) : 0.f, b1 = ep.bias ? __ldg(ep.bias + col + 1) : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              acc[4 * j + 2 * h] += b0; acc[4 * j + 2 * h + 1] += b1;
+              sum[h] += acc[4 * j + 2 * h] + acc[4 * j + 2 * h + 1];
+            }
+          }
+        }
+        float mu[2], sq[2] = {0.f, 0.f}, rs[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+          sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+          mu[h] = sum[h] * inv_n;
+        }
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          if (8 * j + 2 * (lane & 3) < N) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float d0 = acc[4 * j + 2 * h] - mu[h], d1 = acc[4 * j + 2 * h + 1] - mu[h];
+              sq[h] = fmaf(d0, d0, fmaf(d1, d1, sq[h]));
+            }
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 1);
+          sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 2);
+          rs[h] = rsqrtf(sq[h] * inv_n + ep.eps);
+          const int row = row0 + 8 * h;
+          if (ep.rstd && (lane & 3) == 0 && row < M) ep.rstd[row] = rs[h];
+        }
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int col = 8 * j + 2 * (lane & 3);
+          if (col < N) {
+            const float g0 = __ldg(ep.gamma + col), g1 = __ldg(ep.gamma + col + 1);
+            const float e0 = __ldg(ep.beta + col), e1 = __ldg(ep.beta + col + 1);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = row0 + 8 * h;
+              if (row < M) {
+                const float x0 = (acc[4 * j + 2 * h] - mu[h]) * rs[h], x1 = (acc[4 * j + 2 * h + 1] - mu[h]) * rs[h];
+                float y0 = fmaf(g0, x0, e0), y1 = fmaf(g1, x1, e1);
+                if (ep.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+                *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + (int64_t)row * ep.ldc + col) = pack_bf16x2(y0, y1);
+                if (ep.xhat) *reinterpret_cast<uint32_t*>(ep.xhat + (int64_t)row * ep.ld_xhat + col) = pack_bf16x2(x0, x1);
+              }
+            }
+          }
+        }
+        continue;
+      }
       const bool stats = !FP8 && ep.S1 != nullptr;
 #pragma unroll
       for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -830,6 +903,33 @@ int dr_cuda_gemm_tn_cross(const void* A, int64_t lda, const void* B, int64_t ldb
   rc = N <= 16 ? TN_EPI(16) : N <= 32 ? TN_EPI(32) : N <= 64 ? TN_EPI(64) : TN_EPI(128);
 #undef TN_EPI
   return rc;
+}
+
+// LayerNorm epilogue (MaskNet's MaskBlock, nn.FusedMaskBlock), on the cooperative kernel at every K:
+//   h = acc + bias,  x^ = (h - mean_row(h)) * rstd,  rstd = 1 / sqrt(var_row(h) + eps),  out = relu?(gamma * x^ + beta)
+// with acc = A[M,K](lda) * B[N,K](ldb)^T in fp32, the row mean and the two-pass variance sum((h - mean)^2) / N over the N columns from the
+// fp32 accumulators, out rounded once to bf16.  bias may be null; x^ (bf16, pitch ld_xhat) and rstd (fp32 [M]) are optional.  out may be a
+// column slice of a wider buffer (ldc > N).  Contract of dr_cuda_gemm_tn_ex for A, B and out, and:  -2  N > 128 (a row must fit one tile),
+// N or a pitch of out / xhat not a multiple of 8;  -3  xhat not 16-byte aligned;  -5  ld_xhat < N;  -4  gamma or beta missing.
+int dr_cuda_gemm_tn_ln(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, const float* bias, const float* gamma,
+                       const float* beta, float eps, int relu, void* out, int64_t ldc, void* xhat, int64_t ld_xhat, float* rstd, int max_ctas,
+                       cudaStream_t s) {
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  if (!gamma || !beta) return -4;
+  if ((lda % 8) || (ldb % 8) || (ldc % 8) || (N % 8) || N > 128 || (xhat && ld_xhat % 8)) return -2;
+  if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)out | (uintptr_t)xhat) & 15) return -3;
+  if (lda < K || ldb < K || ldc < N || (xhat && ld_xhat < N)) return -5;
+  if (max_ctas <= 0) max_ctas = num_sms();
+  CUtensorMap ta;
+  int rc = make_tmap(&ta, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BLOCK_K, BLOCK_M);
+  if (rc) return rc;
+  EpilogueLN ep;
+  static_cast<Epilogue&>(ep) = Epilogue{bias, nullptr, out, nullptr, ldc, 0, relu, 0, nullptr, nullptr, nullptr, nullptr, 0, 1.f};
+  ep.gamma = gamma; ep.beta = beta; ep.xhat = (__nv_bfloat16*)xhat; ep.rstd = rstd; ep.ld_xhat = ld_xhat; ep.eps = eps;
+  if (N <= 16) return launch_tn<16, false, false, false, false, false, kEpiLayerNorm>(ta, B, M, N, K, ldb, ep, max_ctas, s);
+  if (N <= 32) return launch_tn<32, false, false, false, false, false, kEpiLayerNorm>(ta, B, M, N, K, ldb, ep, max_ctas, s);
+  if (N <= 64) return launch_tn<64, false, false, false, false, false, kEpiLayerNorm>(ta, B, M, N, K, ldb, ep, max_ctas, s);
+  return launch_tn<128, false, false, false, false, false, kEpiLayerNorm>(ta, B, M, N, K, ldb, ep, max_ctas, s);
 }
 
 // A/B switches for the GEMM variants (same effect as DEEPREC_GEMM_2CTA / DEEPREC_GEMM_BRES, settable at run time; return the previous value).

@@ -21,7 +21,7 @@ from deeprec_b200.utils import Trainer
 
 def get_arg_parser():
     p = argparse.ArgumentParser()
-    p.add_argument("--model", default="dlrm")
+    p.add_argument("--model", default="dlrm", help="dlrm or a zoo model (models/zoo.py: CRITEO_MODELS, TAOBAO_MODELS); masknet_parallel / masknet_serial are the reference MaskNet's two modes")
     p.add_argument("--steps", type=int, default=100)
     p.add_argument("--batch_size", type=int, default=2048)
     p.add_argument("--learning_rate", type=float, default=0.01)
@@ -51,7 +51,7 @@ def get_arg_parser():
                         "roles with `python -m deeprec_b200.parallel.ps_train`")
     p.add_argument("--timeline", type=int, default=0)
     p.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
-    p.add_argument("--engine", action="store_true", help="fused sm_90a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / DIN / DIEN / BST, and DSSM / ESMM / MMoE / DBMTL / PLE / SimpleMultiTask over pooled history bags, through FusedRecEngine (models/rec_engine.py)")
+    p.add_argument("--engine", action="store_true", help="fused sm_90a engines: DLRM (models/dlrm_engine.py); WDL / DeepFM / DCN / DCNv2 / MaskNet / masknet_parallel / masknet_serial (the reference MaskNet, MaskBlocks on nn.FusedMaskBlock) / DIN / DIEN / BST, and DSSM / ESMM / MMoE / DBMTL / PLE / SimpleMultiTask over pooled history bags, through FusedRecEngine (models/rec_engine.py)")
     p.add_argument("--interaction_op", default="dot", choices=["dot", "dcnv2"],
                    help="--model dlrm: the dot interaction, or DLRM-DCNv2 (a low-rank cross net; with --engine the MLPerf shapes: D = 128, "
                         "bottom 512-256-128, top 1024-1024-512-256, 3 cross layers of rank 512)")

@@ -1,6 +1,6 @@
 """Model zoo on the framework API (modelzoo/ in the reference: 15 models with one flag surface).
 
-Criteo-shaped (dense [B,13], ids [T,B]):  WDL, DLRM (models/dlrm.py), DeepFM, DCN, DCNv2, MaskNet
+Criteo-shaped (dense [B,13], ids [T,B]):  WDL, DLRM (models/dlrm.py), DeepFM, DCN, DCNv2, MaskNet, MaskBlockNet (parallel / serial)
 Taobao-shaped (user/item/cat + behaviour history): DIN, DIEN, BST, DSSM, and the multi-task family ESMM, MMoE, DBMTL,
 PLE, SimpleMultiTask.
 
@@ -267,6 +267,46 @@ class MaskNet(CriteoModel):
         for m, b in zip(self.masks, self.blocks):
             h = b(h * m(v))
         return self.out(torch.cat([h, dense], 1)).squeeze(-1)
+
+
+class MaskBlockNet(CriteoModel):
+    """MaskNet as the reference builds it (masknet/train.py:97-224): x = [13 dense | 26 embeddings] (429 wide at dim 16) feeds every MaskBlock
+    (:class:`nn.FusedMaskBlock`) as V_emb.
+
+    * ``model_type="parallel"`` (the reference's default): ``num_blocks`` blocks on (x, x), concatenated, then ``[64, 16]`` with ReLU and
+      BatchNorm and a plain Linear(16, 1) logit.  The reference's ``_dnn([64, 16, 1])`` also puts ReLU and BatchNorm on the 1-unit logit,
+      which pins the logit at >= 0 before a per-batch normalisation; that quirk is not reproduced.
+    * ``model_type="serial"``: V_out = block_i(x, V_out) from V_out = x, then Linear(block_dim, 1).
+
+    ``reduction_ratio`` widens each block's first mask layer to ``hidden_in * reduction_ratio``.  :class:`MaskNet` is this project's older serial
+    variant and stays as it is."""
+
+    def __init__(self, model_type: str = "parallel", num_blocks: int = 5, block_dim: int = 64, reduction_ratio: int = 1, **kw):
+        super().__init__(name=kw.pop("name", f"masknet_{model_type}"), **kw)
+        from ..nn import FusedMaskBlock
+        if model_type not in ("parallel", "serial"):
+            raise ValueError(f"MaskBlockNet: model_type must be parallel | serial, not {model_type!r}")
+        dev = kw.get("device")
+        self.model_type = model_type
+        d = self.num_dense + self.num_sparse * self.emb_dim
+        hidden = [d] * num_blocks if model_type == "parallel" else [d] + [block_dim] * (num_blocks - 1)
+        self.blocks = nn.ModuleList([FusedMaskBlock(h, d, block_dim, reduction_ratio, device=dev) for h in hidden])
+        if model_type == "parallel":
+            self.head = mlp((64, 16), num_blocks * block_dim, bn=True, device=dev)
+            self.out = nn.Linear(16, 1, device=dev)
+        else:
+            self.head = nn.Identity()
+            self.out = nn.Linear(block_dim, 1, device=dev)
+
+    def logits(self, dense, embs):
+        x = torch.cat([dense, embs.flatten(1)], 1)
+        if self.model_type == "parallel":
+            h = torch.cat([b(x, x) for b in self.blocks], 1)
+        else:
+            h = x
+            for b in self.blocks:
+                h = b(x, h)
+        return self.out(self.head(h)).squeeze(-1)
 
 
 # --------------------------------------------------------------------------------------------------------------
@@ -569,8 +609,14 @@ class DLRMDCN(CriteoModel):
         return self.out(self.top(x)).squeeze(-1)
 
 
+def _masknet(model_type: str):
+    def build(**kw):
+        return MaskBlockNet(model_type=model_type, **kw)
+    return build
+
+
 CRITEO_MODELS = {"wdl": WDL, "wide_and_deep": WDL, "deepfm": DeepFM, "dcn": DCN, "dcnv2": DCNv2, "masknet": MaskNet, "dlrm_dcn": DLRMDCN,
-                 "mlperf": DLRMDCN}
+                 "mlperf": DLRMDCN, "masknet_parallel": _masknet("parallel"), "masknet_serial": _masknet("serial")}
 TAOBAO_MODELS = {"din": DIN, "dien": DIEN, "bst": BST, "dssm": DSSM, "esmm": ESMM, "mmoe": MMoE, "dbmtl": DBMTL, "ple": PLE,
                  "simple_multitask": SimpleMultiTask}
 

@@ -11,6 +11,8 @@
     forward and backward through time on csrc/cuda/rnn_kernels.cu.
   * ``fused_encoder_layer``: a post-norm Transformer encoder layer with a key-padding mask for training -- in_proj, out_proj and the FFN on
     the wgmma GEMM, the multi-head self-attention core forward and backward on csrc/cuda/mha_kernels.cu.
+  * ``FusedMaskBlock``: MaskNet's MaskBlock as one autograd node -- the mask MLP's GEMMs with their BatchNorm statistics in the epilogue,
+    the last BatchNorm fused with the instance-guided product, and the block's Linear with LayerNorm + ReLU in the GEMM epilogue.
 
 The reference runs these through cuBLAS (stream_executor/cuda/cuda_blas.cc) and ~10 TF ops per interaction
 (modelzoo/dlrm/train.py:163-236, modelzoo/deepfm/train.py:178-187).  CPU tensors fall back to the equivalent torch expression.
@@ -56,6 +58,19 @@ def _to_bf16_padded(x: torch.Tensor, Kp: int) -> torch.Tensor:
     return y.contiguous()
 
 
+def _pack_weight(W: torch.Tensor, Np: int, Kp: int):
+    """fp32 master W [N, K] -> (bf16 W [Np, Kp], bf16 W^T [Kp, Np]), zero padded: the B operands of the forward and the dX GEMM."""
+    N, K = W.shape
+    Wp = W.detach().float()
+    if (Np, Kp) != (N, K):
+        Wp = F.pad(Wp, (0, Kp - K, 0, Np - N))
+    Wp = Wp.contiguous()
+    wb = torch.empty(Np, Kp, dtype=torch.bfloat16, device=W.device)
+    wt = torch.empty(Kp, Np, dtype=torch.bfloat16, device=W.device)
+    check(_native.cuda().dr_cuda_pack_weights(ptr(Wp), Np, Kp, ptr(wb), ptr(wt), Np, stream_ptr()), "pack_weights")
+    return wb, wt
+
+
 class _FusedMLPFn(torch.autograd.Function):
     """y = L_n(...relu(L_1(x))) ; ``params`` = W_1, b_1, ..., W_n, b_n (fp32 masters, W_i [N_i, K_i])."""
 
@@ -75,13 +90,7 @@ class _FusedMLPFn(torch.autograd.Function):
             N, K = W.shape
             Np, Kp = _pad8(N), _pad8(K)
             assert Kp == acts[-1].shape[1], f"layer {i}: expected input width {K}, got {acts[-1].shape[1]}"
-            Wp = W.detach().float()
-            if (Np, Kp) != (N, K):
-                Wp = F.pad(Wp, (0, Kp - K, 0, Np - N))
-            Wp = Wp.contiguous()
-            wb = torch.empty(Np, Kp, dtype=torch.bfloat16, device=dev)
-            wt = torch.empty(Kp, Np, dtype=torch.bfloat16, device=dev)
-            check(lib.dr_cuda_pack_weights(ptr(Wp), Np, Kp, ptr(wb), ptr(wt), Np, s), "pack_weights")
+            wb, wt = _pack_weight(W, Np, Kp)
             bias = b.detach().float() if b is not None else None
             if bias is not None and Np != N:
                 bias = F.pad(bias, (0, Np - N))
@@ -387,3 +396,167 @@ def fused_encoder_layer(x: torch.Tensor, layer: nn.TransformerEncoderLayer, vali
     h = layer.norm1(x2 + a.to(x.dtype))
     f = _FusedMLPFn.apply(h.to(torch.bfloat16), False, layer.linear1.weight, layer.linear1.bias, layer.linear2.weight, layer.linear2.bias)
     return layer.norm2(h + f.to(h.dtype)).reshape(B, S, E)
+
+
+# ---- MaskNet MaskBlock -------------------------------------------------------------------------------------------------------
+MASKBLOCK_MAX_OUT = 128               # the LayerNorm GEMM epilogue holds a whole output row in one tile
+
+
+def _bn_tf(x: torch.Tensor, bn: nn.BatchNorm1d) -> torch.Tensor:
+    """``tf.layers.batch_normalization`` of [B, N]: batch statistics while training, the moving averages updated with the biased batch
+    variance at decay ``1 - bn.momentum`` (what dr_cuda_bn_finalize does; torch's BatchNorm1d would use the unbiased variance); the moving
+    averages in eval mode."""
+    if not bn.training:
+        return F.batch_norm(x, bn.running_mean, bn.running_var, bn.weight, bn.bias, False, 0.0, bn.eps)
+    with torch.no_grad():
+        xf = x.detach().float()
+        bn.running_mean.mul_(1.0 - bn.momentum).add_(xf.mean(0), alpha=bn.momentum)
+        bn.running_var.mul_(1.0 - bn.momentum).add_(xf.var(0, unbiased=False), alpha=bn.momentum)
+    return F.batch_norm(x, None, None, bn.weight, bn.bias, True, 0.0, bn.eps)
+
+
+class _FusedMaskBlockFn(torch.autograd.Function):
+    """out = relu(LN(W3 (BN2(relu(W2 BN1(relu(W1 v_emb + b1)) + b2)) * v_hidden)))  on the kernels; ``params`` = W1, b1, gamma1, beta1, W2, b2,
+    gamma2, beta2, W3, gamma_ln, beta_ln (fp32 masters).  The BatchNorm moving averages of ``blk`` are updated in place by dr_cuda_bn_finalize.
+    Widths are zero padded to multiples of 8: padded weight rows / columns, BatchNorm scale and shift are 0, so padded columns stay 0."""
+
+    @staticmethod
+    def forward(ctx, v_emb, v_hidden, blk, training: bool, *params):
+        lib, s, dev = _native.cuda(), stream_ptr(), v_emb.device
+        W1, b1, g1, be1, W2, b2, g2, be2, W3, gl, bl = params
+        M, E = v_emb.shape
+        H, R, O = v_hidden.shape[1], W1.shape[0], W3.shape[0]
+        Ep, Hp, Rp = _pad8(E), _pad8(H), _pad8(R)
+        f32 = dict(dtype=torch.float32, device=dev)
+        bf = dict(dtype=torch.bfloat16, device=dev)
+        xe = _to_bf16_padded(v_emb, Ep)
+        xh = xe if v_hidden is v_emb else _to_bf16_padded(v_hidden, Hp)
+        w1b, w1t = _pack_weight(W1, Rp, Ep)
+        w2b, w2t = _pack_weight(W2, Hp, Rp)
+        w3b, w3t = _pack_weight(W3, O, Hp)
+
+        def lin_relu_bn(x, Kp, wb, b, N, Np, bn, g, be):
+            """a = relu(x W^T + b) with its column statistics in the GEMM epilogue -> st = [mean | rstd | scale | shift] of the BatchNorm"""
+            a = torch.empty(M, Np, **bf)
+            S = torch.zeros(2, Np, **f32) if training else None
+            bias = F.pad(b.detach().float(), (0, Np - N)).contiguous()
+            check(lib.dr_cuda_gemm_tn_ex(ptr(x), Kp, ptr(wb), Kp, M, Np, Kp, ptr(bias), 1, None, 0, 0, ptr(a), Np, None,
+                                         ptr(S[0]) if training else None, ptr(S[1]) if training else None, 0, 0, s), "gemm_tn")
+            st = torch.zeros(4, Np, **f32)
+            check(lib.dr_cuda_bn_finalize(ptr(S[0]) if training else None, ptr(S[1]) if training else None, N, M, ptr(g.detach().float().contiguous()),
+                                          ptr(be.detach().float().contiguous()), bn.eps, 1.0 - bn.momentum, ptr(bn.running_mean), ptr(bn.running_var),
+                                          ptr(st[0]), ptr(st[1]), ptr(st[2]), ptr(st[3]), int(training), s), "bn_finalize")
+            return a, st
+
+        a1, st1 = lin_relu_bn(xe, Ep, w1b, b1, R, Rp, blk.bn1, g1, be1)
+        m1 = torch.empty(M, Rp, **bf)
+        check(lib.dr_cuda_bn_apply(ptr(a1), M, Rp, Rp, ptr(st1[2]), ptr(st1[3]), ptr(m1), Rp, s), "bn_apply")
+        a2, st2 = lin_relu_bn(m1, Rp, w2b, b2, H, Hp, blk.bn2, g2, be2)
+        p = torch.empty(M, Hp, **bf)
+        check(lib.dr_cuda_bn_apply_mul(ptr(a2), Hp, ptr(st2[2]), ptr(st2[3]), ptr(xh), Hp, M, Hp, ptr(p), Hp, s), "bn_apply_mul")
+        y = torch.empty(M, O, **bf)
+        xhat = torch.empty(M, O, **bf)
+        rstd = torch.empty(M, **f32)
+        glf = gl.detach().float().contiguous()
+        check(lib.dr_cuda_gemm_tn_ln(ptr(p), Hp, ptr(w3b), Hp, M, O, Hp, None, ptr(glf), ptr(bl.detach().float().contiguous()), blk.ln.eps, 1,
+                                     ptr(y), O, ptr(xhat), O, ptr(rstd), 0, s), "gemm_tn_ln")
+        ctx.save_for_backward(xe, xh, a1, m1, a2, p, y, xhat, rstd, w1t, w2t, w3t, st1, st2, glf)
+        ctx.meta = (E, H, R, O, v_emb.dtype, v_hidden.dtype)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib, s = _native.cuda(), stream_ptr()
+        xe, xh, a1, m1, a2, p, y, xhat, rstd, w1t, w2t, w3t, st1, st2, glf = ctx.saved_tensors
+        E, H, R, O, edt, hdt = ctx.meta
+        M, Ep, Hp, Rp = xe.shape[0], xe.shape[1], xh.shape[1], a1.shape[1]
+        dev = gy.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        bf = dict(dtype=torch.bfloat16, device=dev)
+        g = gy.to(torch.bfloat16).contiguous()
+        # LayerNorm + ReLU, then the block's Linear (no bias)
+        dh = torch.empty(M, O, **bf)
+        dgl, dbl = torch.zeros(O, **f32), torch.zeros(O, **f32)
+        check(lib.dr_cuda_ln_relu_bwd(ptr(g), O, ptr(y), O, ptr(xhat), O, ptr(rstd), ptr(glf), M, O, ptr(dh), O, ptr(dgl), ptr(dbl), s), "ln_relu_bwd")
+        dW3 = torch.zeros(O, Hp, **f32)
+        check(lib.dr_cuda_gemm_dw(ptr(dh), O, ptr(p), Hp, M, O, Hp, ptr(dW3), Hp, 0, s), "gemm_dw")
+        dp = torch.empty(M, Hp, **bf)
+        check(lib.dr_cuda_gemm_tn_ex(ptr(dh), O, ptr(w3t), O, M, Hp, O, None, 0, None, 0, 0, ptr(dp), Hp, None, None, None, 0, 0, s), "gemm_dx")
+        # p = BN2(a2) * v_hidden: dv_hidden, and the BatchNorm-backward sums of dm = dp * v_hidden
+        dv = torch.empty(M, Hp, **bf)
+        dm = torch.empty(M, Hp, **bf)
+        S = torch.zeros(2, Hp, **f32)
+        check(lib.dr_cuda_bn_mul_bwd(ptr(dp), Hp, ptr(a2), Hp, ptr(xh), Hp, ptr(st2[2]), ptr(st2[3]), M, Hp, ptr(dv), Hp, ptr(dm), Hp, ptr(S[0]), ptr(S[1]), s),
+              "bn_mul_bwd")
+
+        def bn_relu_lin_bwd(dy, a, st, S, N, Np, x, Kp):
+            """BatchNorm backward (with the ReLU mask of a) from the sums S, then the Linear's weight and bias gradients against its input x"""
+            dg, dbe, c = torch.zeros(N, **f32), torch.zeros(N, **f32), torch.zeros(2, Np, **f32)
+            check(lib.dr_cuda_bn_bwd_finalize(ptr(S[0]), ptr(S[1]), N, M, ptr(st[0]), ptr(st[1]), ptr(dg), ptr(dbe), ptr(c[0]), ptr(c[1]), 1.0, s),
+                  "bn_bwd_finalize")
+            da, db = torch.empty(M, Np, **bf), torch.zeros(Np, **f32)
+            check(lib.dr_cuda_bn_bwd_apply_v2(ptr(dy), ptr(a), M, Np, Np, ptr(st[2]), ptr(st[0]), ptr(st[1]), ptr(c[0]), ptr(c[1]), ptr(da), 1, ptr(db), s),
+                  "bn_bwd_apply")
+            dW = torch.zeros(Np, Kp, **f32)
+            check(lib.dr_cuda_gemm_dw(ptr(da), Np, ptr(x), Kp, M, Np, Kp, ptr(dW), Kp, 0, s), "gemm_dw")
+            return da, dW, db, dg, dbe
+
+        da2, dW2, db2, dg2, dbe2 = bn_relu_lin_bwd(dm, a2, st2, S, H, Hp, m1, Rp)
+        # dm1 = da2 W2, with the BatchNorm-backward sums of layer 1 (sum dm1, sum dm1 * a1) in the GEMM epilogue
+        dm1 = torch.empty(M, Rp, **bf)
+        S = torch.zeros(2, Rp, **f32)
+        check(lib.dr_cuda_gemm_tn_ex(ptr(da2), Hp, ptr(w2t), Hp, M, Rp, Hp, None, 0, ptr(a1), Rp, 2, ptr(dm1), Rp, None, ptr(S[0]), ptr(S[1]), 0, 0, s),
+              "gemm_dx")
+        da1, dW1, db1, dg1, dbe1 = bn_relu_lin_bwd(dm1, a1, st1, S, R, Rp, xe, Ep)
+        dxe = None
+        if ctx.needs_input_grad[0]:
+            dxe = torch.empty(M, Ep, **bf)
+            check(lib.dr_cuda_gemm_tn_ex(ptr(da1), Rp, ptr(w1t), Rp, M, Ep, Rp, None, 0, None, 0, 0, ptr(dxe), Ep, None, None, None, 0, 0, s), "gemm_dx")
+            dxe = dxe[:, :E].to(edt)
+        dxh = dv[:, :H].to(hdt) if ctx.needs_input_grad[1] else None
+        return (dxe, dxh, None, None, dW1[:R, :E], db1[:R], dg1, dbe1, dW2[:H, :R], db2[:H], dg2, dbe2, dW3[:, :H], dgl, dbl)
+
+
+class FusedMaskBlock(nn.Module):
+    """MaskNet's MaskBlock (modelzoo/masknet/train.py:150-177):
+
+        V_mask = BN(ReLU(Linear(BN(ReLU(Linear(V_emb, hidden_in * reduction_ratio))), hidden_in)))
+        out    = ReLU(LayerNorm(Linear(V_mask * V_hidden, out_dim, bias=False)))
+
+    with tf's defaults: BatchNorm eps 1e-3 and decay 0.99 (torch momentum 0.01; the moving variance takes the biased batch variance, as
+    ``_bn_tf``), LayerNorm eps 1e-3.  ``forward(v_emb [B, emb_in], v_hidden [B, hidden_in]) -> [B, out_dim]``.
+
+    On CUDA (and on the kernel emulation), unless ``DEEPREC_FUSED_NN=0``: one autograd node on the sm_90a kernels -- bf16 activations, fp32
+    statistics and weight gradients, the BatchNorm moving averages updated inside the step (so a captured CUDA graph updates them too);
+    ``out_dim`` must be a multiple of 8 and at most ``MASKBLOCK_MAX_OUT``.  Otherwise the same expression in torch ops, which is the oracle."""
+
+    def __init__(self, hidden_in: int, emb_in: int, out_dim: int = 64, reduction_ratio: int = 1, bn_eps: float = 1e-3, bn_momentum: float = 0.01,
+                 ln_eps: float = 1e-3, device=None):
+        super().__init__()
+        self.hidden_in, self.emb_in, self.out_dim = hidden_in, emb_in, out_dim
+        r = hidden_in * reduction_ratio
+        self.fc1 = nn.Linear(emb_in, r, device=device)
+        self.bn1 = nn.BatchNorm1d(r, eps=bn_eps, momentum=bn_momentum, device=device)
+        self.fc2 = nn.Linear(r, hidden_in, device=device)
+        self.bn2 = nn.BatchNorm1d(hidden_in, eps=bn_eps, momentum=bn_momentum, device=device)
+        self.fc3 = nn.Linear(hidden_in, out_dim, bias=False, device=device)
+        self.ln = nn.LayerNorm(out_dim, eps=ln_eps, device=device)
+        for fc in (self.fc1, self.fc2, self.fc3):                 # tf.layers.dense: glorot_uniform kernel, zero bias
+            nn.init.xavier_uniform_(fc.weight)
+            if fc.bias is not None:
+                nn.init.zeros_(fc.bias)
+
+    def forward(self, v_emb: torch.Tensor, v_hidden: torch.Tensor) -> torch.Tensor:
+        import os
+        if _native.on_device(v_emb) and os.environ.get("DEEPREC_FUSED_NN", "1") != "0":
+            if self.out_dim % 8 or self.out_dim > MASKBLOCK_MAX_OUT:
+                raise ValueError(f"FusedMaskBlock: out_dim {self.out_dim} is not supported on CUDA (a multiple of 8, at most {MASKBLOCK_MAX_OUT})")
+            return _FusedMaskBlockFn.apply(v_emb, v_hidden, self, self.training, self.fc1.weight, self.fc1.bias, self.bn1.weight, self.bn1.bias,
+                                           self.fc2.weight, self.fc2.bias, self.bn2.weight, self.bn2.bias, self.fc3.weight, self.ln.weight, self.ln.bias)
+        return self.expression(v_emb, v_hidden)
+
+    def expression(self, v_emb: torch.Tensor, v_hidden: torch.Tensor) -> torch.Tensor:
+        """The block in torch ops (the CPU path and the oracle of the kernels)."""
+        m = _bn_tf(torch.relu(self.fc1(v_emb)), self.bn1)
+        m = _bn_tf(torch.relu(self.fc2(m)), self.bn2)
+        return torch.relu(self.ln(self.fc3(m * v_hidden)))

@@ -423,6 +423,24 @@ def _build_program(model, max_len: int = 50, tables: Optional[list] = None, pool
         if p.tables is None:
             p.tables = [_EvTable(ev) for ev in _evs_of(model.emb)] + [_EvTable(ev) for ev in _evs_of(model.wide)]
         p.id_map = list(range(T)) + list(range(T))
+    elif isinstance(model, zoo.MaskBlockNet):                            # reference MaskNet: blocks on x = [dense | emb]
+        x = p.concat(["dense", "emb"])
+
+        def bn_affine(src, bn):
+            s = bn.weight.detach().float() / torch.sqrt(bn.running_var.detach().float() + bn.eps)
+            return p.affine(src, s, bn.bias.detach().float() - bn.running_mean.detach().float() * s)
+
+        def block(b, v_hidden):                                          # relu(LN(W3 (BN2(relu(W2 BN1(relu(W1 x)))) * v_hidden)))
+            m = bn_affine(p.linear(x, b.fc1.weight, b.fc1.bias, relu=True), b.bn1)
+            m = bn_affine(p.linear(m, b.fc2.weight, b.fc2.bias, relu=True), b.bn2)
+            return p.layernorm(p.linear(p.mul(m, v_hidden), b.fc3.weight, None), b.ln, relu=True)
+        if model.model_type == "parallel":
+            h = p.sequential(p.concat([block(b, x) for b in model.blocks]), model.head)
+        else:
+            h = x
+            for b in model.blocks:
+                h = block(b, h)
+        p.out = p.linear(h, model.out.weight, model.out.bias)
     elif isinstance(model, zoo.MaskNet):                                 # serial MaskBlocks: h = ReLU(LN(W (h * mask(v))))
         h = p.layernorm("emb", model.ln_emb)
         for m, b in zip(model.masks, model.blocks):
@@ -547,7 +565,7 @@ def _build_program(model, max_len: int = 50, tables: Optional[list] = None, pool
             x = p.cross_linear(x0, x, p.linear(x, U.detach().t(), None), V.detach().t(), b)
         p.out = p.linear(p.sequential(x, model.top), model.out.weight, model.out.bias)
     else:
-        raise TypeError(f"op-program export: no builder for {type(model).__name__} (WDL, DeepFM, DCN, DCNv2, MaskNet, DLRMDCN, DIN, DIEN, BST, DSSM, ESMM, MMoE, DBMTL, PLE, SimpleMultiTask; DLRM has export_saved_model_module)")
+        raise TypeError(f"op-program export: no builder for {type(model).__name__} (WDL, DeepFM, DCN, DCNv2, MaskNet, MaskBlockNet, DLRMDCN, DIN, DIEN, BST, DSSM, ESMM, MMoE, DBMTL, PLE, SimpleMultiTask; DLRM has export_saved_model_module)")
     return p
 
 
