@@ -102,6 +102,10 @@ _sig("dr_cuda_bn_fold", [P, P, INT, i64, P, P, f32, f32, P, P, P, P, P, P, INT, 
 _sig("dr_cuda_dw_fixup", [P, P, P, P, INT, INT, INT, S])
 _sig("dr_cuda_bn_bwd_apply_v2", [P, P, i64, INT, i64, P, P, P, P, P, P, INT, P, S])
 _sig("dr_cuda_gemm_dw", [P, i64, P, i64, INT, INT, INT, P, i64, INT, S])
+_sig("dr_cuda_gemm_tn_grouped", [INT, P, P, P, P, INT, INT, INT, P, INT, P, P, P, P, P, INT, S])
+_sig("dr_cuda_gemm_dw_grouped", [INT, P, P, P, P, INT, INT, INT, P, P, INT, S])
+_sig("dr_cuda_moe_mix_fwd", [P, i64, i64, INT, INT, INT, P, P, P, P, P, P, P, P, P, P, S])
+_sig("dr_cuda_moe_mix_bwd", [P, i64, i64, INT, INT, INT, P, P, P, P, P, P, P, P, P, P, i64, P, P, P, S])
 _sig("dr_cuda_colstats", [P, P, i64, INT, i64, i64, P, P, S])
 _sig("dr_cuda_bn_finalize", [P, P, INT, i64, P, P, f32, f32, P, P, P, P, P, P, INT, S])
 _sig("dr_cuda_bn_apply", [P, i64, INT, i64, P, P, P, i64, S])

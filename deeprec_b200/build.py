@@ -39,6 +39,7 @@ CUDA_SOURCES = [
     "cuda/fused_ops.cu",
     "cuda/allocator.cu",
     "cuda/attention_kernels.cu",
+    "cuda/moe_kernels.cu",
     "cuda/rnn_kernels.cu",              # tensor-core GRU recurrence (mma.sync): hardware only, not in EMU_SOURCES
     "cuda/mha_kernels.cu",              # tensor-core multi-head self-attention (mma.sync): hardware only, not in EMU_SOURCES
     "cuda/sm_partition.cu",             # green-context SM partition (driver API): hardware only, not in EMU_SOURCES
@@ -133,6 +134,7 @@ EMU_SOURCES = [
     "cuda/program_kernels.cu",
     "cuda/sparse_utils.cu",
     "cuda/attention_kernels.cu",
+    "cuda/moe_kernels.cu",              # expert-mixture gates (MMoE / PLE)
     "cuda/serving_runtime.cu",
     "cuda/sparse_pipeline.cu",          # unique-first model-parallel pipeline: ranks = host threads, peer memory = the shared address space
     "cuda/comm_kernels.cu",

@@ -128,6 +128,43 @@ int dr_cuda_gemm_dw(const void* dY, int64_t ldy, const void* X, int64_t ldx, int
   return 0;
 }
 
+// gemm_wgmma.cu::dr_cuda_gemm_tn_grouped / dr_cuda_gemm_dw_grouped: every group checked first (same codes, kMaxGroups = 12), then the
+// per-group entries above, so each group's result is the one its own call gives.
+int dr_cuda_gemm_tn_grouped(int G, const void* const* A, const int64_t* lda, const void* const* B, const int64_t* ldb, int M, int N, int K,
+                            const float* const* bias, int relu, const void* const* mask_src, const int64_t* ld_mask, void* const* out,
+                            const int64_t* ldc, float* const* S1, int max_ctas, cudaStream_t s) {
+  if (G < 1 || G > 12) return -6;
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  for (int g = 0; g < G; ++g) {
+    if ((lda[g] % 8) || (ldb[g] % 8) || (ldc[g] % 8) || (N % 8)) return -2;
+    if (((uintptr_t)A[g] | (uintptr_t)B[g] | (uintptr_t)out[g]) & 15) return -3;
+    if (lda[g] < K || ldb[g] < K || ldc[g] < N) return -5;
+    if (S1 && !S1[g]) return -4;
+  }
+  for (int g = 0; g < G; ++g) {
+    const void* mk = mask_src ? mask_src[g] : nullptr;
+    const int rc = dr_cuda_gemm_tn_ex(A[g], lda[g], B[g], ldb[g], M, N, K, bias ? bias[g] : nullptr, relu, mk, mk ? ld_mask[g] : 0, mk ? 1 : 0, out[g],
+                                      ldc[g], nullptr, S1 ? S1[g] : nullptr, nullptr, max_ctas, 0, s);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+int dr_cuda_gemm_dw_grouped(int G, const void* const* dY, const int64_t* ldy, const void* const* X, const int64_t* ldx, int batch, int N_out,
+                            int K_in, float* const* dW, const int64_t* ldw, int splits, cudaStream_t s) {
+  if (G < 1 || G > 12) return -6;
+  if (batch <= 0 || N_out <= 0 || K_in <= 0) return 0;
+  for (int g = 0; g < G; ++g) {
+    if ((ldy[g] % 8) || (ldx[g] % 8)) return -2;
+    if (((uintptr_t)dY[g] | (uintptr_t)X[g]) & 15) return -3;
+  }
+  for (int g = 0; g < G; ++g) {
+    const int rc = dr_cuda_gemm_dw(dY[g], ldy[g], X[g], ldx[g], batch, N_out, K_in, dW[g], ldw[g], splits, s);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
 // gemm_fp8.cu: the fp8 serving path is not emulated (ModelConfig {"fp8": true} fails to initialise on the emulation, loudly)
 int dr_cuda_gemm_fp8_tn(const void*, int64_t, const void*, int64_t, int, int, int, const float*, const float*, int, void*, int64_t, int, float, cudaStream_t) { return -100; }
 int dr_cuda_quantize_e4m3(const void*, int, int64_t, int, int64_t, void*, int, float, cudaStream_t) { return -100; }

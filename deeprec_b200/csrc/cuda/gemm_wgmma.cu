@@ -25,6 +25,7 @@
 #include <cuda.h>
 
 #include <algorithm>
+#include <cstring>
 #include <type_traits>
 
 #include "common.cuh"
@@ -821,6 +822,303 @@ int launch_tn_sel(const CUtensorMap& ta, const void* B, int M, int N, int K, int
   return launch_tn<BN, false, false, false>(ta, B, M, N, K, ldb, ep, max_ctas, s);
 }
 
+// -------------------------------------------------------------------------------------------------
+// Grouped GEMMs (expert MLPs: nn.fused_expert_mlps): G problems of one shape in one persistent launch.
+//   k_gemm_tn_grouped        out_g = A_g B_g^T (+bias_g)(ReLU)(* relu-mask_g)(S1_g column sums) over the tiles (g, m, n), g-major; a tile
+//                            runs the mainloop and the kind-0 epilogue of k_gemm_tn's cooperative consumers, so each group's output and
+//                            statistics are bit-identical to a dr_cuda_gemm_tn_ex call on that group.  The kernel is separate from
+//                            k_gemm_tn so that k_gemm_tn's instantiations stay exactly as they were.
+//   k_gemm_nt_splitk_grouped k_gemm_nt_splitk with blockIdx.z = g * splits + split, then k_dw_reduce_grouped (blockIdx.y = g) adds each
+//                            group's splits in order, as dr_cuda_gemm_dw does.
+// The per-group tensor maps are __grid_constant__ kernel parameters: no host-to-device copy per call and no tensormap fence, and a captured
+// CUDA graph holds them by value.  kMaxGroups is what fits the classic 4 KB parameter space: 12 x (2 x 128 B maps + 40 B of operands).
+// -------------------------------------------------------------------------------------------------
+constexpr int kMaxGroups = 12;
+
+struct GroupTN {
+  const float* bias;                  // [N] or null
+  const __nv_bfloat16* mask;          // aux tile (aux_mode 1) or null
+  __nv_bfloat16* out;
+  int64_t ldc, ld_mask;
+};
+struct GroupedTN {
+  CUtensorMap tmA[kMaxGroups];
+  CUtensorMap tmB[kMaxGroups];
+  GroupTN g[kMaxGroups];
+  float* stat_ws;                     // [m_tiles][G N]: the S1 partials of group g in columns [g N, g N + N) (or null)
+  int G, relu;
+};
+static_assert(sizeof(GroupedTN) + 3 * sizeof(int) <= 4096, "grouped GEMM parameters exceed the 4 KB kernel parameter space");
+
+template <int BLOCK_N>
+__global__ void __launch_bounds__(kGemmThreads, 1) k_gemm_tn_grouped(const __grid_constant__ GroupedTN p, int M, int N, int K) {
+  using L = SmemLayoutTN<BLOCK_N, false>;
+  constexpr int kSt = L::kSt;
+  constexpr int kAcc = BLOCK_N / 2;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* sS1 = reinterpret_cast<float*>(ring + kSt * L::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sS1) + L::kStatBytes);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + kSt;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
+  const int n_tiles = (N + BLOCK_N - 1) / BLOCK_N;
+  const int tiles = m_tiles * n_tiles;
+  const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
+  const int num_units = p.G * tiles;
+
+  if (threadIdx.x == 0) {
+    for (int g = 0; g < p.G; ++g) { tma_prefetch_desc(&p.tmA[g]); tma_prefetch_desc(&p.tmB[g]); }
+    for (int i = 0; i < kSt; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_sync();
+
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+        const int g = u / tiles, m_blk = (u % tiles) / n_tiles, n_blk = u % n_tiles;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = ring + stage * L::kStageBytes;
+          mbar_expect_tx(&full_bar[stage], L::kStageBytes);
+          tma_load_2d(sa, &p.tmA[g], &full_bar[stage], kb * BLOCK_K, m_blk * BLOCK_M);
+          tma_load_2d(sa + L::kABytes, &p.tmB[g], &full_bar[stage], kb * BLOCK_K, n_blk * BLOCK_N);
+          if (++stage == kSt) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    const int wg = (warp >> 2) - 1;
+    const int wl = warp & 3;
+    const int ct = threadIdx.x - 128;
+    int stage = 0; uint32_t phase = 0;
+    const bool stats = p.stat_ws != nullptr;
+    for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+      const int g = u / tiles, m_blk = (u % tiles) / n_tiles, n_blk = u % n_tiles;
+      float acc[kAcc];
+#pragma unroll
+      for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(ring + stage * L::kStageBytes) + wg * 64 * 128;
+        const uint32_t sb = smem_u32(ring + stage * L::kStageBytes) + L::kABytes;
+        const uint64_t adesc = gmma_desc_sw128(sa, 16, 1024);
+        const uint64_t bdesc = gmma_desc_sw128(sb, 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_bf16<BLOCK_N, 0, 0>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kSt) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      // ---- the kind-0 epilogue of k_gemm_tn: bias, ReLU, aux-mode-1 mask, S1 partials in the same order
+      const GroupTN& q = p.g[g];
+      const int row0 = m_blk * BLOCK_M + wg * 64 + wl * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int col = n_blk * BLOCK_N + 8 * j + 2 * (lane & 3);
+        const bool col_ok = col < N;
+        float b0 = 0.f, b1 = 0.f;
+        if (col_ok && q.bias) { b0 = __ldg(q.bias + col); b1 = __ldg(q.bias + col + 1); }
+        float p1[2] = {0.f, 0.f};
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          const bool ok = col_ok && row < M;
+          float v0 = acc[4 * j + 2 * h] + b0;
+          float v1 = acc[4 * j + 2 * h + 1] + b1;
+          if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          if (q.mask && ok) {
+            const __nv_bfloat16* ms = q.mask + (int64_t)row * q.ld_mask + col;
+            if (!(__bfloat162float(ms[0]) > 0.f)) v0 = 0.f;
+            if (!(__bfloat162float(ms[1]) > 0.f)) v1 = 0.f;
+          }
+          if (ok) {
+            *reinterpret_cast<uint32_t*>(q.out + (int64_t)row * q.ldc + col) = pack_bf16x2(v0, v1);
+            if (stats) { p1[0] += v0; p1[1] += v1; }
+          }
+        }
+        if (stats) {
+#pragma unroll
+          for (int c = 0; c < 2; ++c)
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) p1[c] += __shfl_xor_sync(0xffffffffu, p1[c], o);
+          if (lane < 4) {
+            float* r1 = sS1 + (warp - 4) * BLOCK_N + 8 * j + 2 * lane;
+            r1[0] = p1[0]; r1[1] = p1[1];
+          }
+        }
+      }
+      if (stats) {
+        consumer_bar_sync();
+        for (int i = ct; i < BLOCK_N; i += 256) {
+          const int col = n_blk * BLOCK_N + i;
+          if (col < N) {
+            float a1 = 0.f;
+#pragma unroll
+            for (int w = 0; w < 8; ++w) a1 += sS1[w * BLOCK_N + i];
+            p.stat_ws[(int64_t)m_blk * p.G * N + (int64_t)g * N + col] = a1;
+          }
+        }
+        consumer_bar_sync();
+      }
+    }
+  }
+}
+
+struct GroupedNT {
+  CUtensorMap tmA[kMaxGroups];
+  CUtensorMap tmB[kMaxGroups];
+};
+
+template <int BLOCK_N>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+k_gemm_nt_splitk_grouped(const __grid_constant__ GroupedNT p, int Mo, int No, int batch, int rows_per_split, int splits, float* __restrict__ part) {
+  using L = SmemLayoutNT<BLOCK_N>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * L::kStageBytes);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + kStages;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_blk = blockIdx.x, n_blk = blockIdx.y, g = blockIdx.z / splits, split = blockIdx.z % splits;
+  const CUtensorMap* tmA = &p.tmA[g];
+  const CUtensorMap* tmB = &p.tmB[g];
+  const int b0 = split * rows_per_split;
+  const int b1 = min(batch, b0 + rows_per_split);
+  const int num_kb = (b1 - b0 + BLOCK_KB - 1) / BLOCK_KB;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(tmA); tma_prefetch_desc(tmB);
+    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_sync();
+  if (num_kb <= 0) return;
+
+  if (warp == 0) {
+    if (lane == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sa = smem + stage * L::kStageBytes;
+        uint8_t* sb = sa + L::kAChunks * kChunkBytes;
+        mbar_expect_tx(&full_bar[stage], L::kStageBytes);
+        const int brow = b0 + kb * BLOCK_KB;
+#pragma unroll
+        for (int c = 0; c < L::kAChunks; ++c) tma_load_2d(sa + c * kChunkBytes, tmA, &full_bar[stage], m_blk * BLOCK_M + c * 64, brow);
+#pragma unroll
+        for (int c = 0; c < L::kBChunks; ++c) tma_load_2d(sb + c * kChunkBytes, tmB, &full_bar[stage], n_blk * BLOCK_N + c * 64, brow);
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else if (warp >= 4) {
+    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+    int stage = 0; uint32_t phase = 0, prev = 0;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * L::kStageBytes) + wg * kChunkBytes;
+      const uint32_t sb = smem_u32(smem + stage * L::kStageBytes) + L::kAChunks * kChunkBytes;
+      const uint64_t adesc = gmma_desc_sw128(sa, kChunkBytes, 1024);
+      const uint64_t bdesc = gmma_desc_sw128(sb, kChunkBytes, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BLOCK_KB / 16; ++k)
+        wgmma_bf16<BLOCK_N, 1, 1>(acc, adesc + (uint64_t)(k * 128), bdesc + (uint64_t)(k * 128), 1);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    float* gpart = part + (int64_t)g * splits * Mo * No;
+    const int row0 = m_blk * BLOCK_M + wg * 64 + wl * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      const int col = n_blk * BLOCK_N + 8 * j + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = row0 + 8 * h;
+        if (row >= Mo) continue;
+        float* dst = gpart + ((int64_t)split * Mo + row) * No + col;
+        if (col < No) dst[0] = acc[4 * j + 2 * h];
+        if (col + 1 < No) dst[1] = acc[4 * j + 2 * h + 1];
+      }
+    }
+  }
+}
+
+struct GroupedDW { float* dW[kMaxGroups]; int64_t ldw[kMaxGroups]; };
+
+// k_dw_reduce for group blockIdx.y: its splits added in order
+__global__ void k_dw_reduce_grouped(const float* __restrict__ part, int splits, int Mo, int No, const __grid_constant__ GroupedDW d) {
+  const int64_t n = (int64_t)Mo * No;
+  const int g = blockIdx.y;
+  const float* gp = part + (int64_t)g * splits * n;
+  float* dW = d.dW[g];
+  const int64_t ldw = d.ldw[g];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float sum = 0.f;
+    for (int k = 0; k < splits; ++k) sum += gp[k * n + i];
+    dW[(i / No) * ldw + i % No] += sum;
+  }
+}
+
+template <int BN>
+int launch_tn_grouped(const GroupedTN& p, int M, int N, int K, int max_ctas, cudaStream_t s) {
+  using L = SmemLayoutTN<BN, false>;
+  static DrPerDeviceOnce attr_once; bool& attr_set = attr_once();
+  if (!attr_set) {
+    DR_CUDA_CHECK(cudaFuncSetAttribute(k_gemm_tn_grouped<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
+    attr_set = true;
+  }
+  int grid = p.G * ((M + BLOCK_M - 1) / BLOCK_M) * ((N + BN - 1) / BN);
+  if (grid > max_ctas) grid = max_ctas;
+  DR_PDL_LAUNCH(k_gemm_tn_grouped<BN>, grid, kGemmThreads, L::kTotal, s, p, M, N, K);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
+template <int BN>
+int launch_nt_grouped(const GroupedNT& p, int G, int Mo, int No, int batch, int splits, const GroupedDW& d, cudaStream_t s) {
+  using L = SmemLayoutNT<BN>;
+  static DrPerDeviceOnce attr_once; bool& attr_set = attr_once();
+  if (!attr_set) {
+    DR_CUDA_CHECK(cudaFuncSetAttribute(k_gemm_nt_splitk_grouped<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
+    attr_set = true;
+  }
+  int rows_per_split = ((batch + splits - 1) / splits + BLOCK_KB - 1) / BLOCK_KB * BLOCK_KB;     // as launch_nt
+  splits = (batch + rows_per_split - 1) / rows_per_split;
+  float* part = dr_workspace(kWsGemmDw, (size_t)G * splits * Mo * No, s);
+  if (!part) return -5;
+  dim3 grid((Mo + BLOCK_M - 1) / BLOCK_M, (No + BN - 1) / BN, G * splits);
+  DR_PDL_LAUNCH((k_gemm_nt_splitk_grouped<BN>), grid, kGemmThreads, L::kTotal, s, p, Mo, No, batch, rows_per_split, splits, part);
+  DR_LAUNCH_CHECK();
+  const int64_t n = (int64_t)Mo * No;
+  k_dw_reduce_grouped<<<dim3((unsigned)std::min<int64_t>((n + 255) / 256, num_sms() * 8), G), 256, 0, s>>>(part, splits, Mo, No, d);
+  DR_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -954,6 +1252,84 @@ int dr_cuda_gemm_dw(const void* dY, int64_t ldy, const void* X, int64_t ldx, int
   const int n_tiles = (K_in + 127) / 128;
   if (splits <= 0) splits = max(1, num_sms() / (m_tiles * n_tiles));
   return launch_nt<128>(ta, tb, N_out, K_in, batch, splits, dW, ldw, s);
+}
+
+// G GEMMs of one shape in one launch (k_gemm_tn_grouped): out[g][M,N] = A[g][M,K](lda[g]) * B[g][N,K](ldb[g])^T (+bias[g])(relu)(*mask[g]).
+// The per-group arguments are host arrays of G entries; bias, mask_src (with ld_mask) and S1 may be null arrays, and bias[g] / mask_src[g]
+// null entries.  A non-null mask_src[g] is the ReLU-backward mask of dr_cuda_gemm_tn_ex's aux_mode 1; S1[g] (all non-null when S1 is given)
+// is accumulated into with the column sums of rows < M.  Each group's out and S1 are bit-identical to a dr_cuda_gemm_tn_ex call on it.
+// Codes:  -6  G outside [1, kMaxGroups];  then per group in order the codes of dr_cuda_gemm_tn_ex:  -2  lda, ldb, ldc or N not a multiple
+// of 8;  -3  A, B or out not 16-byte aligned;  -5  lda < K, ldb < K, ldc < N (or no workspace);  -4  S1 given with a null entry.
+int dr_cuda_gemm_tn_grouped(int G, const void* const* A, const int64_t* lda, const void* const* B, const int64_t* ldb, int M, int N, int K,
+                            const float* const* bias, int relu, const void* const* mask_src, const int64_t* ld_mask, void* const* out,
+                            const int64_t* ldc, float* const* S1, int max_ctas, cudaStream_t s) {
+  if (G < 1 || G > kMaxGroups) return -6;
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  for (int g = 0; g < G; ++g) {
+    if ((lda[g] % 8) || (ldb[g] % 8) || (ldc[g] % 8) || (N % 8)) return -2;
+    if (((uintptr_t)A[g] | (uintptr_t)B[g] | (uintptr_t)out[g]) & 15) return -3;
+    if (lda[g] < K || ldb[g] < K || ldc[g] < N) return -5;
+    if (S1 && !S1[g]) return -4;
+  }
+  if (max_ctas <= 0) max_ctas = num_sms();
+  const int BN = N <= 16 ? 16 : N <= 32 ? 32 : N <= 64 ? 64 : 128;      // the tile width dr_cuda_gemm_tn_ex picks
+  GroupedTN p;
+  memset(&p, 0, sizeof(p));
+  p.G = G; p.relu = relu;
+  for (int g = 0; g < G; ++g) {
+    int rc = make_tmap(&p.tmA[g], A[g], (uint64_t)K, (uint64_t)M, (uint64_t)lda[g] * 2, BLOCK_K, BLOCK_M);
+    if (rc) return rc;
+    rc = make_tmap(&p.tmB[g], B[g], (uint64_t)K, (uint64_t)N, (uint64_t)ldb[g] * 2, BLOCK_K, (uint32_t)BN);
+    if (rc) return rc;
+    p.g[g] = GroupTN{bias ? bias[g] : nullptr, mask_src ? (const __nv_bfloat16*)mask_src[g] : nullptr, (__nv_bfloat16*)out[g], ldc[g],
+                     mask_src ? ld_mask[g] : 0};
+  }
+  const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
+  if (S1) {
+    p.stat_ws = dr_workspace(kWsGemmStats, (size_t)m_tiles * G * N, s);
+    if (!p.stat_ws) return -5;
+  }
+  int rc = BN == 16 ? launch_tn_grouped<16>(p, M, N, K, max_ctas, s)
+         : BN == 32 ? launch_tn_grouped<32>(p, M, N, K, max_ctas, s)
+         : BN == 64 ? launch_tn_grouped<64>(p, M, N, K, max_ctas, s)
+                    : launch_tn_grouped<128>(p, M, N, K, max_ctas, s);
+  if (rc || !S1) return rc;
+  for (int g = 0; g < G; g += kDetColsumMaxRanges) {     // workspace row m_blk holds every group's tile sums: one range per group
+    DetColsumRange r[kDetColsumMaxRanges] = {};
+    for (int j = 0; j < kDetColsumMaxRanges && g + j < G; ++j) r[j] = DetColsumRange{(int64_t)(g + j) * N, N, S1[g + j]};
+    det_colsum(p.stat_ws, m_tiles, (int64_t)G * N, r, s);
+    DR_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
+// G weight gradients of one shape (k_gemm_nt_splitk_grouped): dW[g][N_out,K_in](ldw[g], fp32, accumulated into) += dY[g]^T * X[g], with
+// the split count and the in-order split sums of dr_cuda_gemm_dw, so each group's dW is bit-identical to a dr_cuda_gemm_dw call on it.
+// Codes:  -6  G outside [1, kMaxGroups];  -2  ldy or ldx not a multiple of 8;  -5  no workspace.
+int dr_cuda_gemm_dw_grouped(int G, const void* const* dY, const int64_t* ldy, const void* const* X, const int64_t* ldx, int batch, int N_out,
+                            int K_in, float* const* dW, const int64_t* ldw, int splits, cudaStream_t s) {
+  if (G < 1 || G > kMaxGroups) return -6;
+  if (batch <= 0 || N_out <= 0 || K_in <= 0) return 0;
+  for (int g = 0; g < G; ++g)
+    if ((ldy[g] % 8) || (ldx[g] % 8)) return -2;
+  GroupedNT p;
+  memset(&p, 0, sizeof(p));
+  GroupedDW d{};
+  for (int g = 0; g < G; ++g) {
+    int rc = make_tmap(&p.tmA[g], dY[g], (uint64_t)N_out, (uint64_t)batch, (uint64_t)ldy[g] * 2, 64, BLOCK_KB);
+    if (rc) return rc;
+    rc = make_tmap(&p.tmB[g], X[g], (uint64_t)K_in, (uint64_t)batch, (uint64_t)ldx[g] * 2, 64, BLOCK_KB);
+    if (rc) return rc;
+    d.dW[g] = dW[g]; d.ldw[g] = ldw[g];
+  }
+  const int m_tiles = (N_out + BLOCK_M - 1) / BLOCK_M;
+  if (K_in <= 64) {
+    if (splits <= 0) splits = max(1, num_sms() / m_tiles);
+    return launch_nt_grouped<64>(p, G, N_out, K_in, batch, splits, d, s);
+  }
+  const int n_tiles = (K_in + 127) / 128;
+  if (splits <= 0) splits = max(1, num_sms() / (m_tiles * n_tiles));
+  return launch_nt_grouped<128>(p, G, N_out, K_in, batch, splits, d, s);
 }
 
 // FP8 (E4M3) GEMM for the serving MLP:  out[M,N] = (A_q[M,K] B_q[N,K]^T) * col_scale[n] + bias[n]  (ReLU)

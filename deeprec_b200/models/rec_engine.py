@@ -336,8 +336,10 @@ def pooled_seq_engine(model, batch_size: int, max_len: int = 50, combiner: str =
     history: the id columns of :func:`din_ids` ([user | item | cat | hist_item x L | hist_cat x L]) pooled into five bags
     [user | item | cat | hist_item | hist_cat] with ``combiner`` (``sum`` is what the framework path's ``_embed_pooled`` computes; the reference
     pools these columns with ``mean``), so the dense net sees a [B, 5, D] activation.  Multi-task models train on labels [B, 2] (click, conversion:
-    :func:`taobao_engine_batch`) with the model's own ``multitask_loss``."""
-    from .zoo import DSSM, _MultiTask
+    :func:`taobao_engine_batch`) with the model's own ``multitask_loss``.  MMoE and PLE run their experts, gates and towers through
+    :data:`nn.FUSED_MOE` (grouped expert GEMMs and the fused softmax-gate mixture)."""
+    from ..nn import FUSED_MOE
+    from .zoo import DSSM, MMoE, PLE, _MultiTask
     L = max_len
     col_table = [0, 1, 2] + [1] * L + [2] * L
     bags = [(1, combiner), (1, combiner), (1, combiner), (L, combiner), (L, combiner)]
@@ -345,6 +347,7 @@ def pooled_seq_engine(model, batch_size: int, max_len: int = 50, combiner: str =
     if not multitask and not isinstance(model, DSSM):
         raise ValueError(f"pooled_seq_engine: {type(model).__name__} is neither DSSM nor a multi-task model")
     dense_net = _StripTables(model)
+    kw_tl = {"moe": FUSED_MOE} if isinstance(model, (MMoE, PLE)) else {}
 
     def fwd(net, dense, emb, ids):
         u = emb[:, 0]
@@ -352,7 +355,7 @@ def pooled_seq_engine(model, batch_size: int, max_len: int = 50, combiner: str =
         pooled = torch.cat([emb[:, 3], emb[:, 4]], -1)
         with torch.autocast(emb.device.type, dtype=torch.bfloat16):
             if multitask:
-                return net.inner.tower_logits(torch.cat([u, q, pooled], -1))
+                return net.inner.tower_logits(torch.cat([u, q, pooled], -1), **kw_tl)
             return net.inner.head(u, q, pooled)
     if multitask:
         kw.setdefault("loss_fn", lambda out, y: dense_net.inner.multitask_loss({k: v.float() for k, v in out.items()}, y[:, 0], y[:, 1]))

@@ -507,6 +507,14 @@ class ESMM(_MultiTask):
         return {"ctr": ctr, "cvr": cvr, "ctcvr": torch.log(p) - torch.log1p(-p)}
 
 
+def _moe_towers(towers, tasks, xs, moe):
+    """Logits of the same-shaped towers ``towers[t] = Sequential(mlp, Linear(H, 1))`` over inputs ``xs`` (task order): the MLPs as one
+    ``moe.expert_mlps`` call, the 1-wide output Linears in torch."""
+    h = moe.expert_mlps(list(xs), [towers[t][0] for t in tasks])
+    H = h.shape[1] // len(tasks)
+    return {t: towers[t][1](h[:, i * H:(i + 1) * H]).squeeze(-1) for i, t in enumerate(tasks)}
+
+
 class MMoE(_MultiTask):
     def __init__(self, num_experts: int = 3, expert_hidden_units=(256, 192, 128, 64), tower=(256, 192, 128, 64), **kw):
         super().__init__(name=kw.pop("name", "mmoe"), **kw)
@@ -515,9 +523,15 @@ class MMoE(_MultiTask):
         self.gates = nn.ModuleDict({t: nn.Linear(self.feat_dim, num_experts, device=dev) for t in self.tasks})
         self.towers = nn.ModuleDict({t: nn.Sequential(mlp(tower, expert_hidden_units[-1], device=dev), nn.Linear(tower[-1], 1, device=dev)) for t in self.tasks})
 
-    def tower_logits(self, f):
-        e = torch.stack([x(f) for x in self.experts], 1)
-        return {t: self.towers[t]((torch.softmax(self.gates[t](f), -1).unsqueeze(-1) * e).sum(1)).squeeze(-1) for t in self.tasks}
+    def tower_logits(self, f, moe=None):
+        """``moe``: the expert-mixture ops (``nn.FUSED_MOE``) to run the experts, gates and towers through; None: plain modules."""
+        if moe is None:
+            e = torch.stack([x(f) for x in self.experts], 1)
+            return {t: self.towers[t]((torch.softmax(self.gates[t](f), -1).unsqueeze(-1) * e).sum(1)).squeeze(-1) for t in self.tasks}
+        G = len(self.experts)
+        e = moe.expert_mlps(f, list(self.experts))
+        mix = moe.mix([f] * len(self.tasks), [self.gates[t] for t in self.tasks], e.view(e.shape[0], G, -1), [range(G)] * len(self.tasks))
+        return _moe_towers(self.towers, self.tasks, mix, moe)
 
 
 class DBMTL(_MultiTask):
@@ -556,7 +570,10 @@ class PLE(_MultiTask):
             d = expert_units[-1]
         self.towers = nn.ModuleDict({t: nn.Sequential(mlp(tower, d, device=dev), nn.Linear(tower[-1], 1, device=dev)) for t in self.tasks})
 
-    def tower_logits(self, f):
+    def tower_logits(self, f, moe=None):
+        """``moe``: the expert-mixture ops (``nn.FUSED_MOE``) to run the experts, gates and towers through; None: plain modules."""
+        if moe is not None:
+            return self._tower_logits_moe(f, moe)
         xs = {t: f for t in self.tasks}
         xs["shared"] = f
         for L in self.layers:
@@ -570,6 +587,27 @@ class PLE(_MultiTask):
             nxt["shared"] = (torch.softmax(L["gate_shared"](xs["shared"]), -1).unsqueeze(-1) * allx).sum(1)
             xs = nxt
         return {t: self.towers[t](xs[t]).squeeze(-1) for t in self.tasks}
+
+    def _tower_logits_moe(self, f, moe):
+        """Each level's experts as one ``moe.expert_mlps`` call (packed [task 0's specific | task 1's ... | shared]; level 0 over the shared input f)
+        and its gates as one ``moe.mix``.  The last level's shared gate feeds nothing, so it is not run: its parameters get no gradient here, as
+        on the plain path."""
+        T = list(self.tasks)
+        xs = {t: f for t in T}
+        xs["shared"] = f
+        for li, L in enumerate(self.layers):
+            ns = len(L[f"spec_{T[0]}"])
+            mlps = [e for t in T for e in L[f"spec_{t}"]] + list(L["shared"])
+            ins = [xs[t] for t in T for _ in range(ns)] + [xs["shared"]] * len(L["shared"])
+            G = len(mlps)
+            e = moe.expert_mlps(f if li == 0 else ins, mlps)
+            shared = list(range(len(T) * ns, G))
+            keys, gates = list(T), [L[f"gate_{t}"] for t in T]
+            select = [list(range(i * ns, (i + 1) * ns)) + shared for i in range(len(T))]
+            if li + 1 < len(self.layers):
+                keys.append("shared"); gates.append(L["gate_shared"]); select.append(list(range(G)))
+            xs = dict(zip(keys, moe.mix([xs[k] for k in keys], gates, e.view(e.shape[0], G, -1), select)))
+        return _moe_towers(self.towers, T, [xs[t] for t in T], moe)
 
 
 class SimpleMultiTask(_MultiTask):

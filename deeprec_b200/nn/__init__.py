@@ -1,4 +1,6 @@
 """nn layers on the hand-written sm_90a kernels (see layers.py)."""
-from .layers import FusedLinear, FusedMaskBlock, FusedMLP, dot_interaction, fm_interaction, fused_encoder_layer, fused_gru
+from .layers import (FUSED_MOE, FusedLinear, FusedMaskBlock, FusedMLP, MoEOps, dot_interaction, fm_interaction, fused_encoder_layer, fused_expert_mlps,
+                     fused_gru, fused_moe_mix)
 
-__all__ = ["FusedLinear", "FusedMaskBlock", "FusedMLP", "dot_interaction", "fm_interaction", "fused_encoder_layer", "fused_gru"]
+__all__ = ["FUSED_MOE", "FusedLinear", "FusedMaskBlock", "FusedMLP", "MoEOps", "dot_interaction", "fm_interaction", "fused_encoder_layer",
+           "fused_expert_mlps", "fused_gru", "fused_moe_mix"]

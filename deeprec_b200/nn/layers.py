@@ -13,13 +13,16 @@
     the wgmma GEMM, the multi-head self-attention core forward and backward on csrc/cuda/mha_kernels.cu.
   * ``FusedMaskBlock``: MaskNet's MaskBlock as one autograd node -- the mask MLP's GEMMs with their BatchNorm statistics in the epilogue,
     the last BatchNorm fused with the instance-guided product, and the block's Linear with LayerNorm + ReLU in the GEMM epilogue.
+  * ``fused_expert_mlps`` / ``fused_moe_mix`` (``FUSED_MOE``): MMoE's and PLE's same-shaped expert and tower MLPs as grouped wgmma GEMMs, and a
+    mixture layer's softmax gates as one kernel (csrc/cuda/moe_kernels.cu).
 
 The reference runs these through cuBLAS (stream_executor/cuda/cuda_blas.cc) and ~10 TF ops per interaction
 (modelzoo/dlrm/train.py:163-236, modelzoo/deepfm/train.py:178-187).  CPU tensors fall back to the equivalent torch expression.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Sequence
+import ctypes as C
+from typing import Callable, List, NamedTuple, Optional, Sequence
 
 import torch
 from torch import nn
@@ -560,3 +563,275 @@ class FusedMaskBlock(nn.Module):
         m = _bn_tf(torch.relu(self.fc1(v_emb)), self.bn1)
         m = _bn_tf(torch.relu(self.fc2(m)), self.bn2)
         return torch.relu(self.ln(self.fc3(m * v_hidden)))
+
+
+# ---- expert mixtures (MMoE, PLE) ---------------------------------------------------------------------------------------------
+GEMM_MAX_GROUPS = 12                  # kMaxGroups of csrc/cuda/gemm_wgmma.cu: groups one grouped-GEMM launch takes (more are split)
+MOE_MAX_GATES, MOE_MAX_EXPERTS, MOE_MAX_H = 8, 32, 512   # limits of one csrc/cuda/moe_kernels.cu launch
+
+
+def _fused_nn(t: torch.Tensor) -> bool:
+    import os
+    return _native.on_device(t) and os.environ.get("DEEPREC_FUSED_NN", "1") != "0"
+
+
+def _ptrs(vals):
+    return (C.c_void_p * len(vals))(*[v.value if isinstance(v, C.c_void_p) else v for v in vals])
+
+
+def _i64s(vals):
+    return (C.c_int64 * len(vals))(*vals)
+
+
+def _ints(vals):
+    return (C.c_int * len(vals))(*vals)
+
+
+def _gemm_tn_grouped(A, lda, B, ldb, M: int, N: int, K: int, out, ldc, bias=None, relu: int = 0, mask=None, ld_mask=None, S1=None) -> None:
+    """dr_cuda_gemm_tn_grouped over per-group lists (raw pointers / pitches), GEMM_MAX_GROUPS groups per launch."""
+    lib, s = _native.cuda(), stream_ptr()
+    for i in range(0, len(A), GEMM_MAX_GROUPS):
+        j = slice(i, i + GEMM_MAX_GROUPS)
+        check(lib.dr_cuda_gemm_tn_grouped(len(A[j]), _ptrs(A[j]), _i64s(lda[j]), _ptrs(B[j]), _i64s(ldb[j]), M, N, K,
+                                          _ptrs(bias[j]) if bias else None, relu, _ptrs(mask[j]) if mask else None,
+                                          _i64s(ld_mask[j]) if mask else None, _ptrs(out[j]), _i64s(ldc[j]), _ptrs(S1[j]) if S1 else None, 0, s),
+              "gemm_tn_grouped")
+
+
+def _gemm_dw_grouped(dY, ldy, X, ldx, batch: int, N_out: int, K_in: int, dW, ldw) -> None:
+    """dr_cuda_gemm_dw_grouped over per-group lists, GEMM_MAX_GROUPS groups per launch."""
+    lib, s = _native.cuda(), stream_ptr()
+    for i in range(0, len(dY), GEMM_MAX_GROUPS):
+        j = slice(i, i + GEMM_MAX_GROUPS)
+        check(lib.dr_cuda_gemm_dw_grouped(len(dY[j]), _ptrs(dY[j]), _i64s(ldy[j]), _ptrs(X[j]), _i64s(ldx[j]), batch, N_out, K_in, _ptrs(dW[j]),
+                                          _i64s(ldw[j]), 0, s), "gemm_dw_grouped")
+
+
+def _addr(t: torch.Tensor, elems: int = 0) -> int:
+    """address of element ``elems`` of t's storage (a column offset into a packed row-major buffer)"""
+    return t.data_ptr() + elems * t.element_size()
+
+
+def _mlp_layers(m: nn.Module):
+    """(weights, biases, last_act) of a ReLU MLP as :func:`models.zoo.mlp` builds it: a ``FusedMLP``, or an ``nn.Sequential`` of Linear / ReLU."""
+    if isinstance(m, FusedMLP):
+        if m.biases is None:
+            raise ValueError("fused_expert_mlps: needs MLPs with biases")
+        return list(m.weights), list(m.biases), m.last_act
+    if isinstance(m, nn.Sequential):
+        ws, bs, acts = [], [], []
+        for mod in m:
+            if isinstance(mod, nn.Linear) and mod.bias is not None:
+                ws.append(mod.weight); bs.append(mod.bias); acts.append(False)
+            elif isinstance(mod, nn.ReLU) and acts and not acts[-1]:
+                acts[-1] = True
+            else:
+                raise ValueError(f"fused_expert_mlps: {type(mod).__name__} in an expert MLP (Linear with bias / ReLU only)")
+        if ws and all(acts[:-1]):
+            return ws, bs, acts[-1]
+    raise ValueError(f"fused_expert_mlps: {type(m).__name__} is not a Linear + ReLU chain")
+
+
+class _FusedExpertsFn(torch.autograd.Function):
+    """G same-shaped MLPs -> their outputs packed side by side [M, G Np_last] (bf16); ``args`` = the inputs (one shared or G), then W, b of every
+    layer of group 0, group 1, ...  Widths are zero padded to multiples of 8; group g's layer-l activation is columns [g Np, g Np + Np) of one
+    [M, G Np] buffer.  Layer 1 over a shared input is one GEMM over the row-concatenated weights (and its dX one GEMM with K = G Np, so the
+    groups' input gradients add up in the accumulator); every other layer is a grouped GEMM, forward, dX (the ReLU mask and the bias gradient
+    of the layer below in its epilogue) and dW."""
+
+    @staticmethod
+    def forward(ctx, nx: int, G: int, nl: int, last_act: bool, *args):
+        lib, s = _native.cuda(), stream_ptr()
+        xs, params = args[:nx], args[nx:]
+        shared = nx == 1
+        M, K0 = xs[0].shape
+        dev = xs[0].device
+        bf = dict(dtype=torch.bfloat16, device=dev)
+        xin = [_to_bf16_padded(x, _pad8(K0)) for x in xs]
+        acts: List[torch.Tensor] = []
+        wts: List[torch.Tensor] = []
+        dims = []
+        for l in range(nl):
+            N, K = params[2 * l].shape
+            Np, Kp = _pad8(N), _pad8(K)
+            Ws = [params[2 * (g * nl + l)] for g in range(G)]
+            bias = torch.cat([F.pad(params[2 * (g * nl + l) + 1].detach().float(), (0, Np - N)) for g in range(G)])
+            relu = int(l + 1 < nl or last_act)
+            out = torch.empty(M, G * Np, **bf)
+            if l == 0 and shared:
+                Wcat = torch.cat([F.pad(W.detach().float(), (0, Kp - K, 0, Np - N)) for W in Ws])
+                wb, wt = _pack_weight(Wcat, G * Np, Kp)
+                check(lib.dr_cuda_gemm_tn_ex(ptr(xin[0]), Kp, ptr(wb), Kp, M, G * Np, Kp, ptr(bias), relu, None, 0, 0, ptr(out), G * Np, None, None, None,
+                                             0, 0, s), "gemm_tn")
+            else:
+                packs = [_pack_weight(W, Np, Kp) for W in Ws]
+                wt = torch.stack([p[1] for p in packs])                              # [G, Kp, Np]: the dX B operands
+                A = [_addr(xin[g]) for g in range(G)] if l == 0 else [_addr(acts[-1], g * Kp) for g in range(G)]
+                _gemm_tn_grouped(A, [Kp if l == 0 else G * Kp] * G, [_addr(p[0]) for p in packs], [Kp] * G, M, Np, Kp,
+                                 [_addr(out, g * Np) for g in range(G)], [G * Np] * G, bias=[_addr(bias, g * Np) for g in range(G)], relu=relu)
+            acts.append(out); wts.append(wt); dims.append((N, K, Np, Kp))
+        ctx.save_for_backward(*xin, *acts, *wts)
+        ctx.meta = (nx, G, nl, last_act, dims, [x.dtype for x in xs], K0)
+        return acts[-1].to(xs[0].dtype)
+
+    @staticmethod
+    def backward(ctx, gy):
+        lib, s = _native.cuda(), stream_ptr()
+        nx, G, nl, last_act, dims, xdt, K0 = ctx.meta
+        saved = ctx.saved_tensors
+        xin, acts, wts = saved[:nx], saved[nx: nx + nl], saved[nx + nl:]
+        shared = nx == 1
+        dev = gy.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        bf = dict(dtype=torch.bfloat16, device=dev)
+        M = gy.shape[0]
+        Np = dims[-1][2]
+        g = gy.to(torch.bfloat16).contiguous()
+        db = torch.zeros(G * Np, **f32)
+        if last_act:
+            one, zero = _const_vec(dev, G * Np, 1.0), _const_vec(dev, G * Np, 0.0)
+            da = torch.empty(M, G * Np, **bf)
+            check(lib.dr_cuda_bn_bwd_apply_v2(ptr(g), ptr(acts[-1]), M, G * Np, G * Np, ptr(one), ptr(zero), ptr(zero), ptr(zero), ptr(zero), ptr(da), 1,
+                                              ptr(db), s), "relu_bwd")
+        else:
+            da = g
+            check(lib.dr_cuda_colstats(ptr(da), None, M, G * Np, G * Np, G * Np, ptr(db), None, s), "colstats")
+        need_dx = any(ctx.needs_input_grad[4: 4 + nx])
+        grads: List[Optional[torch.Tensor]] = [None] * (2 * G * nl)
+        dxs: List[Optional[torch.Tensor]] = [None] * nx
+        for l in range(nl - 1, -1, -1):
+            N, K, Np, Kp = dims[l]
+            dY = [_addr(da, gi * Np) for gi in range(G)]
+            if l == 0 and shared:
+                dW = torch.zeros(G * Np, Kp, **f32)
+                check(lib.dr_cuda_gemm_dw(ptr(da), G * Np, ptr(xin[0]), Kp, M, G * Np, Kp, ptr(dW), Kp, 0, s), "gemm_dw")
+                dW = dW.view(G, Np, Kp)
+            else:
+                dW = torch.zeros(G, Np, Kp, **f32)
+                X = [_addr(xin[gi]) for gi in range(G)] if l == 0 else [_addr(acts[l - 1], gi * Kp) for gi in range(G)]
+                _gemm_dw_grouped(dY, [G * Np] * G, X, [Kp if l == 0 else G * Kp] * G, M, Np, Kp, [_addr(dW[gi]) for gi in range(G)], [Kp] * G)
+            for gi in range(G):
+                grads[2 * (gi * nl + l)] = dW[gi, :N, :K]
+                grads[2 * (gi * nl + l) + 1] = db[gi * Np: gi * Np + N]
+            if l > 0:
+                prev = torch.empty(M, G * Kp, **bf)
+                db = torch.zeros(G * Kp, **f32)
+                _gemm_tn_grouped(dY, [G * Np] * G, [_addr(wts[l][gi]) for gi in range(G)], [Np] * G, M, Kp, Np, [_addr(prev, gi * Kp) for gi in range(G)],
+                                 [G * Kp] * G, mask=[_addr(acts[l - 1], gi * Kp) for gi in range(G)], ld_mask=[G * Kp] * G,
+                                 S1=[_addr(db, gi * Kp) for gi in range(G)])
+                da = prev
+            elif need_dx and shared:
+                dx = torch.empty(M, Kp, **bf)
+                check(lib.dr_cuda_gemm_tn_ex(ptr(da), G * Np, ptr(wts[0]), G * Np, M, Kp, G * Np, None, 0, None, 0, 0, ptr(dx), Kp, None, None, None, 0, 0, s),
+                      "gemm_dx")
+                dxs[0] = dx[:, :K0].to(xdt[0])
+            elif need_dx:
+                dx = torch.empty(M, G * Kp, **bf)
+                _gemm_tn_grouped(dY, [G * Np] * G, [_addr(wts[0][gi]) for gi in range(G)], [Np] * G, M, Kp, Np, [_addr(dx, gi * Kp) for gi in range(G)],
+                                 [G * Kp] * G)
+                dxs = [dx[:, gi * Kp: gi * Kp + K0].to(xdt[gi]) for gi in range(G)]
+        return (None, None, None, None, *dxs, *grads)
+
+
+def fused_expert_mlps(x, mlps: Sequence[nn.Module]) -> torch.Tensor:
+    """Runs G same-shaped ReLU MLPs (``models.zoo.mlp``: a ``FusedMLP``, or the ``nn.Sequential`` of Linear / ReLU it builds off the GPU) over one
+    shared input ``x`` [M, K] or over one input each (``x`` a list of G [M, K] tensors), and returns their outputs side by side: [M, G H], group g
+    in columns [g H, g H + H).  Trains the modules' own parameters, so state dicts, checkpoints and the op-program export are unchanged.
+
+    On CUDA (and on the kernel emulation), unless ``DEEPREC_FUSED_NN=0``: one autograd node (bf16 activations, output in ``x``'s dtype).  A shared input's first layer is one
+    GEMM over the row-concatenated weights; every other layer runs the G groups as one grouped wgmma GEMM (csrc/cuda/gemm_wgmma.cu), forward
+    and backward, with fp32 weight gradients.  H must be a multiple of 8 there.  Otherwise the modules themselves, concatenated."""
+    xs = list(x) if isinstance(x, (list, tuple)) else [x]
+    if len(xs) not in (1, len(mlps)):
+        raise ValueError(f"fused_expert_mlps: {len(xs)} inputs for {len(mlps)} MLPs (one shared input, or one each)")
+    if not _fused_nn(xs[0]):
+        return torch.cat([m(xs[0] if len(xs) == 1 else xi) for m, xi in zip(mlps, xs * len(mlps) if len(xs) == 1 else xs)], -1)
+    layers = [_mlp_layers(m) for m in mlps]
+    shapes = [[tuple(w.shape) for w in ws] for ws, _, _ in layers]
+    if any(sh != shapes[0] for sh in shapes) or any(la != layers[0][2] for _, _, la in layers):
+        raise ValueError("fused_expert_mlps: the MLPs differ in shape or in their last activation")
+    H = shapes[0][-1][0]
+    if H % 8:
+        raise ValueError(f"fused_expert_mlps: output width {H} is not a multiple of 8")
+    params = [t for ws, bs, _ in layers for w, b in zip(ws, bs) for t in (w, b)]
+    return _FusedExpertsFn.apply(len(xs), len(mlps), len(shapes[0]), layers[0][2], *[xi.reshape(-1, xi.shape[-1]) for xi in xs], *params)
+
+
+class _MoEMixFn(torch.autograd.Function):
+    """mix_t = sum_e softmax(x_t W_t^T + b_t)_e X[:, sel_t[e]] for the T gates of one mixture layer on csrc/cuda/moe_kernels.cu; ``args`` = the
+    gate inputs, weights and biases (T each).  X: the packed experts [M, E_total H] (bf16)."""
+
+    @staticmethod
+    def forward(ctx, T: int, E_total: int, H: int, sel, X, *args):
+        lib, s = _native.cuda(), stream_ptr()
+        xs = [x.to(torch.bfloat16).contiguous() for x in args[:T]]
+        Ws = [w.detach().float().contiguous() for w in args[T: 2 * T]]
+        bs = [b.detach().float().contiguous() for b in args[2 * T:]]
+        M, dev = X.shape[0], X.device
+        mix = [torch.empty(M, H, dtype=torch.bfloat16, device=dev) for _ in range(T)]
+        g = [torch.empty(M, len(sl), dtype=torch.float32, device=dev) for sl in sel]
+        sel_a = _ints([i for sl in sel for i in list(sl) + [0] * (MOE_MAX_EXPERTS - len(sl))])
+        check(lib.dr_cuda_moe_mix_fwd(ptr(X), X.shape[1], M, E_total, H, T, _ptrs([x.data_ptr() for x in xs]), _i64s([x.shape[1] for x in xs]),
+                                      _ints([x.shape[1] for x in xs]), _ints([len(sl) for sl in sel]), _ptrs([w.data_ptr() for w in Ws]),
+                                      _ptrs([b.data_ptr() for b in bs]), sel_a, _ptrs([m.data_ptr() for m in mix]), _i64s([H] * T),
+                                      _ptrs([t.data_ptr() for t in g]), s), "moe_mix_fwd")
+        ctx.save_for_backward(X, *xs, *Ws, *g)
+        ctx.meta = (T, E_total, H, sel, [x.dtype for x in args[:T]])
+        return tuple(m.to(x.dtype) for m, x in zip(mix, args[:T]))
+
+    @staticmethod
+    def backward(ctx, *dmix):
+        lib, s = _native.cuda(), stream_ptr()
+        T, E_total, H, sel, xdt = ctx.meta
+        saved = ctx.saved_tensors
+        X, xs, Ws, g = saved[0], saved[1: 1 + T], saved[1 + T: 1 + 2 * T], saved[1 + 2 * T:]
+        M, dev = X.shape[0], X.device
+        dm = [d.to(torch.bfloat16).contiguous() if d is not None else torch.zeros(M, H, dtype=torch.bfloat16, device=dev) for d in dmix]
+        dX = torch.empty(M, E_total * H, dtype=torch.bfloat16, device=dev)
+        need = [ctx.needs_input_grad[5 + t] for t in range(T)]
+        dx = [torch.empty(M, x.shape[1], dtype=torch.bfloat16, device=dev) if n else None for x, n in zip(xs, need)]
+        dWb = [torch.zeros(w.numel() + w.shape[0], dtype=torch.float32, device=dev) for w in Ws]
+        sel_a = _ints([i for sl in sel for i in list(sl) + [0] * (MOE_MAX_EXPERTS - len(sl))])
+        check(lib.dr_cuda_moe_mix_bwd(ptr(X), X.shape[1], M, E_total, H, T, _ptrs([x.data_ptr() for x in xs]), _i64s([x.shape[1] for x in xs]),
+                                      _ints([x.shape[1] for x in xs]), _ints([len(sl) for sl in sel]), _ptrs([w.data_ptr() for w in Ws]), sel_a,
+                                      _ptrs([t.data_ptr() for t in g]), _ptrs([d.data_ptr() for d in dm]), _i64s([H] * T), ptr(dX), E_total * H,
+                                      _ptrs([d.data_ptr() if d is not None else 0 for d in dx]), _i64s([x.shape[1] for x in xs]),
+                                      _ptrs([d.data_ptr() for d in dWb]), s), "moe_mix_bwd")
+        dxs = [d.to(dt) if d is not None else None for d, dt in zip(dx, xdt)]
+        dWs = [d[: w.numel()].view_as(w) for d, w in zip(dWb, Ws)]
+        dbs = [d[w.numel():] for d, w in zip(dWb, Ws)]
+        return (None, None, None, None, dX, *dxs, *dWs, *dbs)
+
+
+def fused_moe_mix(xs: Sequence[torch.Tensor], gates: Sequence[nn.Linear], experts: torch.Tensor, select: Sequence[Sequence[int]]) -> List[torch.Tensor]:
+    """One mixture layer of MMoE / PLE: for every gate t, ``softmax(gates[t](xs[t])) . experts[:, select[t]]`` -> [M, H], where ``experts`` is
+    [M, E, H] (expert e's output in ``experts[:, e]``, e.g. a view of :func:`fused_expert_mlps`' packed output) and ``select[t]`` the experts
+    gate t mixes, in the order of its logits.
+
+    On CUDA (and on the kernel emulation), unless ``DEEPREC_FUSED_NN=0``: one autograd node on csrc/cuda/moe_kernels.cu -- fp32 logits and
+    softmax from bf16 inputs and the fp32 gate weights, a bf16 mix (returned in ``xs[t]``'s dtype); the backward sums each expert's gradient over the gates that read it in gate
+    order, with no atomics.  At most MOE_MAX_GATES gates, MOE_MAX_EXPERTS experts, H a multiple of 8 up to MOE_MAX_H.  Otherwise the same
+    expression in torch ops, which is the oracle."""
+    if len(xs) != len(gates) or len(gates) != len(select):
+        raise ValueError("fused_moe_mix: xs, gates and select differ in length")
+    M, E_total, H = experts.shape
+    if not _fused_nn(experts):
+        return [(torch.softmax(gate(x), -1).unsqueeze(-1) * experts[:, list(sl)]).sum(1) for x, gate, sl in zip(xs, gates, select)]
+    T = len(gates)
+    if T > MOE_MAX_GATES or E_total > MOE_MAX_EXPERTS or H % 8 or H > MOE_MAX_H or any(not 1 <= len(sl) <= MOE_MAX_EXPERTS for sl in select):
+        raise ValueError(f"fused_moe_mix: {T} gates over {E_total} experts of width {H} is not supported on CUDA (at most {MOE_MAX_GATES} gates and "
+                         f"{MOE_MAX_EXPERTS} experts, H a multiple of 8 up to {MOE_MAX_H})")
+    if any(g.bias is None for g in gates):
+        raise ValueError("fused_moe_mix: needs gates with biases")
+    X = experts.reshape(M, E_total * H).to(torch.bfloat16).contiguous()
+    sel = tuple(tuple(int(i) for i in sl) for sl in select)
+    return list(_MoEMixFn.apply(T, E_total, H, sel, X, *[x.reshape(M, -1) for x in xs], *[g.weight for g in gates], *[g.bias for g in gates]))
+
+
+class MoEOps(NamedTuple):
+    """The expert-mixture ops a model's ``tower_logits(f, moe=...)`` runs its experts, gates and towers through."""
+    expert_mlps: Callable
+    mix: Callable
+
+
+FUSED_MOE = MoEOps(fused_expert_mlps, fused_moe_mix)
