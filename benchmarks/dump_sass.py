@@ -15,6 +15,7 @@ WANT = {  # object file -> kernel-name substrings to dump in full
     "fused_interaction_gemm.cu.o": ["k_dlrm_inter_gemm"],
     "interaction_kernels.cu.o": ["k_dot_fwd_tcILb1", "k_dot_bwd_tcILb1"],
     "mha_kernels.cu.o": ["k_mha_fwdILi8ELi64", "k_mha_bwdILi8ELi64"],
+    "din_att_kernels.cu.o": ["k_din_att_fwdILi32E13__nv_bfloat16", "k_din_att_bwdILi32E13__nv_bfloat16", "k_din_att_bwdILi32EfE"],
     "gemm_wgmma.cu.o": ["k_gemm_tnILi128ELb0ELb0ELb0ELb0", "k_gemm_tnILi128ELb0ELb1ELb0ELb0", "k_gemm_tnILi64ELb0ELb0ELb1ELb1",
                         "k_gemm_nt_splitkILi128"],
     "tier_kernels.cu.o": ["k_tier_miss_list", "k_tier_evict"],

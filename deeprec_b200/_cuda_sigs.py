@@ -133,6 +133,8 @@ _sig("dr_cuda_gru_fwd", [P, P, P, P, INT, INT, INT, P, S])
 _sig("dr_cuda_gru_bwd", [P, P, P, P, P, P, INT, INT, INT, P, P, P, P, P, S])
 _sig("dr_cuda_mha_fwd", [P, P, INT, INT, INT, INT, P, S])
 _sig("dr_cuda_mha_bwd", [P, P, P, P, INT, INT, INT, INT, P, S])
+_sig("dr_cuda_din_att_fwd", [P, P, INT, P, INT, INT, INT, P, P, INT, P, P, INT, P, INT, P, S])
+_sig("dr_cuda_din_att_bwd", [P, P, INT, P, P, INT, INT, INT, P, P, INT, P, P, INT, P, INT, P, P, P, P, P, P, P, P, P, S])
 _sig("dr_cuda_din_attention_fwd", [P, P, P, i64, INT, INT, P, P, INT, P, P, INT, P, f32, P, S])
 _sig("dr_cuda_din_attention_bwd", [P, P, P, P, i64, INT, INT, P, P, INT, P, P, INT, P, f32, P, P, P, P, P, P, P, P, S])
 _sig("dr_cuda_layer_norm_fwd", [P, i64, INT, P, P, f32, P, P, P, S])

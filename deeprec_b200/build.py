@@ -42,6 +42,7 @@ CUDA_SOURCES = [
     "cuda/moe_kernels.cu",
     "cuda/rnn_kernels.cu",              # tensor-core GRU recurrence (mma.sync): hardware only, not in EMU_SOURCES
     "cuda/mha_kernels.cu",              # tensor-core multi-head self-attention (mma.sync): hardware only, not in EMU_SOURCES
+    "cuda/din_att_kernels.cu",          # tensor-core DIN attention unit for training (mma.sync): hardware only, not in EMU_SOURCES
     "cuda/sm_partition.cu",             # green-context SM partition (driver API): hardware only, not in EMU_SOURCES
 ]
 

@@ -277,7 +277,7 @@ inline float* dr_workspace(int slot, size_t nfloat, cudaStream_t s) {
   w.cap = n;
   return p;
 }
-enum { kWsGemmStats = 0, kWsGemmDw = 1, kWsColstats = 2, kWsHead = 3, kWsBnBwd = 4, kWsCross = 5, kWsLnBwd = 6, kWsBnMul = 7, kWsMoe = 8 };
+enum { kWsGemmStats = 0, kWsGemmDw = 1, kWsColstats = 2, kWsHead = 3, kWsBnBwd = 4, kWsCross = 5, kWsLnBwd = 6, kWsBnMul = 7, kWsMoe = 8, kWsDinAtt = 9 };
 
 // k_det_colsum: for every column c of a range, dst[c] += s with s = ((0.f + ws[0][c]) + ws[1][c]) + ... + ws[rows-1][c], one fp32 add after
 // the other in row order, so the result does not depend on this kernel's grid.  What makes it fast is memory parallelism alone: a block owns

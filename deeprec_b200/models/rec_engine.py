@@ -304,13 +304,15 @@ def din_engine(model, batch_size: int, max_len: int = 50, table_rows: Sequence[i
     hist_cat x L] over the three tables (user, item, cat); the history positions are columns of the item / category tables, padding (-1) gives
     zero rows and the attention mask.  DIEN's two GRUs run on :func:`nn.fused_gru`, which stops each sample after ``mask.sum(1)`` steps: its
     padding must be a tail (every id after the first -1 of a history is -1 too), as :func:`din_ids` of the project's Taobao-shaped batches
-    gives.  BST's encoder block runs on :func:`nn.fused_encoder_layer` with the key mask [history mask | True]; its padding may sit anywhere."""
-    from ..nn import fused_encoder_layer, fused_gru
-    from .zoo import BST, DIEN
+    gives.  BST's encoder block runs on :func:`nn.fused_encoder_layer` with the key mask [history mask | True]; its padding may sit anywhere.
+    DIN's and DIEN's attention units run on :func:`nn.fused_din_attention`."""
+    from ..nn import fused_din_attention, fused_encoder_layer, fused_gru
+    from .zoo import BST, DIEN, DIN
     L = max_len
     col_table = [0, 1, 2] + [1] * L + [2] * L
     dense_net = _StripTables(model)
-    kw_head = {"gru": fused_gru} if isinstance(model, DIEN) else {"encoder": fused_encoder_layer} if isinstance(model, BST) else {}
+    kw_head = ({"gru": fused_gru, "attention": fused_din_attention} if isinstance(model, DIEN) else {"encoder": fused_encoder_layer}
+               if isinstance(model, BST) else {"attention": fused_din_attention} if isinstance(model, DIN) else {})
 
     def fwd(net, dense, emb, ids):
         u = emb[:, 0]

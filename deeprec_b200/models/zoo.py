@@ -364,11 +364,12 @@ class DIN(_SeqBase):
         self.top = nn.Sequential(nn.Linear(self.emb_dim + 3 * D2, 200, device=dev), nn.PReLU(device=dev), nn.Linear(200, 80, device=dev), nn.PReLU(device=dev),
                                  nn.Linear(80, 1, device=dev))
 
-    def head(self, u, q, k, mask):
+    def head(self, u, q, k, mask, attention=None):
         """Dense part on already-looked-up embeddings (user [B, D], target [B, 2D], history [B, L, 2D] zero-padded, mask [B, L]) --
-        what :func:`models.rec_engine.din_engine` runs on top of the unique-first sparse pipeline."""
+        what :func:`models.rec_engine.din_engine` runs on top of the unique-first sparse pipeline.  ``attention=None`` runs the unit through
+        :func:`din_attention`; otherwise ``attention(q, k, mask, self.att)`` (:func:`nn.fused_din_attention`, what the engine passes)."""
         pooled = k.sum(1)
-        att = din_attention(q, k, mask, self.att)
+        att = din_attention(q, k, mask, self.att) if attention is None else attention(q, k, mask, self.att)
         return self.top(self.bn(torch.cat([u, q, pooled, att], -1))).squeeze(-1)
 
     def forward(self, b):
@@ -388,19 +389,24 @@ class DIEN(_SeqBase):
         self.top = nn.Sequential(nn.Linear(self.emb_dim + D2 + hidden + D2, 200, device=dev), nn.PReLU(device=dev), nn.Linear(200, 80, device=dev), nn.PReLU(device=dev),
                                  nn.Linear(80, 1, device=dev))
 
-    def head(self, u, q, k, mask, gru=None):
+    def head(self, u, q, k, mask, gru=None, attention=None):
         """Dense part on already-looked-up embeddings (user [B, D], target [B, 2D], history [B, L, 2D] zero-padded at the tail, mask [B, L]).
         ``gru=None`` runs both layers through ``nn.GRU``; otherwise ``gru(x, module, lengths)`` (:func:`nn.fused_gru`, what
-        :func:`models.rec_engine.din_engine` passes) runs each layer only over the first ``lengths = max(mask.sum(1), 1)`` steps of a sample."""
+        :func:`models.rec_engine.din_engine` passes) runs each layer only over the first ``lengths = max(mask.sum(1), 1)`` steps of a sample.
+        ``attention=None`` computes the attention weights inline; otherwise ``attention(qh, h1, mask, self.att, weights=True)``
+        (:func:`nn.fused_din_attention`, what the engine passes) with ``qh = self.qproj(q)``."""
         lens = mask.sum(1).clamp_min(1)
         run = (lambda x, m: m(x)[0]) if gru is None else (lambda x, m: gru(x, m, lens))
         # Both paths give the same logits.  A GRU is causal, so h1 and h2 agree on the first lens steps, the only steps the masked softmax
         # weighs and ``final`` reads.  An empty history (mask all False) counts as length 1: the all-masked softmax gives every position
         # 1 / L, and final = h2[0] depends on step 0 alone, which the length-1 run computes too.
         h1 = run(k, self.gru1)
-        qh = self.qproj(q).unsqueeze(1).expand_as(h1)
-        s = self.att(torch.cat([qh, h1, qh - h1, qh * h1], -1)).squeeze(-1).masked_fill(~mask, -2 ** 31)
-        w = torch.softmax(s, -1).unsqueeze(-1)
+        if attention is None:
+            qh = self.qproj(q).unsqueeze(1).expand_as(h1)
+            s = self.att(torch.cat([qh, h1, qh - h1, qh * h1], -1)).squeeze(-1).masked_fill(~mask, -2 ** 31)
+            w = torch.softmax(s, -1).unsqueeze(-1)
+        else:
+            w = attention(self.qproj(q), h1, mask, self.att, weights=True).unsqueeze(-1)
         h2 = run(h1 * w, self.gru2)
         final = h2[torch.arange(h2.shape[0], device=h2.device), lens - 1]
         return self.top(torch.cat([u, q, final, k.sum(1)], -1)).squeeze(-1)

@@ -11,6 +11,8 @@
     forward and backward through time on csrc/cuda/rnn_kernels.cu.
   * ``fused_encoder_layer``: a post-norm Transformer encoder layer with a key-padding mask for training -- in_proj, out_proj and the FFN on
     the wgmma GEMM, the multi-head self-attention core forward and backward on csrc/cuda/mha_kernels.cu.
+  * ``fused_din_attention``: DIN's attention unit (the weighted sum of the history, or DIEN's softmax weights) for training, forward and backward
+    on csrc/cuda/din_att_kernels.cu.
   * ``FusedMaskBlock``: MaskNet's MaskBlock as one autograd node -- the mask MLP's GEMMs with their BatchNorm statistics in the epilogue,
     the last BatchNorm fused with the instance-guided product, and the block's Linear with LayerNorm + ReLU in the GEMM epilogue.
   * ``fused_expert_mlps`` / ``fused_moe_mix`` (``FUSED_MOE``): MMoE's and PLE's same-shaped expert and tower MLPs as grouped wgmma GEMMs, and a
@@ -399,6 +401,91 @@ def fused_encoder_layer(x: torch.Tensor, layer: nn.TransformerEncoderLayer, vali
     h = layer.norm1(x2 + a.to(x.dtype))
     f = _FusedMLPFn.apply(h.to(torch.bfloat16), False, layer.linear1.weight, layer.linear1.bias, layer.linear2.weight, layer.linear2.bias)
     return layer.norm2(h + f.to(h.dtype)).reshape(B, S, E)
+
+
+# ---- DIN attention unit ------------------------------------------------------------------------------------------------------
+DIN_ATT_DIMS = (16, 32, 48, 64)       # widths of q and k csrc/cuda/din_att_kernels.cu is compiled for
+DIN_ATT_MAX_H1, DIN_ATT_MAX_H2, DIN_ATT_MAX_LEN = 128, 64, 128
+
+
+class _DinAttentionFn(torch.autograd.Function):
+    """q [B, D], k [B, L, D], mask [B, L] and the unit's parameters -> out fp32 [B, D] (mode 0) or w fp32 [B, L] (mode 1) on
+    csrc/cuda/din_att_kernels.cu.  The backward recomputes the unit from q, k and the mask; b3 gets an exact 0 gradient."""
+
+    @staticmethod
+    def forward(ctx, q, k, mask, mode: int, W1, b1, W2, b2, W3, b3):
+        B, L, D = k.shape
+        qf = q.detach().float().contiguous()
+        kd = k.detach()
+        if kd.dtype not in (torch.bfloat16, torch.float32):
+            kd = kd.float()
+        kd = kd.contiguous()
+        mk = mask.to(device=q.device, dtype=torch.bool).contiguous()
+        ws = [t.detach().float().contiguous() for t in (W1, b1, W2, b2, W3.reshape(-1))]
+        out = torch.empty((B, D) if mode == 0 else (B, L), dtype=torch.float32, device=q.device)
+        check(_native.cuda().dr_cuda_din_att_fwd(ptr(qf), ptr(kd), int(kd.dtype == torch.bfloat16), ptr(mk), B, L, D, ptr(ws[0]), ptr(ws[1]),
+                                                 W1.shape[0], ptr(ws[2]), ptr(ws[3]), W2.shape[0], ptr(ws[4]), mode, ptr(out), stream_ptr()),
+              "din_att_fwd")
+        ctx.save_for_backward(qf, kd, mk, *ws)
+        ctx.mode, ctx.dtypes, ctx.w3_shape = mode, (q.dtype, k.dtype, b3.dtype), W3.shape
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        qf, kd, mk, W1, b1, W2, b2, w3 = ctx.saved_tensors
+        B, L, D = kd.shape
+        H1, H2 = W1.shape[0], W2.shape[0]
+        dev = qf.device
+        gf = g.detach().float().contiguous()
+        dq, dk = torch.empty_like(qf), torch.empty_like(kd)
+        dW1, db1, dW2, db2 = torch.empty_like(W1), torch.empty_like(b1), torch.empty_like(W2), torch.empty_like(b2)
+        dw3, db3 = torch.empty_like(w3), torch.empty(1, dtype=torch.float32, device=dev)
+        scratch = torch.empty(B * L * (2 * D + 2 * H1 + H2), dtype=torch.bfloat16, device=dev)
+        check(_native.cuda().dr_cuda_din_att_bwd(ptr(qf), ptr(kd), int(kd.dtype == torch.bfloat16), ptr(mk), ptr(gf), B, L, D, ptr(W1), ptr(b1), H1,
+                                                 ptr(W2), ptr(b2), H2, ptr(w3), ctx.mode, ptr(dq), ptr(dk), ptr(dW1), ptr(db1), ptr(dW2), ptr(db2),
+                                                 ptr(dw3), ptr(db3), ptr(scratch), stream_ptr()), "din_att_bwd")
+        tq, tk, tb3 = ctx.dtypes
+        return (dq.to(tq), dk.to(tk), None, None, dW1, db1, dW2, db2, dw3.view(ctx.w3_shape), db3.to(tb3))
+
+
+def _check_din_unit(q: torch.Tensor, k: torch.Tensor, att: nn.Module) -> None:
+    from ..ops.attention import _fusable
+    if not _fusable(att):
+        raise ValueError("fused_din_attention: needs the Linear-Sigmoid-Linear-Sigmoid-Linear(1) unit with biases")
+    D = q.shape[-1]
+    if k.dim() != 3 or k.shape[-1] != D or att[0].in_features != 4 * D or att[2].in_features != att[0].out_features \
+            or att[4].in_features != att[2].out_features:
+        raise ValueError(f"fused_din_attention: q [B, D], k [B, L, D] and a unit over 4 D = {4 * D} inputs are needed "
+                         f"(got q {tuple(q.shape)}, k {tuple(k.shape)}, first layer in_features {att[0].in_features})")
+
+
+def fused_din_attention(q: torch.Tensor, k: torch.Tensor, mask: torch.Tensor, att: nn.Module, weights: bool = False) -> torch.Tensor:
+    """DIN's attention unit over the behaviour history: scores ``att(cat[q, k_t, q - k_t, q * k_t])`` for ``q`` [B, D], ``k`` [B, L, D], a
+    masked softmax over the positions with ``mask`` (bool [B, L], True = valid), then the weighted sum of the keys [B, D] (``weights=False``,
+    DIN; 0 for a sample with no valid position) or the softmax weights fp32 [B, L] (``weights=True``, DIEN; 1 / L everywhere for a sample
+    with no valid position).  ``att`` is the Linear-Sigmoid-Linear-Sigmoid-Linear(1) unit; the op trains its own parameters, so state dicts
+    and exports do not change.
+
+    CUDA: one autograd node on csrc/cuda/din_att_kernels.cu (mma.sync with bf16 operands, fp32 softmax and gradients, no floating-point atomics,
+    no host synchronisation, so it can be captured in a CUDA graph).  No gradient reaches a masked position or a sample with no valid position.
+    D must be one of ``DIN_ATT_DIMS``, the hidden widths multiples of 16 (<= 128) and 8 (<= 64), L at most ``DIN_ATT_MAX_LEN``.  Elsewhere (CPU,
+    the kernel emulation, ``DEEPREC_FUSED_NN=0``): the torch expressions ``ops.attention.din_attention`` (sum) and DIEN's inline softmax."""
+    _check_din_unit(q, k, att)
+    if not (_fused_nn(q) and q.is_cuda):
+        if not weights:
+            from ..ops.attention import din_attention
+            return din_attention(q, k, mask, att)
+        qe = q.unsqueeze(1).expand_as(k)
+        s = att(torch.cat([qe, k, qe - k, qe * k], -1)).squeeze(-1).masked_fill(~mask, -2 ** 31)
+        return torch.softmax(s, -1)
+    B, L, D = k.shape
+    H1, H2 = att[0].out_features, att[2].out_features
+    if D not in DIN_ATT_DIMS or H1 % 16 or H1 > DIN_ATT_MAX_H1 or H2 % 8 or H2 > DIN_ATT_MAX_H2 or not 1 <= L <= DIN_ATT_MAX_LEN or B < 1:
+        raise ValueError(f"fused_din_attention: D = {D}, H1 = {H1}, H2 = {H2}, L = {L} are not supported on CUDA (D one of {DIN_ATT_DIMS}, "
+                         f"H1 a multiple of 16 up to {DIN_ATT_MAX_H1}, H2 a multiple of 8 up to {DIN_ATT_MAX_H2}, 1 <= L <= {DIN_ATT_MAX_LEN})")
+    l1, l2, l3 = att[0], att[2], att[4]
+    out = _DinAttentionFn.apply(q, k, mask, 1 if weights else 0, l1.weight, l1.bias, l2.weight, l2.bias, l3.weight, l3.bias)
+    return out if weights else out.to(q.dtype)
 
 
 # ---- MaskNet MaskBlock -------------------------------------------------------------------------------------------------------
