@@ -7,11 +7,11 @@
 //                  issue wgmma.mma_async straight from the 128B-swizzled K-major smem tiles and run the fused epilogue from their
 //                  accumulator registers.  A 4-stage smem ring of mbarrier-guarded stages keeps the loads of the next tile in flight
 //                  while the consumers finish the current one.
-//                  bf16 streaming at K < 512 (the default there): ping-pong consumers.  Each warpgroup owns whole 128-row tiles, alternate tiles of
+//                  bf16 streaming (the default): ping-pong consumers.  Each warpgroup owns whole 128-row tiles, alternate tiles of
 //                  the schedule, so one warpgroup's epilogue overlaps the other's MMAs; the aux tile arrives by TMA into the
-//                  warpgroup's output buffer and the bf16 tile leaves by TMA store.  FP8 / MX, BRES, CL2 and bf16 at K >= 512:
-//                  cooperative consumers,
-//                  each warpgroup owns 64 rows of every tile and stores straight from registers.
+//                  warpgroup's output buffer and the bf16 tile leaves by TMA store.  FP8 / MX, BRES, CL2, the cross / residual /
+//                  LayerNorm epilogues and unaligned aux operands: cooperative consumers, each warpgroup owns 64 rows of every tile
+//                  and stores straight from registers.
 //                  Variants: BRES (B-resident: a CTA keeps one [BLOCK_N, K] weight slab in smem for its whole life and streams only
 //                  A) and CL2 (thread-block cluster of 2 CTAs on vertically adjacent tiles: each CTA loads half of the B tile and
 //                  multicasts it to both, halving the B traffic from L2).
@@ -325,59 +325,89 @@ k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         if (t == 0) tma_store_wait_read();
         wg_bar_sync(wg);
       }
-      // ---- epilogue: the arithmetic and the statistics' summation order of the cooperative epilogue below, row group g = 4 half + wl
+      // ---- epilogue: the arithmetic and the statistics' summation order of the cooperative epilogue below, row group g = 4 half + wl.
+      // It runs on 4 warps, one per SM sub-partition, so its time is latency, not issue: the aux mode, the statistics and whether the
+      // tile lies wholly inside M x N are template arguments, so the element loop does not branch or reconverge on any of them.
+      // The statistics use the shuffle tree of the cooperative epilogue (row lanes paired by xor 1, 2, 4 of lane / 4), but a pair of
+      // lanes exchanges only the half of its column partials that the other lane keeps: 4 shuffles per 8 columns instead of 12, and
+      // each add sees the same two operands, so the same bits.
+      auto epilogue = [&](auto full_c, auto auxm_c, auto stats_c) {
+        constexpr bool kFull = decltype(full_c)::value;
+        constexpr int kAuxM = decltype(auxm_c)::value;  // 0: no aux element read   1: ReLU-backward mask   2: S2 partner
+        constexpr bool kStats = decltype(stats_c)::value;
+        const uint32_t obuf_s = smem_u32(obuf);
+        const bool relu = ep.relu != 0;
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        const int lrow0 = half * 64 + wl * 16 + (lane >> 2);
-        const int row0 = m_blk * BLOCK_M + lrow0;
+        for (int half = 0; half < 2; ++half) {
+          const int lrow0 = half * 64 + wl * 16 + (lane >> 2);
+          const int row0 = m_blk * BLOCK_M + lrow0;
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          const int lcol = 8 * j + 2 * (lane & 3);
-          const int col = n_blk * BLOCK_N + lcol;
-          const bool col_ok = col < N;
-          float b0 = 0.f, b1 = 0.f;
-          if (col_ok && ep.bias) { b0 = __ldg(ep.bias + col); b1 = __ldg(ep.bias + col + 1); }
-          float p1[2] = {0.f, 0.f}, p2[2] = {0.f, 0.f};
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int lcol = 8 * j + 2 * (lane & 3);
+            const int col = n_blk * BLOCK_N + lcol;
+            const bool col_ok = kFull || col < N;
+            float b0 = 0.f, b1 = 0.f;
+            if (col_ok && ep.bias) { b0 = __ldg(ep.bias + col); b1 = __ldg(ep.bias + col + 1); }
+            float p1[2] = {0.f, 0.f}, p2[2] = {0.f, 0.f};
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = row0 + 8 * h;
-            const bool ok = col_ok && row < M;
-            float v0 = acc[half][4 * j + 2 * h] + b0;
-            float v1 = acc[half][4 * j + 2 * h + 1] + b1;
-            if (ep.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            uint32_t* sp = reinterpret_cast<uint32_t*>(obuf + out_tile_offset<BLOCK_N>(lrow0 + 8 * h, lcol));
-            float w0 = 0.f, w1 = 0.f;
-            if (has_aux && ok) {
-              const float2 w = unpack_bf16x2(*sp);
-              w0 = w.x; w1 = w.y;
-              if (ep.aux_mode == 1) { if (!(w0 > 0.f)) v0 = 0.f; if (!(w1 > 0.f)) v1 = 0.f; }
-            }
-            *sp = pack_bf16x2(v0, v1);                  // rows >= M and columns >= N are clipped by the store's tensor map
-            if (ok) {
-              if (ep.out_f32) *reinterpret_cast<float2*>(ep.out_f32 + (int64_t)row * ep.ldc + col) = make_float2(v0, v1);
-              if (stats) {
-                p1[0] += v0; p1[1] += v1;
-                const float a0 = ep.aux_mode == 2 ? w0 : v0, a1 = ep.aux_mode == 2 ? w1 : v1;
-                p2[0] += v0 * a0; p2[1] += v1 * a1;
+            for (int h = 0; h < 2; ++h) {
+              const int row = row0 + 8 * h;
+              const bool ok = kFull || (col_ok && row < M);
+              float v0 = acc[half][4 * j + 2 * h] + b0;
+              float v1 = acc[half][4 * j + 2 * h + 1] + b1;
+              v0 = relu ? fmaxf(v0, 0.f) : v0;
+              v1 = relu ? fmaxf(v1, 0.f) : v1;
+              const uint32_t sp = obuf_s + out_tile_offset<BLOCK_N>(lrow0 + 8 * h, lcol);
+              float w0 = 0.f, w1 = 0.f;
+              if (kAuxM != 0 && ok) {
+                uint32_t raw;
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(raw) : "r"(sp));
+                const float2 w = unpack_bf16x2(raw);
+                w0 = w.x; w1 = w.y;
+                if (kAuxM == 1) { v0 = w0 > 0.f ? v0 : 0.f; v1 = w1 > 0.f ? v1 : 0.f; }
+              }
+              // rows >= M and columns >= N are clipped by the store's tensor map
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(sp), "r"(pack_bf16x2(v0, v1)));
+              if (ok) {
+                if (ep.out_f32) *reinterpret_cast<float2*>(ep.out_f32 + (int64_t)row * ep.ldc + col) = make_float2(v0, v1);
+                if (kStats) {
+                  p1[0] += v0; p1[1] += v1;
+                  const float a0 = kAuxM == 2 ? w0 : v0, a1 = kAuxM == 2 ? w1 : v1;
+                  p2[0] += v0 * a0; p2[1] += v1 * a1;
+                }
               }
             }
-          }
-          if (stats) {
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-#pragma unroll
-              for (int o = 4; o < 32; o <<= 1) {
-                p1[c] += __shfl_xor_sync(0xffffffffu, p1[c], o);
-                p2[c] += __shfl_xor_sync(0xffffffffu, p2[c], o);
-              }
-            }
-            if (lane < 4) {
-              float* r1 = wS1 + (4 * half + wl) * BLOCK_N + 8 * j + 2 * lane;
-              float* r2 = wS2 + (4 * half + wl) * BLOCK_N + 8 * j + 2 * lane;
-              r1[0] = p1[0]; r1[1] = p1[1]; r2[0] = p2[0]; r2[1] = p2[1];
+            if (kStats) {
+              // partial k = 2 s + c (s: S1 / S2, c: column 2 (lane & 3) + c).  Row bit 0 (lane xor 4): keep partials 2 b, 2 b + 1;
+              // row bit 1 (xor 8): keep 2 b + c; row bit 2 (xor 16): both lanes keep it.  Lanes 0-15 then hold the group's sums.
+              const bool b = (lane >> 2) & 1, c = (lane >> 3) & 1;
+              const float s0 = b ? p1[0] : p2[0], s1 = b ? p1[1] : p2[1];
+              float y0 = b ? p2[0] : p1[0], y1 = b ? p2[1] : p1[1];
+              const float r0 = __shfl_xor_sync(0xffffffffu, s0, 4), r1 = __shfl_xor_sync(0xffffffffu, s1, 4);
+              y0 += r0; y1 += r1;
+              float z = c ? y1 : y0;
+              z += __shfl_xor_sync(0xffffffffu, c ? y0 : y1, 8);
+              z += __shfl_xor_sync(0xffffffffu, z, 16);
+              if (lane < 16) (b ? wS2 : wS1)[(4 * half + wl) * BLOCK_N + lcol + (c ? 1 : 0)] = z;
             }
           }
         }
+      };
+      {
+        using F = std::false_type;
+        using T = std::true_type;
+        using A0 = std::integral_constant<int, 0>;
+        using A1 = std::integral_constant<int, 1>;
+        using A2 = std::integral_constant<int, 2>;
+        const bool full = (m_blk + 1) * BLOCK_M <= M && (n_blk + 1) * BLOCK_N <= N;
+        const int auxm = !has_aux ? 0 : ep.aux_mode == 1 ? 1 : ep.aux_mode == 2 ? 2 : 0;
+        auto by_aux = [&](auto full_c, auto stats_c) {
+          if (auxm == 1) epilogue(full_c, A1{}, stats_c);
+          else if (auxm == 2) epilogue(full_c, A2{}, stats_c);
+          else epilogue(full_c, A0{}, stats_c);
+        };
+        if (full) { if (stats) by_aux(T{}, T{}); else by_aux(T{}, F{}); }
+        else { if (stats) by_aux(F{}, T{}); else by_aux(F{}, F{}); }
       }
       fence_proxy_async();                              // the generic-proxy tile writes are visible to the TMA store
       wg_bar_sync(wg);
@@ -815,10 +845,9 @@ int launch_tn_sel(const CUtensorMap& ta, const void* B, int M, int N, int K, int
   if (gemm_bres_enabled() && (K + BLOCK_K - 1) / BLOCK_K <= kMaxKbRes && (N + BN - 1) / BN <= max_ctas)
     return launch_tn<BN, true, false, false>(ta, B, M, N, K, ldb, ep, max_ctas, s);
   // the ping-pong kernel reads the aux tile by TMA, which needs a 16-byte aligned base and pitch; the contract does not ask that of
-  // mask_src / ld_mask, so any other aux operand runs the cooperative kernel (same results bit for bit).  At K >= 512 the mainloop
-  // outweighs the epilogue and the cooperative kernel was the faster one on an H100 (the three K = 512 calls of the DLRM step, 5-12 %)
+  // mask_src / ld_mask, so any other aux operand runs the cooperative kernel (same results bit for bit)
   const bool aux_tma = !ep.mask_src || ((((uintptr_t)ep.mask_src) & 15) == 0 && ep.ld_mask % 8 == 0 && ep.ld_mask >= N);
-  if (aux_tma && K < 512) return launch_tn<BN, false, false, false, false, true>(ta, B, M, N, K, ldb, ep, max_ctas, s);
+  if (aux_tma) return launch_tn<BN, false, false, false, false, true>(ta, B, M, N, K, ldb, ep, max_ctas, s);
   return launch_tn<BN, false, false, false>(ta, B, M, N, K, ldb, ep, max_ctas, s);
 }
 
